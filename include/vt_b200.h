@@ -1,5 +1,5 @@
 /*
- * vt_b200.h — C ABI of the B200 (sm_100a) video-transformer hot-path kernels.
+ * vt_b200.h — C ABI of the H100 (sm_90a) video-transformer hot-path kernels.
  *
  * Drop-in boundary (SURVEY.md §8b): the reference has no FFI layer of its own — its hot path is the
  * forward/backward of the nn.Modules in transformer.py / video_transformer.py, executed by stock
@@ -32,14 +32,14 @@ int vt_version(void);
 int vt_last_error(char* buf, size_t buf_bytes);
 /* number of SMs of the current device (grid sizing is done inside the library) */
 int vt_sm_count(void);
-/* leave n SMs free of the persistent GEMM CTAs (each pins an SM's whole shared memory) so that NCCL's all-reduce
- * kernels, issued on a side stream while backward is still running, can be scheduled; 0 restores the default */
+/* plan GEMM tile counts (wave quantisation, split-K) for vt_sm_count() - n SMs; 0 restores the default.  The GEMM runs one
+ * CTA per tile, not persistent CTAs, so this does not keep SMs free for concurrent kernels (NCCL) */
 int vt_set_reserved_sms(int n);
 /* number of kernels this library has launched in this process (mod 2^31); bench.py's gpu_launches */
 int vt_launch_count(void);
 
 /* ---------------------------------------------------------------------------------------------
- * GEMM on tcgen05 tensor cores:  acc[M,N] = sum_k A[m,k] * B[n,k]   (bf16 x bf16 -> fp32 in TMEM)
+ * GEMM on Hopper tensor cores (wgmma):  acc[M,N] = sum_k A[m,k] * B[n,k]   (bf16 x bf16 -> fp32 in registers)
  * Operands are fed by TMA into 128B-swizzled shared memory.
  *   a_mn_major = 0 : A stored row-major [M, K] (leading dim lda)      "K-major"
  *   a_mn_major = 1 : A stored row-major [K, M] (leading dim lda)      "MN-major" (no transpose copy)
@@ -49,7 +49,7 @@ int vt_launch_count(void);
  *   :267 (temporal_fc), :501-505 (FFN), the Conv2d/Conv3d patch projection :116-126 after im2col,
  *   and autograd's dgrad / wgrad GEMMs of the same layers.
  *
- * Epilogues (thread = accumulator row, fused in the TMEM->register drain):
+ * Epilogues (fused, applied to the accumulator registers):
  *   VT_EPI_BF16  : out_bf16[orow(m), n]  = s(m) * (acc + bias[n])
  *   VT_EPI_F32   : out_f32 [orow(m), n]  = s(m) * (acc + bias[n]) + (aux ? aux_f32[arow(m), n] : 0)
  *                  (residual add / pos+time-embed add / fp32 gradients)
@@ -83,27 +83,23 @@ typedef struct {
   int64_t workspace_bytes;
   int32_t force_splits;    /* 0 = heuristic, >0 = exactly this many K splits (tests) */
   int32_t force_bn;        /* 0 = heuristic, 128 / 192 / 256 (tests) */
-  int32_t force_cluster;   /* 0/1 = single CTAs, 2 = clusters of 2 CTAs along M sharing each B tile by TMA multicast,
-                              3 = CTA pairs issuing tcgen05.mma.cta_group::2 (256 x BN tiles, half of B per SM) */
-  void* debug;             /* diagnostics only: int64 [grid][16] clock64 stamps of the kernel's phases, or NULL */
+  int32_t force_cluster;   /* accepted for ABI compatibility; every tile runs on one CTA */
+  void* debug;             /* unused, NULL */
   /* Affine description of out_row / aux_row for VT_EPI_F32 with aux (the residual scatter of the divided space-time blocks),
    * map_period = 0: none.  GEMM row m -> outer = m / map_period, inner = m % map_period.  Rows with inner < map_skip are
    * "special" (the per-frame cls replicas of the spatial pass): no addend, written to out + map_special_base +
    * outer * map_special_stride (dropped when map_special_base < 0).  Every other row reads its addend from / writes its
    * result to element offset  map_base + (outer % map_tcount) * map_stride_t + (inner - map_skip) * map_stride_p +
-   * (outer / map_tcount) * map_stride_b  of aux / out.  With it the epilogue moves whole 32 x 32 boxes by TMA through a
-   * tensor map (col, row in sample, sample) of the token stream (reference einops: transformer.py:250, :279-280, :352-356,
-   * :375-377) instead of per-thread rows; the out_row / aux_row arrays, when also given, must describe the same mapping
-   * (they serve the generic epilogue, which also covers map_tcount > 1: the element-strided boxes that case needs fault
-   * on hardware and stay switched off). */
+   * (outer / map_tcount) * map_stride_b  of aux / out: the einops regroupings of the token stream (reference
+   * transformer.py:250, :279-280, :352-356, :375-377) computed in the epilogue instead of read from index arrays; the
+   * out_row / aux_row arrays, when also given, must describe the same mapping. */
   int32_t map_period, map_skip, map_tcount;
-  int32_t force_tail;      /* 0 = heuristic, 1 = never cut the partial last row of tiles into narrow units, 2 = prefer to */
+  int32_t force_tail;      /* accepted for ABI compatibility; non-zero only disables the remainder-row split (vt_gemm_rows) */
   int64_t map_stride_t, map_stride_p, map_stride_b, map_base;
   int64_t map_special_base, map_special_stride;
   const float* bias2;      /* VT_EPI_F32 with aux only: out = s(m) * (acc + bias[n]) + bias2[n] + aux — the bias of a second
                               linear layer folded into this GEMM (temporal_fc after proj, transformer.py:264-267) */
-  int32_t out_zeroed;      /* split-K accumulates into `out` by TMA reduce-add and normally zeroes it first; 1 = the caller
-                              already did (a gradient arena / DDP bucket zeroed once per step) */
+  int32_t out_zeroed;      /* accepted for ABI compatibility: split-K partials are summed from `workspace` into `out` */
 } vt_gemm_params;
 
 int vt_gemm(const vt_gemm_params* p, void* stream);
@@ -203,16 +199,16 @@ int vt_gelu_bwd_colsum_bf16(const vt_gelu_bwd_colsum_params* p, void* stream);
  *   qkv bf16 [Bp, N, 3, H, hd] (the layout produced by transformer.py:167's reshape), hd = 64
  *   ctx bf16 [Bp, N, H*hd] = softmax(q k^T * scale) v      (transformer.py:170-174)
  *   lse fp32 [Bp, H, N]   (saved for backward);  probs fp32 [Bp,H,N,N] optional (Attention returns it, :177)
- * Three kernels behind one entry point: a tcgen05/TMEM flash kernel for the spatial pass (N = 197: S, dP and the
- * gradient accumulators in TMEM, K/V resident in shared memory, P/dS re-read transposed through MN-major UMMA
- * descriptors), a warp-per-problem kernel for the temporal pass (N = 8, 18 816 problems/layer), and a generic
- * warp-per-query kernel for any other N <= 256 (ViViT N = 9, tests, probs output).
+ * Three kernels behind one entry point: a tensor-core flash kernel for the spatial pass (N = 197; mma.sync bf16 with
+ * fp32 accumulators, K/V tiles in shared memory, vt_attention_mma.cu), a warp-per-problem kernel for the temporal pass
+ * (N = 8, 18 816 problems/layer), and a generic warp-per-query kernel for any other N <= 256 (ViViT N = 9, probs output).
+ * VT_ATTN_TCGEN05 selects the tensor-core kernel (the name is kept for ABI compatibility).
  * ------------------------------------------------------------------------------------------- */
 enum { VT_ATTN_AUTO = 0, VT_ATTN_GENERIC = 1, VT_ATTN_TCGEN05 = 2, VT_ATTN_WARP8 = 3 };
 typedef struct {
   const void* qkv; void* ctx; float* lse; float* probs;
   int32_t Bp, N, H, hd; float scale;
-  int32_t impl;   /* VT_ATTN_AUTO picks: N == 8 -> warp-per-problem kernel; 32 < N <= 256 -> tcgen05 flash kernel; else generic */
+  int32_t impl;   /* VT_ATTN_AUTO picks: N == 8 -> warp-per-problem kernel; 32 < N <= 256 -> tensor-core kernel; else generic */
 } vt_attn_fwd_params;
 int vt_attn_fwd(const vt_attn_fwd_params* p, void* stream);
 typedef struct {
@@ -221,8 +217,6 @@ typedef struct {
   int32_t impl;
 } vt_attn_bwd_params;
 int vt_attn_bwd(const vt_attn_bwd_params* p, void* stream);
-/* diagnostics only: int64 [grid][32] clock64 phase stamps of the tcgen05 attention kernels (NULL disables) */
-int vt_debug_buffer(void* device_ptr);
 
 /* ---------------------------------------------------------------------------------------------
  * Patch / tubelet embedding operand: non-overlapping Conv2d k16 s16 (transformer.py:116-120,:145-147)
@@ -287,19 +281,19 @@ int vt_pool_bwd(const vt_pool_bwd_params* p, void* stream);
 /* Softmax attention with separate, strided Q / K / V and Nq != Nk (pooling attention):
  *   element (b, h, n, c) of q at q[b*q_bs + h*q_hs + n*q_rs + c] (bf16), same for k, v, o (and dout, dq).
  *   o = softmax(scale * q k^T) v ;  lse fp32 [B,H,Nq] = log sum exp(scale * q k^T).
- * Two implementations: tcgen05 flash kernels (vt_xattention_tc.cu: head dim 96 staged as 128 padded columns = two
- * 128-byte swizzle atoms, S / dP / accumulators in TMEM, K/V streamed by TMA) and CUDA-core kernels for arbitrary
- * strides (two threads per query row, K/V tiles staged in shared memory). */
+ * Two implementations, head dim 64 or 96: tensor-core flash kernels (vt_attention_mma.cu, VT_XATTN_TCGEN05 — the name is
+ * kept for ABI compatibility) and CUDA-core kernels for arbitrary strides (two threads per query row, K/V tiles staged in
+ * shared memory). */
 enum { VT_XATTN_AUTO = 0, VT_XATTN_SIMT = 1, VT_XATTN_TCGEN05 = 2 };
 typedef struct {
   const void* q; const void* k; const void* v; void* o; float* lse;
   int64_t q_bs, q_hs, q_rs, k_bs, k_hs, k_rs, v_bs, v_hs, v_rs, o_bs, o_hs, o_rs;
   int32_t B, H, Nq, Nk, hd; float scale;
-  int32_t impl;   /* VT_XATTN_AUTO: tcgen05 kernels when every operand is token-major ([B,N,H*hd] slices) or head-major
+  int32_t impl;   /* VT_XATTN_AUTO: tensor-core kernels when every operand is token-major ([B,N,H*hd] slices) or head-major
                      contiguous ([B,H,N,hd]) with 16-byte aligned rows, else the CUDA-core kernels */
 } vt_xattn_fwd_params;
 int vt_xattn_fwd(const vt_xattn_fwd_params* p, void* stream);
-/* dq: bf16 with its own strides.  dk, dv: fp32 [B,H,Nk,hd] contiguous (zeroed by the call, accumulated with atomics).
+/* dq: bf16 with its own strides.  dk, dv: fp32 [B,H,Nk,hd] contiguous (every element written by the call).
  * delta: fp32 scratch [B,H,Nq]. */
 typedef struct {
   const void* q; const void* k; const void* v; const void* o; const void* dout; const float* lse;

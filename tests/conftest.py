@@ -11,8 +11,29 @@ if ROOT not in sys.path:
 GOLD = os.path.join(ROOT, 'tests', 'golden')
 
 
+class GoldenArrays(dict):
+    """Arrays of one fixture: `<name>.npz` plus its continuation files `<name>.1.npz`, `<name>.2.npz`, ... (fixtures are
+    split so that no file exceeds 1 MB)."""
+
+    @property
+    def files(self):
+        return list(self)
+
+
+def load_golden(name):
+    z, i, path = GoldenArrays(), 0, os.path.join(GOLD, name + '.npz')
+    while os.path.exists(path):
+        with np.load(path) as part:
+            z.update({k: part[k] for k in part.files})
+        i += 1
+        path = os.path.join(GOLD, f'{name}.{i}.npz')
+    if not z:
+        raise FileNotFoundError(os.path.join(GOLD, name + '.npz'))
+    return z
+
+
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box: pytest -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100: pytest -m gpu)')
     config.addinivalue_line('markers', 'experimental: kernel paths that ship disabled until confirmed on hardware '
                                        '(run with VT_EXPERIMENTAL=1; the test switches the path on itself)')
 
@@ -35,7 +56,7 @@ class Golden:
     """One reference-generated fixture (oracle/make_golden.py)."""
 
     def __init__(self, name):
-        z = np.load(os.path.join(GOLD, name + '.npz'))
+        z = load_golden(name)
         self.raw = z
         self.x = torch.from_numpy(z['x'])
         self.sd = {k[4:]: torch.from_numpy(z[k]) for k in z.files if k.startswith('sd::')}
@@ -54,7 +75,7 @@ class MaskFeatGolden:
     def __init__(self, name):
         import ast
         from oracle import mvit_oracle as mo
-        z = np.load(os.path.join(GOLD, name + '.npz'))
+        z = load_golden(name)
         self.kwargs = ast.literal_eval(str(z['cfg_kwargs'][0]))
         self.cfg = mo.maskfeat_config(**self.kwargs)
         self.seed, self.B = int(z['seed']), int(z['B'])

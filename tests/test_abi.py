@@ -20,17 +20,17 @@ def test_library_exports_every_declared_symbol():
     assert dll.vt_version() == 1
 
 
-def test_sass_is_blackwell_native():
+def test_sass_is_hopper_native():
     import shutil
     import subprocess
     from videotransformer_pytorch_b200 import build
     if not shutil.which('cuobjdump'):
         return
     sass = subprocess.run(['cuobjdump', '-sass', build.build()], capture_output=True, text=True).stdout
-    assert 'UTCHMMA' in sass        # tcgen05.mma
-    assert 'UTMALDG' in sass        # TMA loads
-    assert 'LDTM' in sass           # tcgen05.ld
-    assert 'HMMA.16816' not in sass  # no legacy mma.sync path
+    assert 'arch = sm_90a' in sass
+    assert 'HGMMA' in sass          # wgmma.mma_async (GEMM)
+    assert 'UTMALDG' in sass        # TMA loads (GEMM)
+    assert 'HMMA.16816.F32.BF16' in sass   # mma.sync (flash attention)
 
 
 def test_missing_library_fails_loudly(monkeypatch):

@@ -1,4 +1,4 @@
-"""Attention core kernels (generic / tcgen05 flash / warp-per-problem) vs torch fp32 on the same bf16 qkv.  -m gpu"""
+"""Attention core kernels (generic / tensor-core flash / warp-per-problem) vs torch fp32 on the same bf16 qkv.  -m gpu"""
 import pytest
 import torch
 
@@ -57,8 +57,8 @@ def test_attn_fwd_bwd(Bp, N, H, impl):
 
 
 def test_attn_kernels_agree_on_adjacent_problems():
-    """The tcgen05 kernel over-reads rows of the next (frame) problem into its padded tiles; results must not
-    depend on what those rows hold."""
+    """The tensor-core kernel stages whole 64-row tiles next to the rows of the next (frame) problem; results must
+    not depend on what those rows hold."""
     Bp, N, H, hd = 3, 197, 2, 64
     torch.manual_seed(0)
     qkv = (torch.randn(Bp, N, 3, H, hd) * 0.7).cuda().bfloat16()

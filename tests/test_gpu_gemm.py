@@ -1,4 +1,8 @@
-"""tcgen05 GEMM (vt_gemm) vs torch fp32 matmul on the same bf16-rounded operands.  -m gpu"""
+"""wgmma GEMM (vt_gemm) vs torch fp32 matmul on the same bf16-rounded operands.  -m gpu
+
+force_cluster, force_tail and the VT_TMA_* / VT_SPLITK_WORKSPACE switches are still accepted by the ABI but select nothing
+on sm_90a (one kernel, register epilogue, split-K through the workspace); the tests that flip them check that both sides
+still match torch."""
 
 import pytest
 import torch

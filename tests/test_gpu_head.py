@@ -5,7 +5,7 @@ import numpy as np
 import pytest
 import torch
 
-from tests.conftest import GOLD, rel_err
+from tests.conftest import load_golden, rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -117,7 +117,7 @@ def test_get_last_selfattention_joint_space_time_1569_tokens():
 
 
 def test_attention_module_long_sequence_forward_backward():
-    """Stand-alone Attention.forward (transformer.py:165-177) past 256 tokens: context from the streaming tcgen05 kernels,
+    """Stand-alone Attention.forward (transformer.py:165-177) past 256 tokens: context from the streaming tensor-core kernels,
     probabilities from the row-tile kernel, gradients through the streaming backward."""
     from videotransformer_pytorch_b200 import Attention
     torch.manual_seed(1)
@@ -141,7 +141,7 @@ def test_attention_module_long_sequence_forward_backward():
 def test_mixup_cutmix_operand_kernel_vs_reference_goldens():
     """vt_im2col_u8_mix_bf16 against clips mixed by the reference's Mixup class (tests/golden/mixup.npz)."""
     from videotransformer_pytorch_b200 import Mixup
-    gold = np.load(os.path.join(GOLD, 'mixup.npz'))
+    gold = load_golden('mixup')
     scale = torch.full((3,), 1.0 / (255.0 * 0.225)).cuda()
     shift = torch.full((3,), -0.45 / 0.225).cuda()
     for seed in gold['seeds']:

@@ -142,7 +142,7 @@ STAGE_BLOCKS = [(0, (8, 56, 56)), (1, (8, 56, 56)), (2, (8, 28, 28)), (3, (8, 28
 
 @pytest.mark.parametrize('index,thw', STAGE_BLOCKS)
 def test_multiscale_block_vs_oracle_at_mvit_b_shapes(index, thw):
-    """One whole MultiScaleBlock (LN, fused q/k/v GEMM, pooling, tcgen05 pooling attention, proj, max-pool skip, MLP, width
+    """One whole MultiScaleBlock (LN, fused q/k/v GEMM, pooling, tensor-core pooling attention, proj, max-pool skip, MLP, width
     change) forward + all gradients against mvit_oracle.multiscale_block at the real token counts."""
     from oracle import mvit_oracle as MO
     from videotransformer_pytorch_b200.maskfeat import MultiScaleBlock

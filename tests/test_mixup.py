@@ -7,12 +7,12 @@ import numpy as np
 import pytest
 import torch
 
-from tests.conftest import GOLD, rel_err
+from tests.conftest import load_golden, rel_err
 
 
 @pytest.fixture(scope='module')
 def gold():
-    return np.load(os.path.join(GOLD, 'mixup.npz'))
+    return load_golden('mixup')
 
 
 def _norm(u8):

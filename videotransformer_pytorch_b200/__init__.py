@@ -1,10 +1,10 @@
-"""B200-native (sm_100a) forward/backward for the video-transformer hot path of
+"""H100-native (sm_90a) forward/backward for the video-transformer hot path of
 mx-mark/VideoTransformer-pytorch, behind the reference's own nn.Module surface.
 
     from videotransformer_pytorch_b200 import TimeSformer, ViViT, MaskFeat
 
 The package is importable without a GPU (module construction, state dicts); any forward needs
-libvt_b200.so (python -m videotransformer_pytorch_b200.build) and a B200 — there is no fallback.
+libvt_b200.so (python -m videotransformer_pytorch_b200.build) and an H100 (sm_90) — there is no fallback.
 """
 from .transformer import (Attention, BasicTransformerBlock, ClassificationHead,  # noqa: F401
                           DividedSpatialAttentionWithPreNorm, DividedTemporalAttentionWithPreNorm, DropPath,

@@ -217,7 +217,7 @@ class Im2colU8MixParams(C.Structure):
 EXPORTS = ['vt_version', 'vt_last_error', 'vt_sm_count', 'vt_set_reserved_sms', 'vt_launch_count', 'vt_gemm', 'vt_layernorm_fwd', 'vt_ln_bwd_blocks',
            'vt_layernorm_bwd', 'vt_reduce_rows', 'vt_colsum_chunks', 'vt_colsum_bf16', 'vt_cast_f32_bf16',
            'vt_cls_rows', 'vt_gather_cast_colsum_blocks', 'vt_gather_cast_colsum_bf16', 'vt_gelu_bwd_colsum_blocks', 'vt_gelu_bwd_colsum_bf16',
-           'vt_gather_cast_bf16', 'vt_gelu_fwd_bf16', 'vt_gelu_bwd_bf16', 'vt_attn_fwd', 'vt_attn_bwd', 'vt_debug_buffer', 'vt_im2col_bf16', 'vt_im2col_u8_bf16', 'vt_col2im_f32', 'vt_hog',
+           'vt_gather_cast_bf16', 'vt_gelu_fwd_bf16', 'vt_gelu_bwd_bf16', 'vt_attn_fwd', 'vt_attn_bwd', 'vt_im2col_bf16', 'vt_im2col_u8_bf16', 'vt_col2im_f32', 'vt_hog',
            'vt_pool_fwd', 'vt_pool_bwd_scratch', 'vt_pool_bwd', 'vt_xattn_fwd', 'vt_xattn_bwd', 'vt_maxpool_fwd',
            'vt_maxpool_bwd', 'vt_im2col3d_bf16', 'vt_mvit_tokens_fwd', 'vt_mvit_tokens_bwd', 'vt_mse_blocks',
            'vt_mse_fwd', 'vt_mse_bwd', 'vt_opt_norm2', 'vt_opt_sgd', 'vt_opt_adamw',
@@ -233,7 +233,7 @@ def load_library() -> C.CDLL:
     if _dll is None:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
-                f'{LIB_PATH} not found: build the sm_100a kernels first '
+                f'{LIB_PATH} not found: build the sm_90a kernels first '
                 f'(python -m videotransformer_pytorch_b200.build, or __graft_entry__.build()). '
                 f'There is no CPU / library fallback for the hot path.')
         _dll = C.CDLL(LIB_PATH)
@@ -1001,7 +1001,7 @@ class CudaKernels:
 
 
 def set_reserved_sms(n: int) -> None:
-    """Keep n SMs free of persistent GEMM CTAs (for overlapped NCCL kernels); see vt_set_reserved_sms."""
+    """Plan GEMM tile counts for vt_sm_count() - n SMs (no SMs are kept free); see vt_set_reserved_sms."""
     _check(load_library().vt_set_reserved_sms(int(n)), 'vt_set_reserved_sms')
 
 

@@ -1,9 +1,9 @@
 // Softmax attention core on packed qkv (bf16 [Bp, N, 3, H, 64]) — generic warp-primitive kernels.
 // One CTA per (batch', head); Q/K/V/dO rows live in shared memory with a 33-word row pitch so that both
 // "lane = key/query index" and "lane = feature pair" access patterns are bank-conflict free.
-// Used for the temporal pass (N = T = 8), ViViT's temporal encoder (N = 9) and as the general-N path;
-// the 197-token spatial pass has its own tcgen05 kernel (vt_attention_tc.cu).
-#include "vt_common.cuh"
+// Used for the temporal pass of ViViT (N = 9), the probability output and as the general-N path; the 197-token spatial
+// pass runs on the tensor-core kernels (vt_attention_mma.cu), N = 8 on the warp-per-problem kernel (vt_attention_small.cu).
+#include "vt_attention_mma.cuh"
 
 namespace vt {
 
@@ -220,8 +220,6 @@ attn_bwd_kernel(const __nv_bfloat16* __restrict__ qkv, const __nv_bfloat16* __re
   }
 }
 
-int attn_tc_fwd_launch(const vt_attn_fwd_params* q, cudaStream_t st);
-int attn_tc_bwd_launch(const vt_attn_bwd_params* q, cudaStream_t st);
 int attn8_fwd_launch(const vt_attn_fwd_params* p, cudaStream_t st);
 int attn8_bwd_launch(const vt_attn_bwd_params* p, cudaStream_t st);
 
@@ -231,6 +229,23 @@ static int pick_impl(int impl, int N, bool probs) {
   if (N == 8) return VT_ATTN_WARP8;
   if (N > 32 && N <= 256) return VT_ATTN_TCGEN05;
   return VT_ATTN_GENERIC;
+}
+
+// packed qkv [Bp, N, 3, H, 64] / ctx [Bp, N, H, 64] as strided q / k / v / o operands of the tensor-core kernels
+static MmaAttn packed_operands(const void* qkv, const void* ctx, const float* lse, int Bp, int N, int H, float scale) {
+  MmaAttn a{};
+  const long long rs = 3LL * H * HD, cs = (long long)H * HD;
+  const __nv_bfloat16* q = static_cast<const __nv_bfloat16*>(qkv);
+  a.q = q; a.k = q + cs; a.v = q + 2 * cs;
+  a.q_bs = a.k_bs = a.v_bs = (long long)N * rs;
+  a.q_hs = a.k_hs = a.v_hs = HD;
+  a.q_rs = a.k_rs = a.v_rs = rs;
+  a.o = static_cast<const __nv_bfloat16*>(ctx);
+  a.o_bs = (long long)N * cs; a.o_hs = HD; a.o_rs = cs;
+  a.lse = const_cast<float*>(lse);
+  a.H = H; a.Nq = N; a.Nk = N; a.scale = scale;
+  (void)Bp;
+  return a;
 }
 
 }  // namespace vt
@@ -244,8 +259,11 @@ extern "C" int vt_attn_fwd(const vt_attn_fwd_params* p, void* stream) {
   VT_REQUIRE(p->Bp > 0 && p->H > 0, "vt_attn_fwd: bad Bp/H");
   const int impl = pick_impl(p->impl, p->N, p->probs != nullptr);
   if (impl == VT_ATTN_TCGEN05) {
-    VT_REQUIRE(p->probs == nullptr && p->N >= 16, "vt_attn_fwd: tcgen05 kernel needs N >= 16 and no probs output");
-    return attn_tc_fwd_launch(p, static_cast<cudaStream_t>(stream));
+    VT_REQUIRE(p->probs == nullptr, "vt_attn_fwd: the tensor-core kernel has no probs output");
+    VT_REQUIRE((((uintptr_t)p->qkv | (uintptr_t)p->ctx) & 15) == 0, "vt_attn_fwd: qkv / ctx must be 16-byte aligned");
+    MmaAttn a = packed_operands(p->qkv, p->ctx, p->lse, p->Bp, p->N, p->H, p->scale);
+    a.o_out = static_cast<__nv_bfloat16*>(p->ctx);
+    return attn_mma_fwd(a, p->Bp, HD, static_cast<cudaStream_t>(stream));
   }
   if (impl == VT_ATTN_WARP8) {
     VT_REQUIRE(p->probs == nullptr && p->N == 8, "vt_attn_fwd: warp8 kernel needs N == 8 and no probs output");
@@ -270,8 +288,17 @@ extern "C" int vt_attn_bwd(const vt_attn_bwd_params* p, void* stream) {
   VT_REQUIRE(p->N >= 1 && p->N <= MAX_N, "vt_attn_bwd: N=%d unsupported (1..%d)", p->N, MAX_N);
   const int impl = pick_impl(p->impl, p->N, false);
   if (impl == VT_ATTN_TCGEN05) {
-    VT_REQUIRE(p->N >= 16, "vt_attn_bwd: tcgen05 kernel needs N >= 16");
-    return attn_tc_bwd_launch(p, static_cast<cudaStream_t>(stream));
+    VT_REQUIRE((((uintptr_t)p->qkv | (uintptr_t)p->ctx | (uintptr_t)p->dctx | (uintptr_t)p->dqkv) & 15) == 0,
+               "vt_attn_bwd: qkv / ctx / dctx / dqkv must be 16-byte aligned");
+    MmaAttn a = packed_operands(p->qkv, p->ctx, p->lse, p->Bp, p->N, p->H, p->scale);
+    a.dout = static_cast<const __nv_bfloat16*>(p->dctx);
+    __nv_bfloat16* d = static_cast<__nv_bfloat16*>(p->dqkv);
+    const long long cs = (long long)p->H * HD;
+    a.dq = d; a.dk16 = d + cs; a.dv16 = d + 2 * cs;
+    a.dq_bs = a.dk_bs = a.dv_bs = a.q_bs;
+    a.dq_hs = a.dk_hs = a.dv_hs = HD;
+    a.dq_rs = a.dk_rs = a.dv_rs = a.q_rs;
+    return attn_mma_bwd(a, p->Bp, HD, static_cast<cudaStream_t>(stream));
   }
   if (impl == VT_ATTN_WARP8) {
     VT_REQUIRE(p->N == 8, "vt_attn_bwd: warp8 kernel needs N == 8");

@@ -28,7 +28,7 @@ bool feature_on(const char* name, bool dflt);
 // narrow-row LayerNorm (D = 32..256 step 32, vt_mvit.cu); vt_layernorm_fwd/bwd dispatch here when D % 128 != 0
 int layernorm_fwd_small(const vt_ln_fwd_params* p, void* stream);
 int layernorm_bwd_small(const vt_ln_bwd_params* p, void* stream);
-int persistent_sm_count();   // sm_count() minus the SMs reserved for concurrent communication kernels
+int persistent_sm_count();   // sm_count() minus vt_set_reserved_sms(): the SM count the GEMM tile planning assumes
 
 // ---- device helpers ---------------------------------------------------------------------------
 __device__ __forceinline__ float warp_sum(float v) {

@@ -1,215 +1,221 @@
-// Persistent warp-specialised bf16 GEMM for sm_100a:
-//   TMA (cp.async.bulk.tensor, 128B swizzle) -> shared-memory ring -> tcgen05.mma (fp32 accum in TMEM,
-//   two accumulator stages) -> tcgen05.ld epilogue fused with bias / GELU / dGELU / residual / row maps.
-// One CTA per SM, 384 threads: warp0 = TMA producer, warp1 = MMA issuer, warp2 = TMEM allocator,
-// warps4-11 = epilogue (warp w drains TMEM lanes 32*(w%4)..+31; the two warpgroups interleave column chunks).
-// Tile: 128 x BN x 64, BN in {128, 256}.  Both operands may be K-major or MN-major (UMMA descriptors),
-// so forward (X W^T), dgrad (dY W) and wgrad (dY^T X) all run without transposed copies.
+// Warp-specialised bf16 GEMM for sm_90a:
+//   TMA (cp.async.bulk.tensor, 128B swizzle) -> shared-memory ring (mbarrier full / empty pairs) -> wgmma.mma_async
+//   (fp32 accumulators in registers) -> epilogue fused with bias / GELU / dGELU / residual / row maps, straight from
+//   the accumulator registers to global memory.
+// One CTA per 128 x BN output tile (x K split), 384 threads: warpgroup 0 = TMA producer (one thread), warpgroups 1-2 =
+// consumers, each owning 64 rows of the tile.  BN in {128, 192, 256}.  Both operands may be K-major or MN-major (wgmma
+// transpose bits), so forward (X W^T), dgrad (dY W) and wgrad (dY^T X) all run without transposed copies.
 #include <stdlib.h>
 #include <string.h>
 
-#include "vt_gemm_common.cuh"
+#include "vt_common.cuh"
+#include "vt_sm90.cuh"
 
 namespace vt {
 
-// RES: instantiation for the fp32 residual epilogue on TMA (epilogue_tile_tma_res): 8 KiB of staging per epilogue warp
-// instead of 4.1 KiB, paid for with one pipeline stage where shared memory is full.
-// compiled defaults of the round-2 paths (environment VT_TMA_RES / VT_TAIL_UNITS / VT_TMA_GELU / VT_TMA_DGELU = 0 | 1 override)
-constexpr bool VT_DEFAULT_TMA_RES = true;
-constexpr bool VT_DEFAULT_TMA_RES_SPATIAL = true;
-constexpr bool VT_DEFAULT_TAIL_UNITS = true;    // MViT step 21.32 -> 21.02 ms (every GEMM there is 8 rows past a tile); neutral elsewhere
-constexpr bool VT_DEFAULT_TMA_GELU = false;
-constexpr bool VT_DEFAULT_TMA_DGELU = false;
-bool tail_units_enabled() { return feature_on("VT_TAIL_UNITS", VT_DEFAULT_TAIL_UNITS); }
+constexpr int BM = 128;
+constexpr int BK = 64;
+constexpr int GEMM_THREADS = 384;        // producer warpgroup + 2 consumer warpgroups
+constexpr int CHUNK_BYTES = 64 * BK * 2;  // one 64-wide MN chunk of an MN-major tile (8 KiB)
 
-template <int BN, bool RES>
+struct GemmDev {
+  int M, N, K;
+  int kblocks, splits;
+  int epi;
+  const float* bias;
+  const float* bias2;      // VT_EPI_F32 with aux only: second bias, added to the addend
+  void* out;
+  void* out2;
+  const void* aux;
+  long long ldo, ldo2, ldaux;
+  const int* out_row;
+  const int* aux_row;
+  const float* row_scale;
+  long long split_stride;  // elements between split partials (EPI_F32 only)
+  // affine row map of the residual epilogue (vt_gemm_params::map_*), map_period = 0: none
+  int map_period, map_skip, map_tcount;
+  long long map_stride_t, map_stride_p, map_stride_b, map_base;
+  float* special_out;      // special rows go to special_out + outer * special_ld, or are dropped
+  long long special_ld;
+};
+
+template <int BN>
 struct GemmCfg {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = RES ? ((BN == 256) ? 3 : (BN == 192 ? 4 : 5)) : ((BN == 256) ? 4 : (BN == 192 ? 4 : 6));
-  static constexpr int TMEM_COLS = (BN == 128) ? 256 : 512;  // two accumulator stages, power of two
-  static constexpr int STAGING_BYTES = RES ? EPI_WARPS * RES_SLOT_BYTES : EPI_WARPS * 32 * EPI_PITCH * 4;
-  static constexpr int BAR_BYTES = 512;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + BAR_BYTES + STAGING_BYTES;
+  static constexpr int STAGES = (BN == 256) ? 4 : (BN == 192 ? 5 : 6);
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
   static_assert(SMEM_BYTES <= 232448, "shared memory budget");
 };
 
-template <int BN, bool RES>
+template <int BN, int TA, int TB>
+__device__ __forceinline__ void wgmma_tile(float (&acc)[BN / 2], uint64_t da, uint64_t db, uint32_t scale_d) {
+  if constexpr (BN == 256) wgmma_m64n256k16<TA, TB>(acc, da, db, scale_d);
+  else if constexpr (BN == 192) wgmma_m64n192k16<TA, TB>(acc, da, db, scale_d);
+  else wgmma_m64n128k16<TA, TB>(acc, da, db, scale_d);
+}
+
+// Where one accumulator row goes: output row pointer (null = dropped), addend row (null = none), second output row.
+struct EpiRow {
+  char* out;
+  const char* aux;
+  char* out2;
+  float s;
+};
+
+__device__ __forceinline__ EpiRow epi_row(const GemmDev& p, int row, int split) {
+  EpiRow r{nullptr, nullptr, nullptr, 1.0f};
+  if (row >= p.M) return r;
+  if (p.row_scale) r.s = p.row_scale[row];
+  if (p.epi == VT_EPI_F32) {
+    float* out = static_cast<float*>(p.out);
+    const float* aux = static_cast<const float*>(p.aux);
+    if (p.map_period > 0) {
+      const int outer = row / p.map_period, inner = row - outer * p.map_period;
+      if (inner < p.map_skip) {
+        if (p.special_out) r.out = reinterpret_cast<char*>(p.special_out + (long long)outer * p.special_ld);
+        return r;
+      }
+      const long long off = p.map_base + (long long)(outer % p.map_tcount) * p.map_stride_t +
+                            (long long)(inner - p.map_skip) * p.map_stride_p + (long long)(outer / p.map_tcount) * p.map_stride_b;
+      r.out = reinterpret_cast<char*>(out + off);
+      r.aux = reinterpret_cast<const char*>(aux + off);
+      return r;
+    }
+    const int orow = p.out_row ? p.out_row[row] : row;
+    if (orow >= 0) r.out = reinterpret_cast<char*>(out + (long long)split * p.split_stride + (long long)orow * p.ldo);
+    if (aux) {
+      const int arow = p.aux_row ? p.aux_row[row] : row;
+      if (arow >= 0) r.aux = reinterpret_cast<const char*>(aux + (long long)arow * p.ldaux);
+    }
+    return r;
+  }
+  const int orow = p.out_row ? p.out_row[row] : row;
+  if (orow < 0) return r;
+  r.out = reinterpret_cast<char*>(static_cast<__nv_bfloat16*>(p.out) + (long long)orow * p.ldo);
+  if (p.epi == VT_EPI_GELU) r.out2 = reinterpret_cast<char*>(static_cast<__nv_bfloat16*>(p.out2) + (long long)orow * p.ldo2);
+  if (p.epi == VT_EPI_DGELU) r.aux = reinterpret_cast<const char*>(static_cast<const __nv_bfloat16*>(p.aux) + (long long)row * p.ldaux);
+  return r;
+}
+
+// columns n, n + 1 of one row (n even, n + 1 < N since N % 8 == 0)
+__device__ __forceinline__ void epi_pair(const GemmDev& p, const EpiRow& r, int n, float v0, float v1) {
+  if (!r.out) return;
+  if (p.bias) {
+    const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+    v0 += b.x; v1 += b.y;
+  }
+  if (p.epi == VT_EPI_BF16) {
+    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(r.out) + n) = pack_bf16x2(r.s * v0, r.s * v1);
+  } else if (p.epi == VT_EPI_F32) {
+    float2 a = make_float2(0.f, 0.f);
+    if (r.aux) a = *reinterpret_cast<const float2*>(reinterpret_cast<const float*>(r.aux) + n);
+    if (p.bias2) {
+      const float2 b2 = __ldg(reinterpret_cast<const float2*>(p.bias2 + n));
+      a.x += b2.x; a.y += b2.y;
+    }
+    *reinterpret_cast<float2*>(reinterpret_cast<float*>(r.out) + n) = make_float2(fmaf(r.s, v0, a.x), fmaf(r.s, v1, a.y));
+  } else if (p.epi == VT_EPI_GELU) {
+    // h from the bf16-rounded z: bit for bit what the stand-alone GELU kernel computes from the stored z
+    const uint32_t z = pack_bf16x2(v0, v1);
+    const float2 zr = unpack_bf16x2(z);
+    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(r.out) + n) = z;
+    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(r.out2) + n) = pack_bf16x2(gelu_fast(zr.x), gelu_fast(zr.y));
+  } else {  // VT_EPI_DGELU
+    const float2 z = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(reinterpret_cast<const __nv_bfloat16*>(r.aux) + n));
+    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(r.out) + n) = pack_bf16x2(v0 * dgelu_fast(z.x), v1 * dgelu_fast(z.y));
+  }
+}
+
+// grid (n tiles, m tiles, K splits); n fastest so that CTAs running together share the A row-block in L2
+template <int BN, int TA, int TB>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                    const __grid_constant__ CUtensorMap tmBt, const __grid_constant__ CUtensorMap tmC,
-                    const __grid_constant__ CUtensorMap tmX, const GemmDev p) {
-  using Cfg = GemmCfg<BN, RES>;
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmDev p) {
+  using Cfg = GemmCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* staging = smem + Cfg::STAGES * Cfg::STAGE_BYTES;                       // 1024-aligned epilogue staging
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + Cfg::STAGING_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
   uint64_t* empty_bar = full_bar + Cfg::STAGES;
-  uint64_t* tfull_bar = empty_bar + Cfg::STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint64_t* aux_bar = tempty_bar + 2;                      // [EPI_WARPS][2] residual-box barriers (RES only)
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(aux_bar + 2 * EPI_WARPS);
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  long long* dbg = p.dbg ? p.dbg + (long long)blockIdx.x * 16 : nullptr;
-  if (dbg && threadIdx.x == 0) dbg[0] = clock64();
-  // Optional cluster of 2 CTAs along M: both work on the same (n, k) sequence, so each loads only half of
-  // every B tile and multicasts it into both CTAs' shared memory (L2 -> SM traffic per CTA drops from
-  // A + B to A + B/2); a stage is released by a multicast tcgen05.commit from both MMA issuers.
-  const uint32_t csize = cluster_nctarank();
-  const uint32_t crank = cluster_ctarank();
-  const uint16_t cmask = (uint16_t)((1u << csize) - 1u);
+  const int wg = threadIdx.x >> 7;
+  const int n0 = blockIdx.x * BN, m0 = blockIdx.y * BM, split = blockIdx.z;
+  const int kb0 = (int)(((long long)p.kblocks * split) / p.splits);
+  const int kb1 = (int)(((long long)p.kblocks * (split + 1)) / p.splits);
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    if (p.tail_bn) tma_prefetch_desc(&tmBt);
-    if (p.tma_store) tma_prefetch_desc(&tmC);
-    if (RES || p.tma_store >= 4) tma_prefetch_desc(&tmX);
-  }
-  if (warp == 1 && lane == 0) {
     for (int i = 0; i < Cfg::STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], csize);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], EPI_WARPS);  // one arrive per epilogue warp
-    }
-    if (RES || p.tma_store == 5) {
-      for (int i = 0; i < 2 * EPI_WARPS; ++i) mbar_init(&aux_bar[i], 1);
+      mbar_init(&empty_bar[i], 8);   // one arrive per consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == 2) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  if (csize > 1) cluster_sync_all();   // peer barriers are initialised before any multicast can target them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (dbg && threadIdx.x == 0) dbg[1] = clock64();   // setup done
 
-  const int total_units = p.full_units + p.tail_units;
-  const int unit0 = blockIdx.x / csize, unit_step = gridDim.x / csize;
-
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
       int stage = 0, phase = 0;
-      for (int unit = unit0; unit < total_units; unit += unit_step) {
-        const GemmUnit u = decode_unit<BN>(p, unit);
-        const int m_blk = u.mp * (int)csize + (int)crank;
-        const bool narrow = u.bn != BN;          // tail unit (single CTAs only): own B map with a tail_bn-row box
-        const int kb0 = u.kb0, kb1 = u.kb1;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
-          uint8_t* sB = sA + Cfg::A_BYTES;
-          mbar_arrive_expect_tx(&full_bar[stage], Cfg::A_BYTES + u.bn * BK * 2);
-          if (!p.a_mn) {
-            tma_load_2d(sA, &tmA, &full_bar[stage], kb * BK, m_blk * BM);
-          } else {
+      for (int kb = kb0; kb < kb1; ++kb) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
+        uint8_t* sB = sA + Cfg::A_BYTES;
+        mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+        if (!TA) {
+          tma_load_2d(sA, &tmA, &full_bar[stage], kb * BK, m0);
+        } else {
 #pragma unroll
-            for (int c = 0; c < BM / 64; ++c)
-              tma_load_2d(sA + c * CHUNK_BYTES, &tmA, &full_bar[stage], m_blk * BM + c * 64, kb * BK);
-          }
-          if (csize == 1) {
-            if (!p.b_mn) {
-              tma_load_2d(sB, narrow ? &tmBt : &tmB, &full_bar[stage], kb * BK, u.n0);
-            } else {
-              for (int c = 0; c < u.bn / 64; ++c)
-                tma_load_2d(sB + c * CHUNK_BYTES, &tmB, &full_bar[stage], u.n0 + c * 64, kb * BK);
-            }
-          } else {
-            // my half of the B tile, delivered to both CTAs (the peer sends the other half)
-            if (!p.b_mn) {
-              const int r0 = (int)crank * (BN / 2);
-              tma_load_2d_mc(sB + r0 * 128, &tmB, &full_bar[stage], kb * BK, u.n0 + r0, cmask);
-            } else {
-              constexpr int NCH = BN / 64;
-              const int c0 = crank == 0 ? 0 : (NCH + 1) / 2, c1 = crank == 0 ? (NCH + 1) / 2 : NCH;
-              for (int c = c0; c < c1; ++c)
-                tma_load_2d_mc(sB + c * CHUNK_BYTES, &tmB, &full_bar[stage], u.n0 + c * 64, kb * BK, cmask);
-            }
-          }
-          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+          for (int c = 0; c < BM / 64; ++c) tma_load_2d(sA + c * CHUNK_BYTES, &tmA, &full_bar[stage], m0 + c * 64, kb * BK);
         }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int stage = 0, phase = 0, acc = 0, acc_phase = 0;
-      for (int unit = unit0; unit < total_units; unit += unit_step) {
-        const GemmUnit u = decode_unit<BN>(p, unit);
-        const uint32_t idesc = make_idesc_bf16(BM, (uint32_t)u.bn, (uint32_t)p.a_mn, (uint32_t)p.b_mn);
-        const int kb0 = u.kb0, kb1 = u.kb1;
-        mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(acc * BN);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          if (dbg && unit == unit0 && kb == kb0) dbg[2] = clock64();   // first operands landed
-          const uint32_t a_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-          const uint32_t b_addr = a_addr + Cfg::A_BYTES;
+        if (!TB) {
+          tma_load_2d(sB, &tmB, &full_bar[stage], kb * BK, n0);
+        } else {
 #pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            const uint64_t adesc = p.a_mn ? sdesc_mnmajor(a_addr + k * 2048, CHUNK_BYTES) : sdesc_kmajor(a_addr + k * 32);
-            const uint64_t bdesc = p.b_mn ? sdesc_mnmajor(b_addr + k * 2048, CHUNK_BYTES) : sdesc_kmajor(b_addr + k * 32);
-            umma_bf16_ss(d_tmem, adesc, bdesc, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          // frees the smem slot (in both CTAs of a cluster: the peer multicasts into it) when these MMAs retire
-          if (csize == 1) umma_commit(&empty_bar[stage]);
-          else umma_commit_mc(&empty_bar[stage], cmask);
-          if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+          for (int c = 0; c < BN / 64; ++c) tma_load_2d(sB + c * CHUNK_BYTES, &tmB, &full_bar[stage], n0 + c * 64, kb * BK);
         }
-        umma_commit(&tfull_bar[acc]);  // accumulator complete -> epilogue
-        if (dbg) { if (unit == unit0) dbg[3] = clock64(); dbg[4] = clock64(); }   // MMAs of first / last tile issued
-        if (++acc == 2) { acc = 0; acc_phase ^= 1; }
+        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp >= 4) {
-    // Epilogue: 8 warps = two warpgroups; warpgroup `half` drains the 32-column chunks c = half, half+2, ...
-    // tcgen05.ld hands each thread one accumulator ROW (32 columns); written straight to global memory that is
-    // 32 different rows per store instruction.  Instead every 32x32 fp32 block takes a trip through a per-warp
-    // shared-memory tile (pitch 33 words, conflict-free both ways) and comes back transposed: 8 lanes x 4 columns
-    // cover 128 contiguous bytes of ONE row, 4 rows per instruction, so residual / z loads and all stores are
-    // whole sectors of contiguous rows.  Loads of the epilogue operand (residual or z) are issued one chunk
-    // ahead so their latency hides behind the TMEM drain + transpose of the current chunk.
-    const int q = warp & 3;             // TMEM lane quadrant this warp may access
-    const int half = (warp - 4) >> 2;   // which warpgroup
-    float* stg = reinterpret_cast<float*>(staging) + (warp - 4) * (32 * EPI_PITCH);
-    uint8_t* slot = staging + (warp - 4) * (RES ? RES_SLOT_BYTES : 4096);
-    uint32_t aux_use[2] = {0u, 0u};
-    int acc = 0, acc_phase = 0;
-    for (int unit = unit0; unit < total_units; unit += unit_step) {
-      const GemmUnit u = decode_unit<BN>(p, unit);
-      const int m_blk = u.mp * (int)csize + (int)crank;
-      const uint32_t t_base = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * BN);
-      if constexpr (RES) {
-        epilogue_tile_tma_res<BN>(p, &tmC, &tmX, slot, aux_bar + 2 * (warp - 4), aux_use, t_base, m_blk, u.n0, u.bn, q, half, lane,
-                                  &tfull_bar[acc], (uint32_t)acc_phase);
-      } else {
-        if (p.tma_store == 5) epilogue_tile_tma_dgelu<BN>(p, &tmC, &tmX, slot, aux_bar + 2 * (warp - 4), aux_use, t_base, m_blk, u.n0, u.bn, q, half, lane, &tfull_bar[acc], (uint32_t)acc_phase);
-        else if (p.tma_store) epilogue_tile_tma<BN>(p, &tmC, &tmX, slot, t_base, m_blk, u.n0, u.bn, u.split, q, half, lane, &tfull_bar[acc], (uint32_t)acc_phase);
-        else epilogue_tile<BN>(p, stg, t_base, m_blk, u.n0, u.bn, u.split, q, half, lane, &tfull_bar[acc], (uint32_t)acc_phase);
-      }
-      if (dbg && warp == 4 && lane == 0) { if (unit == unit0) dbg[5] = clock64(); dbg[6] = clock64(); }   // first / last tile drained
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-      if (++acc == 2) { acc = 0; acc_phase ^= 1; }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (csize > 1) cluster_sync_all();   // no CTA leaves while its peer may still multicast into it
-  if (dbg && threadIdx.x == 0) dbg[7] = clock64();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
+  setmaxnreg_inc<232>();
+  const int cw = wg - 1;                       // consumer: rows [64 cw, 64 cw + 64) of the tile
+  const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+  int stage = 0, phase = 0, prev = -1;
+  for (int kb = kb0; kb < kb1; ++kb) {
+    mbar_wait(&full_bar[stage], phase);
+    const uint32_t a_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES) + cw * (TA ? CHUNK_BYTES : 64 * 128);
+    const uint32_t b_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < BK / 16; ++k) {
+      const uint64_t da = TA ? sdesc_mnmajor(a_addr + k * 2048, CHUNK_BYTES) : sdesc_kmajor(a_addr + k * 32);
+      const uint64_t db = TB ? sdesc_mnmajor(b_addr + k * 2048, CHUNK_BYTES) : sdesc_kmajor(b_addr + k * 32);
+      wgmma_tile<BN, TA, TB>(acc, da, db, (kb > kb0 || k > 0) ? 1u : 0u);
+    }
+    wgmma_commit();
+    // the previous k-block's MMAs have retired once at most this one is in flight: its stage is free
+    wgmma_wait<1>();
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+    prev = stage;
+    if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+
+  const int r0 = m0 + cw * 64 + warp * 16 + (lane >> 2);
+  const EpiRow e0 = epi_row(p, r0, split), e1 = epi_row(p, r0 + 8, split);
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int n = n0 + 8 * j + 2 * (lane & 3);
+    if (n >= p.N) break;
+    epi_pair(p, e0, n, acc[4 * j], acc[4 * j + 1]);
+    epi_pair(p, e1, n, acc[4 * j + 2], acc[4 * j + 3]);
   }
 }
 
@@ -247,178 +253,6 @@ int make_tmap_bf16_2d(CUtensorMap* map, const void* base, long long rows, long l
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   VT_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) rows=%lld cols=%lld ld=%lld box_rows=%d", (int)r,
              rows, cols, ld, box_rows);
-  return 0;
-}
-
-// Output map for the TMA-store epilogue: [splits][M][N] (bf16 or fp32), box {32 cols, 32 rows, 1}, swizzle = row bytes.
-int make_tmap_out_3d(CUtensorMap* map, const void* base, int fp32, long long M, long long N, long long ld, long long splits,
-                     long long split_stride) {
-  EncodeTiledFn fn = get_encode_fn();
-  VT_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled entry point unavailable");
-  const int esz = fp32 ? 4 : 2;
-  cuuint64_t gdim[3] = {(cuuint64_t)N, (cuuint64_t)M, (cuuint64_t)splits};
-  cuuint64_t gstr[2] = {(cuuint64_t)(ld * esz), (cuuint64_t)((splits > 1 ? split_stride : M * ld) * esz)};
-  cuuint32_t box[3] = {32u, 32u, 1u};
-  cuuint32_t estr[3] = {1u, 1u, 1u};
-  CUresult r = fn(map, fp32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), gdim,
-                  gstr, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, fp32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
-                  CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  VT_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(out) failed (%d) M=%lld N=%lld ld=%lld", (int)r, M, N, ld);
-  return 0;
-}
-
-// 3-D fp32 map (col, p, b), box {32, 32, 1}: the row maps whose period is a single run of rows (temporal, or no map at all)
-// estride > 1: the box covers 32 rows that lie `estride` rows apart (box height 32 * estride, element stride estride <= 8)
-int make_tmap_rows_3d(CUtensorMap* map, const void* base, long long cols, long long pcount, long long bcount, long long stride_p,
-                      long long stride_b, int estride = 1) {
-  EncodeTiledFn fn = get_encode_fn();
-  VT_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled entry point unavailable");
-  VT_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0, "TMA base pointer must be 16-byte aligned");
-  VT_REQUIRE(stride_p % 4 == 0 && stride_b % 4 == 0 && stride_p > 0 && stride_b > 0, "row-map strides must be positive multiples of 4");
-  VT_REQUIRE(estride >= 1 && estride <= 8, "row-map element stride %d outside 1..8", estride);
-  cuuint64_t gdim[3] = {(cuuint64_t)cols, (cuuint64_t)pcount, (cuuint64_t)bcount};
-  cuuint64_t gstr[2] = {(cuuint64_t)(stride_p * 4), (cuuint64_t)(stride_b * 4)};
-  cuuint32_t box[3] = {32u, 32u * (cuuint32_t)estride, 1u};
-  cuuint32_t estr[3] = {1u, (cuuint32_t)estride, 1u};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void*>(base), gdim, gstr, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  VT_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled(rows 3d) failed (%d) dims %lld %lld %lld strides %lld %lld", (int)r, cols,
-             pcount, bcount, stride_p, stride_b);
-  return 0;
-}
-
-// Residual epilogue on TMA (GemmDev::tma_store = 3): fp32 output with an fp32 addend whose rows — and the output's — follow
-// either no map or the affine map described in vt_gemm_params (map_period ...).  Fills tmC / tmX and the map fields of d.
-bool res_tma_applicable(const vt_gemm_params* q) {
-  if (q->epilogue != VT_EPI_F32 || !q->aux || getenv("VT_NO_TMA_STORE") || !feature_on("VT_TMA_RES", VT_DEFAULT_TMA_RES)) return false;
-  if (q->N % 4 != 0) return false;
-  if (q->map_period > 0) {
-    if (q->map_tcount > 1) {        // spatial regrouping: element-strided boxes, own switch
-      if (!feature_on("VT_TMA_RES_SPATIAL", VT_DEFAULT_TMA_RES_SPATIAL)) return false;
-      if (q->map_tcount > 8 || q->map_stride_p != (long long)q->map_tcount * q->map_stride_t) return false;
-    }
-    // groups of 32 rows that straddle a period boundary or start on a special row are written row by row from the index arrays
-    if ((q->map_period % 32 != 0 || q->map_skip > 0) && !(q->out_row && q->aux_row)) return false;
-    return q->map_period >= 32 && q->map_tcount >= 1 && q->M % q->map_period == 0;
-  }
-  return !q->out_row && !q->aux_row && q->ldo % 4 == 0 && q->ldaux % 4 == 0;
-}
-
-int setup_res_maps(const vt_gemm_params* q, GemmDev& d, CUtensorMap* tmC, CUtensorMap* tmX) {
-  d.tma_store = 3;
-  if (q->map_period > 0) {
-    d.map_period = q->map_period; d.map_skip = q->map_skip; d.map_tcount = q->map_tcount;
-    const long long outers = q->M / q->map_period;
-    const long long bcount = (outers + q->map_tcount - 1) / q->map_tcount;
-    const long long pcount = q->map_period - q->map_skip;
-    // one map for both regroupings: (col, row in sample, sample).  map_tcount > 1 (spatial): the stream rows of one frame are
-    // map_tcount rows apart = element stride of the box
-    d.map_rank = 3;
-    const long long rows_in_sample = pcount * q->map_tcount;
-    const long long row_stride = q->map_tcount > 1 ? q->map_stride_t : q->map_stride_p;
-    int rc = make_tmap_rows_3d(tmC, static_cast<float*>(q->out) + q->map_base, q->N, rows_in_sample, bcount, row_stride, q->map_stride_b,
-                               q->map_tcount);
-    if (rc) return rc;
-    rc = make_tmap_rows_3d(tmX, static_cast<const float*>(q->aux) + q->map_base, q->N, rows_in_sample, bcount, row_stride,
-                           q->map_stride_b, q->map_tcount);
-    if (rc) return rc;
-    d.special_out = q->map_special_base >= 0 ? static_cast<float*>(q->out) + q->map_special_base : nullptr;
-    d.special_ld = q->map_special_stride;
-    return 0;
-  }
-  d.map_period = q->M; d.map_skip = 0; d.map_tcount = 1; d.map_rank = 3;
-  d.special_out = nullptr; d.special_ld = 0;
-  // one "sample" of M rows: (col, row, 0); the third dimension only exists to clip rows >= M of a two-segment group
-  int rc = make_tmap_rows_3d(tmC, q->out, q->N, q->M, 1, q->ldo, (long long)q->M * q->ldo);
-  if (rc) return rc;
-  return make_tmap_rows_3d(tmX, q->aux, q->N, q->M, 1, q->ldaux, (long long)q->M * q->ldaux);
-}
-
-// ------------------------------------------------------------------------------------------------
-// Unit schedule.  Regular units = (macro row, n tile, K split); if the last macro row holds only a few valid rows
-// (M = 12 552 = 98 x 128 + 8: TimeSformer's FFN; 12 608 = 98 x 128 + 64: its spatial pass) it is cut into narrow units of
-// `tail_bn` columns instead, which cost a fraction of a tile (their A rows are mostly TMA zero fill, their MMAs N = tail_bn
-// wide) and spread over the CTAs that would otherwise idle in a whole extra round.
-//   makespan model (in units of one full tile): units are dealt round-robin to `slots` CTAs / CTA pairs.
-// ------------------------------------------------------------------------------------------------
-struct Schedule { int full_units, tail_units, tail_bn, tail_mp; double makespan; };
-
-Schedule plan_units(int M, int N, int bn, int rows_per_macro, int splits, int slots, int tail_bn_cand, int tail_mode) {
-  const int num_mp = (M + rows_per_macro - 1) / rows_per_macro;
-  const int num_n = (N + bn - 1) / bn;
-  Schedule best;
-  best.full_units = num_mp * num_n * splits; best.tail_units = 0; best.tail_bn = 0; best.tail_mp = 0;
-  best.makespan = (double)((best.full_units + slots - 1) / slots);
-  const int valid_tail = M - (num_mp - 1) * rows_per_macro;       // rows in the last macro row
-  // tail_mode: 0 = take the narrow tail when the model says it is faster, 1 = never, 2 = whenever the shape allows (tests)
-  if (tail_mode == 1 || splits != 1 || num_mp < 2 || valid_tail == rows_per_macro || valid_tail > 64 || tail_bn_cand <= 0 ||
-      tail_bn_cand >= bn || N % 8 != 0)
-    return best;
-  Schedule t;
-  t.full_units = (num_mp - 1) * num_n; t.tail_bn = tail_bn_cand; t.tail_mp = num_mp - 1;
-  t.tail_units = (N + tail_bn_cand - 1) / tail_bn_cand;
-  // cost of a tail unit relative to a full tile: operand bytes that really come from L2 (valid A rows + narrow B) vs a full
-  // stage, floored by the MMA time ratio, plus the fixed per-unit overhead share
-  const double bytes = (double)(valid_tail + tail_bn_cand) / (double)(rows_per_macro > 128 ? 128 + bn / 2 : 128 + bn);
-  const double mma = (double)tail_bn_cand / bn;
-  const double tcost = (bytes > mma ? bytes : mma) + 0.08;
-  const int total = t.full_units + t.tail_units;
-  double worst = 0.0;
-  for (int sl = 0; sl < slots; ++sl) {            // the kernel deals unit u to slot u % slots
-    const int nf = sl < t.full_units ? (t.full_units - 1 - sl) / slots + 1 : 0;
-    const int nall = sl < total ? (total - 1 - sl) / slots + 1 : 0;
-    const double load = nf + (nall - nf) * tcost;
-    if (load > worst) worst = load;
-  }
-  t.makespan = worst;
-  return (tail_mode == 2 || t.makespan < best.makespan - 1e-9) ? t : best;
-}
-
-// Split-K partials can be reduce-added straight into the output by TMA (cp.reduce.async.bulk.tensor ... add) instead of
-// going through the fp32 workspace + reduce_rows: needs the plain fp32 TMA epilogue and a dense output.
-bool splitk_in_place(const vt_gemm_params* q) {
-  return q->ldo == q->N && !getenv("VT_NO_TMA_STORE") && !getenv("VT_SPLITK_WORKSPACE");
-}
-
-// Decide whether the plain TMA-store epilogue applies and build its map (called after the split decision).
-// in_place: d.out is the final output and the d.splits partial tiles of every output tile are reduce-added into it.
-int setup_out_map(const vt_gemm_params* q, GemmDev& d, CUtensorMap* tmC, bool in_place, CUtensorMap* tmC2) {
-  d.tma_store = 0;
-  memset(tmC, 0, sizeof(*tmC));
-  if (q->epilogue == VT_EPI_GELU && !q->out_row && !getenv("VT_NO_TMA_STORE") && feature_on("VT_TMA_GELU", VT_DEFAULT_TMA_GELU) && tmC2) {
-    // z and h = gelu(z) both leave through TMA stores (two bf16 boxes per chunk)
-    int rc = make_tmap_out_3d(tmC, d.out, 0, q->M, q->N, d.ldo, 1, 0);
-    if (rc) return rc;
-    rc = make_tmap_out_3d(tmC2, d.out2, 0, q->M, q->N, d.ldo2, 1, 0);
-    if (rc) return rc;
-    d.tma_store = 4;
-    return 0;
-  }
-  if (q->epilogue == VT_EPI_DGELU && !q->out_row && !q->aux_row && q->aux && !getenv("VT_NO_TMA_STORE") &&
-      feature_on("VT_TMA_DGELU", VT_DEFAULT_TMA_DGELU) && tmC2 &&
-      q->ldo % 8 == 0 && q->ldaux % 8 == 0) {
-    // out = acc * gelu'(z): z boxes TMA-loaded into the staging buffers, product TMA-stored from there (opt-in: VT_TMA_DGELU=1)
-    int rc = make_tmap_out_3d(tmC, d.out, 0, q->M, q->N, d.ldo, 1, 0);
-    if (rc) return rc;
-    rc = make_tmap_out_3d(tmC2, q->aux, 0, q->M, q->N, q->ldaux, 1, 0);
-    if (rc) return rc;
-    d.tma_store = 5;
-    return 0;
-  }
-  const bool plain = (q->epilogue == VT_EPI_BF16 || q->epilogue == VT_EPI_F32) && !q->out_row && !q->aux;
-  if (!plain || getenv("VT_NO_TMA_STORE")) return 0;
-  const int fp32 = q->epilogue == VT_EPI_F32;
-  int rc = make_tmap_out_3d(tmC, d.out, fp32, q->M, q->N, d.ldo, in_place ? 1 : d.splits, in_place ? 0 : d.split_stride);
-  if (rc) return rc;
-  d.tma_store = in_place ? 2 : 1;
-  return 0;
-}
-
-// zero the output ahead of an in-place split-K launch
-int splitk_zero(const vt_gemm_params* q, cudaStream_t st) {
-  cudaError_t e = cudaMemsetAsync(q->out, 0, (size_t)q->M * q->N * sizeof(float), st);
-  VT_REQUIRE(e == cudaSuccess, "vt_gemm: split-K output memset: %s", cudaGetErrorString(e));
   return 0;
 }
 
@@ -494,111 +328,56 @@ int launch_reduce_rows(const float* in, float* out, long long stride, int S, lon
   return check_launch("reduce_rows_kernel");
 }
 
-template <int BN, bool RES>
-static int launch_gemm(const vt_gemm_params* q, GemmDev& d, cudaStream_t st) {
-  using Cfg = GemmCfg<BN, RES>;
+template <int BN, int TA, int TB>
+static int launch_gemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& d, int num_m, cudaStream_t st) {
+  using Cfg = GemmCfg<BN>;
   static bool attr_set = false;  // benign race: idempotent
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_tcgen05_kernel<BN, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, TA, TB>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
     VT_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(smem=%d) failed: %s", Cfg::SMEM_BYTES, cudaGetErrorString(e));
     attr_set = true;
   }
-  CUtensorMap tmA, tmB, tmBt, tmC, tmX;
-  memset(&tmBt, 0, sizeof(tmBt));
-  memset(&tmX, 0, sizeof(tmX));
+  const dim3 grid((unsigned)((d.N + BN - 1) / BN), (unsigned)num_m, (unsigned)d.splits);
+  gemm_wgmma_kernel<BN, TA, TB><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(tmA, tmB, d);
+  return check_launch("gemm_wgmma_kernel");
+}
+
+template <int BN>
+static int launch_gemm(const vt_gemm_params* q, GemmDev& d, cudaStream_t st) {
+  CUtensorMap tmA, tmB;
   int rc;
   if (!q->a_mn_major) rc = make_tmap_bf16_2d(&tmA, q->a, q->M, q->K, q->lda, BM);
   else rc = make_tmap_bf16_2d(&tmA, q->a, q->K, q->M, q->lda, BK);
   if (rc) return rc;
-  d.num_m = (q->M + BM - 1) / BM;
-  // clusters of 2 along M whenever there are at least two row tiles (force_cluster: 1 = never, 2 = always)
-  // Measured on B200 (profiles/): sharing B by multicast does not speed this kernel up — its mainloop is limited by
-  // shared-memory capacity (bytes in flight per SM), not by L2->SM bandwidth — so clusters are opt-in.
-  const int csize = q->force_cluster == 2 ? 2 : 1;
-  if (!q->b_mn_major) rc = make_tmap_bf16_2d(&tmB, q->b, q->N, q->K, q->ldb, BN / csize);
+  if (!q->b_mn_major) rc = make_tmap_bf16_2d(&tmB, q->b, q->N, q->K, q->ldb, BN);
   else rc = make_tmap_bf16_2d(&tmB, q->b, q->K, q->N, q->ldb, BK);
   if (rc) return rc;
-  d.num_mp = (d.num_m + csize - 1) / csize;
-
-  d.num_n = (q->N + BN - 1) / BN;
-  d.kblocks = (q->K + BK - 1) / BK;
-  const int sms = persistent_sm_count();
-
-  int splits = 1;
+  const int num_m = (q->M + BM - 1) / BM;
+  VT_REQUIRE(num_m <= 65535, "vt_gemm: M=%d too large", q->M);
   const long long tile_out = (long long)q->M * q->N;
-  if (q->epilogue == VT_EPI_F32 && q->workspace && !q->out_row && !q->aux && !q->row_scale && !q->bias) {
-    if (q->force_splits > 0) splits = q->force_splits;
-    else splits = d.splits > 0 ? d.splits : 1;    // chosen together with BN by choose_config()
-    const long long max_by_ws = q->workspace_bytes / (tile_out * 4);
-    if (splits > max_by_ws) splits = (int)max_by_ws;
-    if (splits > d.kblocks) splits = d.kblocks;
-    if (splits < 1) splits = 1;
-  }
-  d.splits = splits;
   void* final_out = d.out;
-  const bool in_place = splits > 1 && splitk_in_place(q);
   d.split_stride = 0;
-  if (in_place) {
-    rc = q->out_zeroed ? 0 : splitk_zero(q, st);
-    if (rc) return rc;
-  } else if (splits > 1) {
+  if (d.splits > 1) {            // partial tiles -> fp32 workspace [splits, M, N], summed below
     d.out = q->workspace;
     d.ldo = q->N;
     d.split_stride = tile_out;
   }
-  if (RES) rc = setup_res_maps(q, d, &tmC, &tmX);
-  else rc = setup_out_map(q, d, &tmC, in_place, &tmX);
+  if (!q->a_mn_major && !q->b_mn_major) rc = launch_gemm_t<BN, 0, 0>(tmA, tmB, d, num_m, st);
+  else if (!q->a_mn_major) rc = launch_gemm_t<BN, 0, 1>(tmA, tmB, d, num_m, st);
+  else if (!q->b_mn_major) rc = launch_gemm_t<BN, 1, 0>(tmA, tmB, d, num_m, st);
+  else rc = launch_gemm_t<BN, 1, 1>(tmA, tmB, d, num_m, st);
   if (rc) return rc;
-  // unit schedule (narrow tail units only for single CTAs here; CTA pairs have their own in vt_gemm2.cu)
-  const int max_clusters = sms / csize;
-  const Schedule sch = plan_units(q->M, q->N, BN, BM * csize, splits, max_clusters, 64,
-                                  (csize != 1 || !tail_units_enabled()) ? 1 : q->force_tail);
-  d.full_units = sch.full_units; d.tail_units = sch.tail_units; d.tail_bn = sch.tail_bn; d.tail_mp = sch.tail_mp;
-  if (d.tail_bn && !q->b_mn_major) {
-    rc = make_tmap_bf16_2d(&tmBt, q->b, q->N, q->K, q->ldb, d.tail_bn);
-    if (rc) return rc;
-  }
-  const int units = d.full_units + d.tail_units;
-  const int grid = (units < max_clusters ? units : max_clusters) * csize;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)grid);
-  cfg.blockDim = dim3(GEMM_THREADS);
-  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = (unsigned)csize;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  cudaError_t le = cudaLaunchKernelEx(&cfg, gemm_tcgen05_kernel<BN, RES>, tmA, tmB, tmBt, tmC, tmX, d);
-  if (le != cudaSuccess) {
-    set_error("gemm_tcgen05_kernel: cudaLaunchKernelEx failed: %s", cudaGetErrorString(le));
-    return 2;
-  }
-  rc = check_launch("gemm_tcgen05_kernel");
-  if (rc) return rc;
-  if (splits > 1 && !in_place) {
-    // partials [splits, M, N] -> out [M, ldo]
-    if (q->ldo == q->N) {
-      return launch_reduce_rows(static_cast<const float*>(q->workspace), static_cast<float*>(final_out), tile_out, splits,
-                                tile_out, 0, 1.0f, st);
-    }
-    set_error("vt_gemm: split-K requires ldo == N");
-    return 1;
+  if (d.splits > 1) {
+    VT_REQUIRE(q->ldo == q->N, "vt_gemm: split-K requires ldo == N");
+    return launch_reduce_rows(static_cast<const float*>(q->workspace), static_cast<float*>(final_out), tile_out, d.splits, tile_out,
+                              0, 1.0f, st);
   }
   return 0;
 }
 
-int launch_gemm2(const vt_gemm_params* q, GemmDev& d, int bn, bool res, cudaStream_t st);
+int launch_gemm_rows(const vt_gemm_params* q, int m0, void* stream);   // vt_gemm_rows.cu
 
 }  // namespace vt
-
-namespace vt {
-int launch_gemm_rows(const vt_gemm_params* q, int m0, void* stream);   // vt_gemm_rows.cu
-}
 
 // M a few rows past a multiple of 128: tensor-core kernel on the full row tiles, CUDA-core dot products for the rest
 // (vt_gemm_rows.cu).  Plain row-major calls only; anything forced by a test goes through the one-kernel path.
@@ -608,8 +387,7 @@ int launch_gemm_rows(const vt_gemm_params* q, int m0, void* stream);   // vt_gem
 static int rows_split_point(const vt_gemm_params* q) {
   const int r = q->M % vt::BM;
   if (r == 0 || r > 16 || q->M < 8 * vt::BM) return 0;
-  // measured (tools/rows_probe.py): the extra launch costs ~10 us, so the split only pays where the partial row of tiles
-  // costs a long extra round — few n-tiles, long K (FC2 and the FC1 data gradient: 82 -> 78 us, 73 -> 62 us)
+  // the extra launch only pays where the partial row of tiles costs a long extra round: few n-tiles, long K
   if (q->N > 1024 || q->K < 2048) return 0;
   if (!vt::feature_on("VT_ROWS_SPLIT", VT_DEFAULT_ROWS_SPLIT)) return 0;
   if (q->a_mn_major || (q->epilogue != VT_EPI_BF16 && q->epilogue != VT_EPI_F32)) return 0;
@@ -652,91 +430,70 @@ static int gemm_dispatch(const vt_gemm_params* q, void* stream) {
   if (q->bias) VT_REQUIRE((reinterpret_cast<uintptr_t>(q->bias) & 15) == 0, "vt_gemm: bias misaligned");
   if (q->bias2) VT_REQUIRE(q->epilogue == VT_EPI_F32 && q->aux && (reinterpret_cast<uintptr_t>(q->bias2) & 15) == 0,
                            "vt_gemm: bias2 needs the fp32 epilogue with an addend, 16-byte aligned");
+  VT_REQUIRE(q->force_bn == 0 || q->force_bn == 128 || q->force_bn == 192 || q->force_bn == 256,
+             "vt_gemm: force_bn must be 128, 192 or 256");
 
   GemmDev d;
   d.M = q->M; d.N = q->N; d.K = q->K;
-  d.a_mn = q->a_mn_major ? 1 : 0;
-  d.b_mn = q->b_mn_major ? 1 : 0;
   d.epi = q->epilogue;
   d.bias = q->bias;
   d.bias2 = q->bias2;
   d.out = q->out; d.out2 = q->out2; d.aux = q->aux;
   d.ldo = q->ldo; d.ldo2 = q->ldo2; d.ldaux = q->ldaux;
   d.out_row = q->out_row; d.aux_row = q->aux_row; d.row_scale = q->row_scale;
-  d.dbg = static_cast<long long*>(q->debug);
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-
-  d.tma_store = 0;
-  d.map_period = q->M > 0 ? q->M : 1; d.map_skip = 0; d.map_tcount = 1; d.map_rank = 3;
+  d.kblocks = (q->K + BK - 1) / BK;
+  d.map_period = 0; d.map_skip = 0; d.map_tcount = 1;
+  d.map_stride_t = d.map_stride_p = d.map_stride_b = d.map_base = 0;
   d.special_out = nullptr; d.special_ld = 0;
-  d.tail_bn = 0; d.full_units = 0; d.tail_units = 0; d.tail_mp = 0;
   if (q->map_period > 0) {
     VT_REQUIRE(q->epilogue == VT_EPI_F32 && q->aux, "vt_gemm: the affine row map applies to the fp32 residual epilogue only");
     VT_REQUIRE(q->M % q->map_period == 0 && q->map_tcount >= 1 && q->map_skip >= 0 && q->map_skip < q->map_period,
                "vt_gemm: bad affine row map (period %d, skip %d, tcount %d, M %d)", q->map_period, q->map_skip, q->map_tcount, q->M);
-  }
-  const bool res = res_tma_applicable(q);
-  if (q->map_period > 0 && !res) {
-    VT_REQUIRE(q->out_row && q->aux_row, "vt_gemm: affine row map given but the TMA residual epilogue is unavailable and no "
-                                         "out_row / aux_row arrays were supplied for the generic epilogue");
+    // the epilogue moves column pairs as float2: every element offset of the map must be even
+    VT_REQUIRE(q->map_base % 2 == 0 && q->map_stride_t % 2 == 0 && q->map_stride_p % 2 == 0 && q->map_stride_b % 2 == 0 &&
+                   (q->map_special_base < 0 || (q->map_special_base % 2 == 0 && q->map_special_stride % 2 == 0)),
+               "vt_gemm: affine row map offsets and strides must be even (8-byte aligned fp32 pairs)");
+    d.map_period = q->map_period; d.map_skip = q->map_skip; d.map_tcount = q->map_tcount;
+    d.map_stride_t = q->map_stride_t; d.map_stride_p = q->map_stride_p; d.map_stride_b = q->map_stride_b; d.map_base = q->map_base;
+    d.special_out = q->map_special_base >= 0 ? static_cast<float*>(q->out) + q->map_special_base : nullptr;
+    d.special_ld = q->map_special_stride;
   }
 
-  int bn = q->force_bn;
-  d.splits = 0;
-  {
-    // Wave-quantisation aware configuration: cost ~ makespan over the SMs x per-unit time, where a unit (tile x
-    // K-split) costs (its k-blocks + a fixed prologue/epilogue overhead) x BN, with a small penalty for narrower
-    // tiles (they re-read A more often and leave less slack on the smem port).  Splitting K is only possible for
-    // plain fp32 outputs with a workspace (weight gradients).  A partial last macro row may run as narrow tail units
-    // (plan_units).
-    const int sms = persistent_sm_count();
-    const int num_m = (q->M + BM - 1) / BM;
-    const int kblocks = (q->K + BK - 1) / BK;
-    const bool can_split = q->epilogue == VT_EPI_F32 && q->workspace && !q->out_row && !q->aux && !q->row_scale && !q->bias;
-    const int tail_mode = tail_units_enabled() ? q->force_tail : 1;
-    // kernel variants: 0 = one CTA per 128 x BN tile (optionally clusters with multicast B), 1 = CTA pairs with
-    // tcgen05.mma.cta_group::2 (256 x BN macro tiles, half of B per SM, 6-8 stages).  The pair kernel's unit time is
-    // ~8% shorter (measured, profiles/) but its macro tiles quantise worse and it has no BN = 192; it is skipped
-    // for small MN-major weight-gradient shapes, where it measured slower.
-    const bool pair_forced = q->force_cluster == 3;
-    const bool pair_ok = pair_forced || (q->force_cluster == 0 && num_m >= 2 &&
-                                         (!q->a_mn_major || (long long)q->M * q->N >= 2000000LL));
-    const int cand[3] = {256, 192, 128};
-    // the residual instantiation of the single-CTA 256-wide kernel runs on 3 pipeline stages: penalised
-    const double penalty[3] = {res ? 1.12 : 1.0, 1.04, 1.10};
-    double best = 1e30;
-    int best_bn = 256, best_s = 1, best_pair = 0;
-    for (int variant = 0; variant < 2; ++variant) {
-      if (variant == 1 && !pair_ok) continue;
-      if (variant == 0 && pair_forced) continue;
-      for (int i = 0; i < 3; ++i) {
-        if (q->force_bn && cand[i] != q->force_bn) continue;
-        if (variant == 1 && cand[i] == 192) continue;
-        const int cs = (q->force_cluster == 2 || variant == 1) ? 2 : 1;
-        const int slots = sms / cs;
-        const int smax = can_split ? 16 : 1;
-        for (int sp = 1; sp <= smax; ++sp) {
-          if (sp > 1 && (kblocks / sp < 4 || (long long)sp * q->M * q->N * 4 > q->workspace_bytes)) break;
-          const Schedule sch = plan_units(q->M, q->N, cand[i], BM * cs, sp, slots, variant == 1 ? 128 : 64,
-                                          (variant == 0 && q->force_cluster == 2) ? 1 : tail_mode);
-          const double cost = sch.makespan * ((double)kblocks / sp + 8.0) * cand[i] * penalty[i] * (variant == 1 ? 0.92 : 1.0);
-          if (cost < best - 1e-9) { best = cost; best_bn = cand[i]; best_s = sp; best_pair = variant; }
-        }
-      }
+  // Wave-quantisation aware configuration: cost ~ waves over the SMs x per-tile time, where a tile (x K split) costs
+  // (its k-blocks + a fixed prologue/epilogue overhead) x BN, with a small penalty for narrower tiles (they re-read A
+  // more often).  Splitting K is only possible for plain fp32 outputs with a workspace (weight gradients).
+  const int sms = persistent_sm_count();
+  const int num_m = (q->M + BM - 1) / BM;
+  const bool can_split = q->epilogue == VT_EPI_F32 && q->workspace && !q->out_row && !q->aux && !q->row_scale && !q->bias &&
+                         q->map_period == 0;
+  const int cand[3] = {256, 192, 128};
+  const double penalty[3] = {1.0, 1.04, 1.10};
+  double best = 1e30;
+  int bn = 128, splits = 1;
+  for (int i = 0; i < 3; ++i) {
+    if (q->force_bn && cand[i] != q->force_bn) continue;
+    const int num_n = (q->N + cand[i] - 1) / cand[i];
+    const int smax = can_split ? 16 : 1;
+    for (int sp = 1; sp <= smax; ++sp) {
+      if (sp > 1 && (d.kblocks / sp < 4 || (long long)sp * q->M * q->N * 4 > q->workspace_bytes)) break;
+      const long long tiles = (long long)num_m * num_n * sp;
+      const double waves = (double)((tiles + sms - 1) / sms);
+      const double cost = waves * ((double)d.kblocks / sp + 8.0) * cand[i] * penalty[i];
+      if (cost < best - 1e-9) { best = cost; bn = cand[i]; splits = sp; }
     }
-    if (bn == 0 || best_pair) bn = best_bn;
-    d.splits = best_s;
-    if (best_pair) return launch_gemm2(q, d, bn, res, st);
   }
-  VT_REQUIRE(bn == 128 || bn == 192 || bn == 256, "vt_gemm: force_bn must be 128, 192 or 256");
-  if (res) {
-    if (bn == 256) return launch_gemm<256, true>(q, d, st);
-    if (bn == 192) return launch_gemm<192, true>(q, d, st);
-    return launch_gemm<128, true>(q, d, st);
+  if (can_split && q->force_splits > 0) {
+    splits = q->force_splits;
+    const long long max_by_ws = q->workspace_bytes / ((long long)q->M * q->N * 4);
+    if (splits > max_by_ws) splits = (int)max_by_ws;
+    if (splits > d.kblocks) splits = d.kblocks;
+    if (splits < 1) splits = 1;
   }
-  if (bn == 256) return launch_gemm<256, false>(q, d, st);
-  if (bn == 192) return launch_gemm<192, false>(q, d, st);
-  return launch_gemm<128, false>(q, d, st);
+  d.splits = splits;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (bn == 256) return launch_gemm<256>(q, d, st);
+  if (bn == 192) return launch_gemm<192>(q, d, st);
+  return launch_gemm<128>(q, d, st);
 }
 
 extern "C" int vt_reduce_rows(const vt_reduce_params* p, void* stream) {

@@ -1,6 +1,6 @@
 // Remainder rows of a GEMM.  M = 12 552 (8 x 1569 tokens: TimeSformer's FFN, MViT's third stage), 50 184 and 200 712 (MViT
 // stages 2 and 1) are all 8 rows past a multiple of 128, and those 8 rows cost a whole extra row of 128-row tiles — for
-// N = 768 that is 297 tiles instead of 294 = a third round on 148 SMs for 0.06 % of the work.  vt_gemm therefore runs the
+// N = 768 that is 297 tiles instead of 294 for 0.06 % of the work.  vt_gemm therefore runs the
 // tensor-core kernel on the first floor(M / 128) * 128 rows and hands the last <= 16 rows to the kernels below: plain
 // CUDA-core dot products, bandwidth-bound on one pass over the weight matrix (<= 4.7 MB), same epilogue arithmetic
 // (s(m) * (acc + bias[n]) + aux[m, n], bf16 or fp32 out).  Operands are read as stored: B [N, K] ("NT", nn.Linear forward)

@@ -5,7 +5,7 @@
 #include <math.h>
 #include <string.h>
 
-#include "vt_common.cuh"
+#include "vt_attention_mma.cuh"
 
 namespace vt {
 
@@ -1162,12 +1162,6 @@ __global__ void mse_bwd_kernel(const float* __restrict__ pred, const float* __re
   }
 }
 
-bool xattn_tc_supported(const void* q, long long q_bs, long long q_hs, long long q_rs, const void* k, long long k_bs,
-                        long long k_hs, long long k_rs, const void* v, long long v_bs, long long v_hs, long long v_rs, int B,
-                        int H, int Nq, int Nk, int hd);
-int xattn_tc_fwd_launch(const vt_xattn_fwd_params* q, cudaStream_t st);
-int xattn_tc_bwd_launch(const vt_xattn_bwd_params* q, cudaStream_t st);
-
 }  // namespace vt
 
 // ================================================================================================
@@ -1322,6 +1316,20 @@ extern "C" int vt_pool_bwd(const vt_pool_bwd_params* p, void* stream) {
   return vt_reduce_rows(&r3, stream);
 }
 
+// q / k / v / o of either pooling-attention entry point as operands of the tensor-core kernels
+template <typename Params>
+static MmaAttn xattn_operands(const Params* p) {
+  MmaAttn a{};
+  a.q = static_cast<const __nv_bfloat16*>(p->q); a.k = static_cast<const __nv_bfloat16*>(p->k);
+  a.v = static_cast<const __nv_bfloat16*>(p->v); a.o = static_cast<const __nv_bfloat16*>(p->o);
+  a.o_out = static_cast<__nv_bfloat16*>(const_cast<void*>(static_cast<const void*>(p->o)));
+  a.q_bs = p->q_bs; a.q_hs = p->q_hs; a.q_rs = p->q_rs; a.k_bs = p->k_bs; a.k_hs = p->k_hs; a.k_rs = p->k_rs;
+  a.v_bs = p->v_bs; a.v_hs = p->v_hs; a.v_rs = p->v_rs; a.o_bs = p->o_bs; a.o_hs = p->o_hs; a.o_rs = p->o_rs;
+  a.lse = const_cast<float*>(p->lse);
+  a.H = p->H; a.Nq = p->Nq; a.Nk = p->Nk; a.scale = p->scale;
+  return a;
+}
+
 static int xa_strides_ok(const long long* s, int n) {
   for (int i = 0; i < n; ++i)
     if (s[i] % 2 != 0) return 0;
@@ -1333,19 +1341,20 @@ extern "C" int vt_xattn_fwd(const vt_xattn_fwd_params* p, void* stream) {
   VT_REQUIRE(p->hd == 96 || p->hd == 64, "vt_xattn_fwd: head dim %d unsupported (64 or 96)", p->hd);
   VT_REQUIRE(p->B > 0 && p->H > 0 && p->Nq > 0 && p->Nk > 0 && (long long)p->B * p->H <= 65535, "vt_xattn_fwd: bad dims");
   VT_REQUIRE(p->impl >= VT_XATTN_AUTO && p->impl <= VT_XATTN_TCGEN05, "vt_xattn_fwd: bad impl %d", p->impl);
-  if (p->impl == VT_XATTN_TCGEN05 ||
-      (p->impl == VT_XATTN_AUTO && xattn_tc_supported(p->q, p->q_bs, p->q_hs, p->q_rs, p->k, p->k_bs, p->k_hs, p->k_rs, p->v, p->v_bs,
-                                                      p->v_hs, p->v_rs, p->B, p->H, p->Nq, p->Nk, p->hd) &&
-       (p->o_rs * 2) % 16 == 0 && ((uintptr_t)p->o & 15) == 0))
-    return xattn_tc_fwd_launch(p, static_cast<cudaStream_t>(stream));
-  VT_REQUIRE(p->hd == 96, "vt_xattn_fwd: the CUDA-core kernels cover head dim 96 only; head dim %d needs a layout the tcgen05 "
-             "kernels accept (token-major or head-major contiguous, 16-byte aligned rows)", p->hd);
+  const bool tc_ok = mma_layout_ok(p->q, p->q_bs, p->q_hs, p->q_rs, p->hd) && mma_layout_ok(p->k, p->k_bs, p->k_hs, p->k_rs, p->hd) &&
+                     mma_layout_ok(p->v, p->v_bs, p->v_hs, p->v_rs, p->hd) && mma_layout_ok(p->o, p->o_bs, p->o_hs, p->o_rs, p->hd);
+  if (p->impl == VT_XATTN_TCGEN05 || (p->impl == VT_XATTN_AUTO && tc_ok)) {
+    VT_REQUIRE(mma_layout_ok(p->q, p->q_bs, p->q_hs, p->q_rs, p->hd), "vt_xattn_fwd: unsupported q layout for the tensor-core kernel");
+    VT_REQUIRE(tc_ok, "vt_xattn_fwd: unsupported k / v / o layout for the tensor-core kernel");
+    return attn_mma_fwd(xattn_operands(p), p->B, p->hd, static_cast<cudaStream_t>(stream));
+  }
   const long long ss[12] = {p->q_bs, p->q_hs, p->q_rs, p->k_bs, p->k_hs, p->k_rs, p->v_bs, p->v_hs, p->v_rs, p->o_bs, p->o_hs, p->o_rs};
   VT_REQUIRE(xa_strides_ok(ss, 12), "vt_xattn_fwd: strides must be even (4-byte aligned bf16 pairs)");
   VT_REQUIRE(((uintptr_t)p->q | (uintptr_t)p->k | (uintptr_t)p->v | (uintptr_t)p->o) % 4 == 0, "vt_xattn_fwd: pointers must be 4-byte aligned");
   const XaStrides s{p->q_bs, p->q_hs, p->q_rs, p->k_bs, p->k_hs, p->k_rs, p->v_bs, p->v_hs, p->v_rs, p->o_bs, p->o_hs, p->o_rs, 0, 0, 0};
   dim3 grid((p->Nq + XA_QPB - 1) / XA_QPB, p->B * p->H);
-  xattn_fwd_kernel<96><<<grid, 2 * XA_QPB, 0, static_cast<cudaStream_t>(stream)>>>(
+  auto kern = p->hd == 96 ? xattn_fwd_kernel<96> : xattn_fwd_kernel<64>;
+  kern<<<grid, 2 * XA_QPB, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(p->q), static_cast<const __nv_bfloat16*>(p->k), static_cast<const __nv_bfloat16*>(p->v),
       static_cast<__nv_bfloat16*>(p->o), p->lse, s, p->H, p->Nq, p->Nk, p->scale);
   return check_launch("xattn_fwd_kernel");
@@ -1356,13 +1365,20 @@ extern "C" int vt_xattn_bwd(const vt_xattn_bwd_params* p, void* stream) {
   VT_REQUIRE(p->hd == 96 || p->hd == 64, "vt_xattn_bwd: head dim %d unsupported (64 or 96)", p->hd);
   VT_REQUIRE(p->B > 0 && p->H > 0 && p->Nq > 0 && p->Nk > 0 && (long long)p->B * p->H <= 65535, "vt_xattn_bwd: bad dims");
   VT_REQUIRE(p->impl >= VT_XATTN_AUTO && p->impl <= VT_XATTN_TCGEN05, "vt_xattn_bwd: bad impl %d", p->impl);
-  if (p->impl == VT_XATTN_TCGEN05 ||
-      (p->impl == VT_XATTN_AUTO && xattn_tc_supported(p->q, p->q_bs, p->q_hs, p->q_rs, p->k, p->k_bs, p->k_hs, p->k_rs, p->v, p->v_bs,
-                                                      p->v_hs, p->v_rs, p->B, p->H, p->Nq, p->Nk, p->hd) &&
-       (p->o_rs * 2) % 16 == 0 && (p->dq_rs * 2) % 16 == 0 && (p->dq_hs * 2) % 16 == 0 && (p->dq_bs * 2) % 16 == 0 &&
-       (((uintptr_t)p->o | (uintptr_t)p->dout | (uintptr_t)p->dq) & 15) == 0))
-    return xattn_tc_bwd_launch(p, static_cast<cudaStream_t>(stream));
-  VT_REQUIRE(p->hd == 96, "vt_xattn_bwd: the CUDA-core kernels cover head dim 96 only (got %d)", p->hd);
+  const bool tc_ok = mma_layout_ok(p->q, p->q_bs, p->q_hs, p->q_rs, p->hd) && mma_layout_ok(p->k, p->k_bs, p->k_hs, p->k_rs, p->hd) &&
+                     mma_layout_ok(p->v, p->v_bs, p->v_hs, p->v_rs, p->hd) && mma_layout_ok(p->o, p->o_bs, p->o_hs, p->o_rs, p->hd) &&
+                     mma_layout_ok(p->dout, p->o_bs, p->o_hs, p->o_rs, p->hd) && mma_layout_ok(p->dq, p->dq_bs, p->dq_hs, p->dq_rs, p->hd);
+  if (p->impl == VT_XATTN_TCGEN05 || (p->impl == VT_XATTN_AUTO && tc_ok)) {
+    VT_REQUIRE(mma_layout_ok(p->q, p->q_bs, p->q_hs, p->q_rs, p->hd), "vt_xattn_bwd: unsupported q layout for the tensor-core kernel");
+    VT_REQUIRE(tc_ok, "vt_xattn_bwd: unsupported k / v / o / dout / dq layout for the tensor-core kernel");
+    MmaAttn a = xattn_operands(p);
+    a.dout = static_cast<const __nv_bfloat16*>(p->dout);
+    a.delta = p->delta;
+    a.dq = static_cast<__nv_bfloat16*>(p->dq);
+    a.dq_bs = p->dq_bs; a.dq_hs = p->dq_hs; a.dq_rs = p->dq_rs;
+    a.dk32 = p->dk; a.dv32 = p->dv;
+    return attn_mma_bwd(a, p->B, p->hd, static_cast<cudaStream_t>(stream));
+  }
   const long long ss[15] = {p->q_bs, p->q_hs, p->q_rs, p->k_bs, p->k_hs, p->k_rs, p->v_bs, p->v_hs, p->v_rs, p->o_bs, p->o_hs, p->o_rs,
                             p->dq_bs, p->dq_hs, p->dq_rs};
   VT_REQUIRE(xa_strides_ok(ss, 15), "vt_xattn_bwd: strides must be even");
@@ -1377,7 +1393,8 @@ extern "C" int vt_xattn_bwd(const vt_xattn_bwd_params* p, void* stream) {
   e = cudaMemsetAsync(p->dv, 0, kv_bytes, st);
   VT_REQUIRE(e == cudaSuccess, "vt_xattn_bwd: memset dv: %s", cudaGetErrorString(e));
   dim3 gq((p->Nq + XA_QPB - 1) / XA_QPB, p->B * p->H);
-  xattn_dq_kernel<96><<<gq, 2 * XA_QPB, 0, st>>>(
+  auto dq_kern = p->hd == 96 ? xattn_dq_kernel<96> : xattn_dq_kernel<64>;
+  dq_kern<<<gq, 2 * XA_QPB, 0, st>>>(
       static_cast<const __nv_bfloat16*>(p->q), static_cast<const __nv_bfloat16*>(p->k), static_cast<const __nv_bfloat16*>(p->v),
       static_cast<const __nv_bfloat16*>(p->o), static_cast<const __nv_bfloat16*>(p->dout), p->lse, p->delta,
       static_cast<__nv_bfloat16*>(p->dq), s, p->H, p->Nq, p->Nk, p->scale);
@@ -1386,7 +1403,8 @@ extern "C" int vt_xattn_bwd(const vt_xattn_bwd_params* p, void* stream) {
   const int qchunks = (p->Nq + XA_QCHUNK - 1) / XA_QCHUNK;
   VT_REQUIRE(qchunks <= 65535, "vt_xattn_bwd: Nq too large");
   dim3 gk((p->Nk + XA_KPB - 1) / XA_KPB, qchunks, p->B * p->H);
-  xattn_dkv_kernel<96><<<gk, 4 * XA_KPB, 0, st>>>(
+  auto dkv_kern = p->hd == 96 ? xattn_dkv_kernel<96> : xattn_dkv_kernel<64>;
+  dkv_kern<<<gk, 4 * XA_KPB, 0, st>>>(
       static_cast<const __nv_bfloat16*>(p->q), static_cast<const __nv_bfloat16*>(p->k), static_cast<const __nv_bfloat16*>(p->v),
       static_cast<const __nv_bfloat16*>(p->dout), p->lse, p->delta, p->dk, p->dv, s, p->H, p->Nq, p->Nk, p->scale);
   return check_launch("xattn_dkv_kernel");

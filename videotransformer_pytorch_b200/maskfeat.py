@@ -1,4 +1,4 @@
-"""MaskFeat (MViT-B encoder + HOG-regression head) on the sm_100a kernels, behind the reference's module surface.
+"""MaskFeat (MViT-B encoder + HOG-regression head) on the sm_90a kernels, behind the reference's module surface.
 
 Mirrors (reference file:line):
   MaskFeat                          video_transformer.py:803-922   (ctor kwargs, forward, forward_features)

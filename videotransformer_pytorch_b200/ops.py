@@ -16,7 +16,7 @@ Data layout: the residual stream stays fp32 `[B, 1+P*T, D]` exactly as in the re
 n = 1 + p*T + t).  The einops regroupings ('b (p t) d -> (b p) t d', '-> (b t) p d', cls replication /
 mean) never materialise: LayerNorm reads rows through an index map and the last GEMM of each
 sub-block scatters rows back through the inverse map while adding the residual.  GEMM operands are
-bf16 (fp32 accumulation in TMEM); weights are bf16 shadows of the fp32 nn.Parameters.
+bf16 (fp32 accumulation); weights are bf16 shadows of the fp32 nn.Parameters.
 """
 from __future__ import annotations
 
@@ -170,7 +170,7 @@ def _dgrad(dout, w, m_tok, k_in, n_out, **kw):
     return K().gemm(dout, w, m_tok, k_in, n_out, b_mn=True, **kw)
 
 
-ATTN_SINGLE_PASS_MAX = 256      # vt_attn_*: whole score row in TMEM / registers; longer sequences stream K/V (vt_xattn_*)
+ATTN_SINGLE_PASS_MAX = 256      # vt_attn_*: single-pass kernels; longer sequences go to the streaming vt_xattn_* kernels
 
 
 def _packed_heads(qkv, Bp, N, H, hd):
@@ -180,7 +180,7 @@ def _packed_heads(qkv, Bp, N, H, hd):
 
 
 def _streaming_attn_bwd(k, qkv, cx, dcx, lse, Bp, N, H, hd):
-    """dqkv of a long-sequence attention through the streaming tcgen05 kernels (q/k/v and dq in place in the packed layout)."""
+    """dqkv of a long-sequence attention through the streaming tensor-core kernels (q/k/v and dq in place in the packed layout)."""
     q4, k4, v4 = _packed_heads(qkv, Bp, N, H, hd)
     dqkv = torch.empty_like(qkv)
     dq4, dk4, dv4 = _packed_heads(dqkv, Bp, N, H, hd)
@@ -362,7 +362,7 @@ class JointAttnFn(torch.autograd.Function):
         if N <= ATTN_SINGLE_PASS_MAX:
             cx, lse, _ = k.attn_fwd(qkv, Bp, N, H, hd, hd ** -0.5)
         else:
-            # long sequences (joint space-time attention: 1 + P*T = 1569 tokens): streaming tcgen05 kernel, q/k/v read in
+            # long sequences (joint space-time attention: 1 + P*T = 1569 tokens): streaming tensor-core kernel, q/k/v read in
             # place from the packed projection
             q4, k4, v4 = _packed_heads(qkv, Bp, N, H, hd)
             cx, lse = k.xattn_fwd(q4, k4, v4, hd ** -0.5)
@@ -581,7 +581,7 @@ class AttentionCoreFn(torch.autograd.Function):
         if N <= ATTN_SINGLE_PASS_MAX:
             cx, lse, probs = k.attn_fwd(qkv, Bp, N, H, hd, hd ** -0.5, want_probs=want_probs)
         else:
-            # long sequences (joint space-time: 1569 tokens): context by the streaming tcgen05 kernel; the probability
+            # long sequences (joint space-time: 1569 tokens): context by the streaming tensor-core kernel; the probability
             # maps the reference returns (transformer.py:171-177) by a row-tile softmax kernel, 8 query rows per CTA
             q4, k4, v4 = _packed_heads(qkv, Bp, N, H, hd)
             cx, lse = k.xattn_fwd(q4, k4, v4, hd ** -0.5)

@@ -1,4 +1,4 @@
-"""Fused gradient clipping + optimizer step on the sm_100a kernels (SURVEY §8f rank 1).
+"""Fused gradient clipping + optimizer step on the sm_90a kernels (SURVEY §8f rank 1).
 
 Drop-in for the two optimizers the reference builds (optimizer.py:33-38) and for `VideoTransformer.clip_gradients`
 (model_trainer.py:155-170):

@@ -1,4 +1,4 @@
-"""`import transformer` of the reference (model_trainer.py:17, video_transformer.py:8-10) -> the B200 modules."""
+"""`import transformer` of the reference (model_trainer.py:17, video_transformer.py:8-10) -> this package's modules."""
 from videotransformer_pytorch_b200.transformer import *  # noqa: F401,F403
 from videotransformer_pytorch_b200.transformer import (Attention, BasicTransformerBlock, ClassificationHead,  # noqa: F401
                                                        DividedSpatialAttentionWithPreNorm,

@@ -1,7 +1,7 @@
 """nn.Module surface of the transformer building blocks — same class names, constructor arguments,
 parameter names/shapes and forward signatures as the reference's transformer.py, so state dicts
 round-trip with strict=True and model_trainer.py / optimizer.py / weight_init.py drive them unchanged.
-Every forward is routed to the sm_100a kernels through ops.py; there is no eager/CPU fallback.
+Every forward is routed to the sm_90a kernels through ops.py; there is no eager/CPU fallback.
 
 Reference classes mirrored (file:line in the reference repo):
   DropPath :25, ClassificationHead :45, PatchEmbed :83, Attention :153,
@@ -149,7 +149,7 @@ class ClassificationHead(nn.Module):
 
 
 class PatchEmbed(nn.Module):
-    """Non-overlapping patch (Conv2d) / tubelet (Conv3d) projection == im2col + tcgen05 GEMM.
+    """Non-overlapping patch (Conv2d) / tubelet (Conv3d) projection == im2col + wgmma GEMM.
     Stand-alone forward returns ((b t'), (h w), D) like the reference; the models call
     ops.PatchTokensFn, which fuses the positional/temporal embedding and the token regroup."""
 

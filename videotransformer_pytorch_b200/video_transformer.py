@@ -1,9 +1,9 @@
 """Model surface: TimeSformer and ViViT with the reference's constructor signatures, attribute names
 and state-dict keys (reference video_transformer.py:20-268 and :270-557), forward/backward on the
-sm_100a kernels.
+sm_90a kernels.
 
 Covered configurations (SURVEY.md §8a, §8f rank 4): TimeSformer `divided_space_time`, `space_only` (197-token joint
-attention per frame) and `joint_space_time` (one 1569-token attention per clip, streaming tcgen05 kernel); ViViT
+attention per frame) and `joint_space_time` (one 1569-token attention per clip, streaming tensor-core kernel); ViViT
 `fact_encoder` (model 2), `joint_space_time` (model 1) and `divided_space_time` (model 3).  Nothing falls back to eager
 PyTorch.
 """
