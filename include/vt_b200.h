@@ -32,8 +32,8 @@ int vt_version(void);
 int vt_last_error(char* buf, size_t buf_bytes);
 /* number of SMs of the current device (grid sizing is done inside the library) */
 int vt_sm_count(void);
-/* plan GEMM tile counts (wave quantisation, split-K) for vt_sm_count() - n SMs; 0 restores the default.  The GEMM runs one
- * CTA per tile, not persistent CTAs, so this does not keep SMs free for concurrent kernels (NCCL) */
+/* run the persistent GEMM on vt_sm_count() - n SMs (grid size, tile shape and split-K planned for that many); 0 restores the
+ * default.  The other n SMs stay free for concurrent kernels (the NCCL all-reduce overlapped with the backward) */
 int vt_set_reserved_sms(int n);
 /* number of kernels this library has launched in this process (mod 2^31); bench.py's gpu_launches */
 int vt_launch_count(void);

@@ -1,0 +1,129 @@
+"""Time every distinct GEMM of the TimeSformer-B step (8 frames of 224^2, batch 8) stand-alone on the GPU.
+
+    python tools/gemm_shapes.py [--reps 50] [--warmup 10] [--json OUT]
+
+For each GEMM it runs vt_gemm with the layouts and epilogue the model uses, under the planner's choice and with each
+tile width forced, and prints TFLOP/s, HBM GB/s (bytes the epilogue and operands must move at least once) and the time
+over the larger of the two data-sheet floors (989 TFLOP/s dense BF16, 3.35 TB/s HBM3, H100 SXM at 700 W).  For the plain
+shapes it times torch.matmul (cuBLAS, bf16) as well: the rate this card reaches at its power limit.  The card's name,
+power limit and SM clocks are read with read-only nvidia-smi queries and printed with the numbers.  Needs a CUDA device;
+there is no CPU path.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+import torch
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+PEAK_TFLOPS, PEAK_TBS = 989.0, 3.35
+B, T, P, D, HID = 8, 8, 196, 768, 3072
+S = 1 + P * T
+M_TOK, M_TEMP, M_SPAT = B * S, B * P * T, B * T * (P + 1)     # 12552, 12544, 12608
+
+
+def card():
+    q = 'name,power.limit,clocks.sm,clocks.max.sm'
+    try:
+        out = subprocess.run(['nvidia-smi', '-i', '0', f'--query-gpu={q}', '--format=csv,noheader'], capture_output=True,
+                             text=True, timeout=30).stdout.strip()
+    except Exception as exc:
+        out = f'nvidia-smi unavailable ({exc})'
+    return dict(zip(q.split(','), [v.strip() for v in out.split(',')])) if out.count(',') == 3 else {'nvidia-smi': out}
+
+
+def events_ms(fn, reps, warmup):
+    for _ in range(warmup):
+        fn()
+    torch.cuda.synchronize()
+    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    t0.record()
+    for _ in range(reps):
+        fn()
+    t1.record()
+    torch.cuda.synchronize()
+    return t0.elapsed_time(t1) / reps
+
+
+def cases(dev):
+    """(name, M, N, K, layouts, kwargs for K.gemm, epilogue bytes per output element, plain)"""
+    from videotransformer_pytorch_b200 import ops
+    maps = ops.token_maps(B, T, P, dev)
+    aff = ops.affine_row_maps(B, T, P, D)
+    bias_d, bias_3d, bias_h = (torch.randn(n, device=dev) for n in (D, 3 * D, HID))
+    stream = torch.randn(B * S + B * T, D, device=dev)
+    z = torch.randn(M_TOK, HID, device=dev).bfloat16()
+    out = [
+        ('qkv fwd temporal', M_TEMP, 3 * D, D, (0, 0), dict(epi='bf16', bias=bias_3d), 2, True),
+        ('qkv fwd spatial', M_SPAT, 3 * D, D, (0, 0), dict(epi='bf16', bias=bias_3d), 2, True),
+        ('proj fwd temporal (affine)', M_TEMP, D, D, (0, 0),
+         dict(epi='f32', bias=bias_d, bias2=bias_d, aux=stream, out=stream, aux_row=maps['temporal'], out_row=maps['temporal'],
+              row_map=aff['temporal']), 8, False),
+        ('proj fwd spatial (affine, cls rows)', M_SPAT, D, D, (0, 0),
+         dict(epi='f32', bias=bias_d, aux=stream, out=stream, aux_row=maps['sp_aux'], out_row=maps['sp_out'],
+              row_map=aff['spatial']), 8, False),
+        ('fc1 fwd (gelu)', M_TOK, HID, D, (0, 0), dict(epi='gelu', bias=bias_h), 4, False),
+        ('fc2 fwd (f32 residual)', M_TOK, D, HID, (0, 0), dict(epi='f32', bias=bias_d, aux=stream[:M_TOK]), 8, False),
+        ('fc2 dgrad (dgelu)', M_TOK, HID, D, (0, 1), dict(epi='dgelu', aux=z), 4, False),
+        ('fc1 dgrad', M_TOK, D, HID, (0, 1), dict(epi='bf16'), 2, True),
+        ('proj dgrad', M_TEMP, D, D, (0, 1), dict(epi='bf16'), 2, True),
+        ('qkv dgrad', M_TEMP, D, 3 * D, (0, 1), dict(epi='bf16'), 2, True),
+        ('qkv wgrad', 3 * D, D, M_TEMP, (1, 1), dict(epi='f32', split_ok=True), 4, True),
+        ('proj wgrad', D, D, M_TEMP, (1, 1), dict(epi='f32', split_ok=True), 4, True),
+        ('fc1 wgrad', HID, D, M_TOK, (1, 1), dict(epi='f32', split_ok=True), 4, True),
+        ('fc2 wgrad', D, HID, M_TOK, (1, 1), dict(epi='f32', split_ok=True), 4, True),
+    ]
+    return out
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
+    ap.add_argument('--reps', type=int, default=50)
+    ap.add_argument('--warmup', type=int, default=10)
+    ap.add_argument('--json', default=None, help='also write the rows as JSON to this file')
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        sys.exit('gemm_shapes: no CUDA device; these are GPU timings and there is no CPU fallback')
+    from videotransformer_pytorch_b200 import _lib
+    K = _lib.K
+    dev = 'cuda:0'
+    torch.manual_seed(0)
+    info = card()
+    print(json.dumps({'card': info, 'sms': _lib.load_library().vt_sm_count()}))
+    rows = []
+    hdr = f'{"gemm":38s} {"M":>6s} {"N":>5s} {"K":>6s} {"tile":>5s} {"us":>8s} {"TFLOP/s":>8s} {"GB/s":>7s} {"x floor":>7s}'
+    print(hdr)
+    for name, M, N, Kd, (a_mn, b_mn), kw, epi_b, plain in cases(dev):
+        a = (torch.randn(Kd, M, device=dev) if a_mn else torch.randn(M, Kd, device=dev)).mul_(0.1).bfloat16()
+        b = (torch.randn(Kd, N, device=dev) if b_mn else torch.randn(N, Kd, device=dev)).mul_(0.1).bfloat16()
+        flop = 2.0 * M * N * Kd
+        byts = 2.0 * (M * Kd + N * Kd) + epi_b * M * N
+        floor_us = max(flop / (PEAK_TFLOPS * 1e12), byts / (PEAK_TBS * 1e12)) * 1e6
+        for bn in (0, 128, 192, 256):
+            us = 1e3 * events_ms(lambda: K.gemm(a, b, M, N, Kd, a_mn=bool(a_mn), b_mn=bool(b_mn), force_bn=bn, **kw),
+                                 args.reps, args.warmup)
+            r = dict(gemm=name, M=M, N=N, K=Kd, tile=bn or 'auto', us=us, tflops=flop / us * 1e-6, gbs=byts / us * 1e-3,
+                     over_floor=us / floor_us)
+            rows.append(r)
+            print(f'{name:38s} {M:6d} {N:5d} {Kd:6d} {str(r["tile"]):>5s} {us:8.1f} {r["tflops"]:8.1f} {r["gbs"]:7.0f} '
+                  f'{r["over_floor"]:7.2f}')
+        if plain:
+            A = a.t() if a_mn else a
+            Bm = b if b_mn else b.t()
+            us = 1e3 * events_ms(lambda: torch.matmul(A, Bm), args.reps, args.warmup)
+            r = dict(gemm=name, M=M, N=N, K=Kd, tile='cublas', us=us, tflops=flop / us * 1e-6, gbs=None,
+                     over_floor=us / floor_us)
+            rows.append(r)
+            print(f'{name:38s} {M:6d} {N:5d} {Kd:6d} {"cublas":>5s} {us:8.1f} {r["tflops"]:8.1f} {"":>7s} {r["over_floor"]:7.2f}')
+    print(json.dumps({'card_after': card()}))
+    if args.json:
+        with open(args.json, 'w') as fh:
+            json.dump({'card': info, 'rows': rows}, fh, indent=1)
+
+
+if __name__ == '__main__':
+    main()

@@ -1001,7 +1001,7 @@ class CudaKernels:
 
 
 def set_reserved_sms(n: int) -> None:
-    """Plan GEMM tile counts for vt_sm_count() - n SMs (no SMs are kept free); see vt_set_reserved_sms."""
+    """Run the persistent GEMM on vt_sm_count() - n SMs, keeping n SMs free; see vt_set_reserved_sms."""
     _check(load_library().vt_set_reserved_sms(int(n)), 'vt_set_reserved_sms')
 
 

@@ -1,10 +1,12 @@
-// Warp-specialised bf16 GEMM for sm_90a:
+// Warp-specialised, persistent bf16 GEMM for sm_90a:
 //   TMA (cp.async.bulk.tensor, 128B swizzle) -> shared-memory ring (mbarrier full / empty pairs) -> wgmma.mma_async
 //   (fp32 accumulators in registers) -> epilogue fused with bias / GELU / dGELU / residual / row maps, straight from
 //   the accumulator registers to global memory.
-// One CTA per 128 x BN output tile (x K split), 384 threads: warpgroup 0 = TMA producer (one thread), warpgroups 1-2 =
-// consumers, each owning 64 rows of the tile.  BN in {128, 192, 256}.  Both operands may be K-major or MN-major (wgmma
-// transpose bits), so forward (X W^T), dgrad (dY W) and wgrad (dY^T X) all run without transposed copies.
+// Persistent: one CTA per SM walks a static sequence of 128 x BN output tiles (x K split), BN in {128, 192, 256}.  384
+// threads: warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = consumers, each owning 64 rows of every tile.  The
+// producer runs ahead across tile boundaries, so the next tile's first k-blocks load while the consumers run the epilogue.
+// Both operands may be K-major or MN-major (wgmma transpose bits), so forward (X W^T), dgrad (dY W) and wgrad (dY^T X) all
+// run without transposed copies.
 #include <stdlib.h>
 #include <string.h>
 
@@ -21,6 +23,7 @@ constexpr int CHUNK_BYTES = 64 * BK * 2;  // one 64-wide MN chunk of an MN-major
 struct GemmDev {
   int M, N, K;
   int kblocks, splits;
+  int num_m, num_n, tiles;   // tiles = num_m x num_n x splits
   int epi;
   const float* bias;
   const float* bias2;      // VT_EPI_F32 with aux only: second bias, added to the addend
@@ -128,25 +131,44 @@ __device__ __forceinline__ void epi_pair(const GemmDev& p, const EpiRow& r, int 
   }
 }
 
-// grid (n tiles, m tiles, K splits); n fastest so that CTAs running together share the A row-block in L2
+// Tile t of the persistent walk: n fastest, then m, then the K split, so the tiles the CTAs run at one time share A
+// row-blocks in L2.
+struct Tile {
+  int m0, n0, split, kb0, kb1;
+};
+
+template <int BN>
+__device__ __forceinline__ Tile tile_at(const GemmDev& p, int t) {
+  Tile c;
+  const int nt = t % p.num_n, rest = t / p.num_n;
+  const int mt = rest % p.num_m;
+  c.split = rest / p.num_m;
+  c.m0 = mt * BM;
+  c.n0 = nt * BN;
+  c.kb0 = (int)(((long long)p.kblocks * c.split) / p.splits);
+  c.kb1 = (int)(((long long)p.kblocks * (c.split + 1)) / p.splits);
+  return c;
+}
+
+// min(tiles, SMs) CTAs; CTA b runs tiles b, b + gridDim.x, ...  The producer thread streams every tile's k-blocks
+// through one shared-memory ring whose stage / phase count runs on across tiles, so barrier set-up, register hand-over and
+// the tensor-map prefetch happen once per CTA and the ring refills during each epilogue.  The walk is static: a tile's
+// result depends only on the tile, not on the grid size.
 template <int BN, int TA, int TB>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmDev p) {
   using Cfg = GemmCfg<BN>;
+  constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + Cfg::STAGES;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
+  uint64_t* empty_bar = full_bar + STAGES;
 
   const int wg = threadIdx.x >> 7;
-  const int n0 = blockIdx.x * BN, m0 = blockIdx.y * BM, split = blockIdx.z;
-  const int kb0 = (int)(((long long)p.kblocks * split) / p.splits);
-  const int kb1 = (int)(((long long)p.kblocks * (split + 1)) / p.splits);
-
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    for (int i = 0; i < Cfg::STAGES; ++i) {
+    for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 8);   // one arrive per consumer warp
     }
@@ -157,65 +179,73 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (wg == 0) {
     setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
-      int stage = 0, phase = 0;
-      for (int kb = kb0; kb < kb1; ++kb) {
-        mbar_wait(&empty_bar[stage], phase ^ 1);
-        uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
-        uint8_t* sB = sA + Cfg::A_BYTES;
-        mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-        if (!TA) {
-          tma_load_2d(sA, &tmA, &full_bar[stage], kb * BK, m0);
-        } else {
+      uint32_t it = 0;   // ring position: k-blocks loaded so far by this CTA
+      for (int t = blockIdx.x; t < p.tiles; t += gridDim.x) {
+        const Tile c = tile_at<BN>(p, t);
+        for (int kb = c.kb0; kb < c.kb1; ++kb, ++it) {
+          const int stage = (int)(it % STAGES);
+          mbar_wait(&empty_bar[stage], ((it / STAGES) & 1) ^ 1);
+          uint8_t* sA = smem + stage * Cfg::STAGE_BYTES;
+          uint8_t* sB = sA + Cfg::A_BYTES;
+          mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+          if (!TA) {
+            tma_load_2d(sA, &tmA, &full_bar[stage], kb * BK, c.m0);
+          } else {
 #pragma unroll
-          for (int c = 0; c < BM / 64; ++c) tma_load_2d(sA + c * CHUNK_BYTES, &tmA, &full_bar[stage], m0 + c * 64, kb * BK);
-        }
-        if (!TB) {
-          tma_load_2d(sB, &tmB, &full_bar[stage], kb * BK, n0);
-        } else {
+            for (int ch = 0; ch < BM / 64; ++ch) tma_load_2d(sA + ch * CHUNK_BYTES, &tmA, &full_bar[stage], c.m0 + ch * 64, kb * BK);
+          }
+          if (!TB) {
+            tma_load_2d(sB, &tmB, &full_bar[stage], kb * BK, c.n0);
+          } else {
 #pragma unroll
-          for (int c = 0; c < BN / 64; ++c) tma_load_2d(sB + c * CHUNK_BYTES, &tmB, &full_bar[stage], n0 + c * 64, kb * BK);
+            for (int ch = 0; ch < BN / 64; ++ch) tma_load_2d(sB + ch * CHUNK_BYTES, &tmB, &full_bar[stage], c.n0 + ch * 64, kb * BK);
+          }
         }
-        if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
       }
     }
     return;
   }
 
   setmaxnreg_inc<232>();
-  const int cw = wg - 1;                       // consumer: rows [64 cw, 64 cw + 64) of the tile
+  const int cw = wg - 1;                       // consumer: rows [64 cw, 64 cw + 64) of every tile
   const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
-  float acc[BN / 2];
+  uint32_t it = 0;
+  for (int t = blockIdx.x; t < p.tiles; t += gridDim.x) {
+    const Tile c = tile_at<BN>(p, t);
+    float acc[BN / 2];
 #pragma unroll
-  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-  int stage = 0, phase = 0, prev = -1;
-  for (int kb = kb0; kb < kb1; ++kb) {
-    mbar_wait(&full_bar[stage], phase);
-    const uint32_t a_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES) + cw * (TA ? CHUNK_BYTES : 64 * 128);
-    const uint32_t b_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES);
-    wgmma_fence();
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int prev = -1;
+    for (int kb = c.kb0; kb < c.kb1; ++kb, ++it) {
+      const int stage = (int)(it % STAGES);
+      mbar_wait(&full_bar[stage], (it / STAGES) & 1);
+      const uint32_t a_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES) + cw * (TA ? CHUNK_BYTES : 64 * 128);
+      const uint32_t b_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES);
+      wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < BK / 16; ++k) {
-      const uint64_t da = TA ? sdesc_mnmajor(a_addr + k * 2048, CHUNK_BYTES) : sdesc_kmajor(a_addr + k * 32);
-      const uint64_t db = TB ? sdesc_mnmajor(b_addr + k * 2048, CHUNK_BYTES) : sdesc_kmajor(b_addr + k * 32);
-      wgmma_tile<BN, TA, TB>(acc, da, db, (kb > kb0 || k > 0) ? 1u : 0u);
+      for (int k = 0; k < BK / 16; ++k) {
+        const uint64_t da = TA ? sdesc_mnmajor(a_addr + k * 2048, CHUNK_BYTES) : sdesc_kmajor(a_addr + k * 32);
+        const uint64_t db = TB ? sdesc_mnmajor(b_addr + k * 2048, CHUNK_BYTES) : sdesc_kmajor(b_addr + k * 32);
+        wgmma_tile<BN, TA, TB>(acc, da, db, (kb > c.kb0 || k > 0) ? 1u : 0u);
+      }
+      wgmma_commit();
+      // the previous k-block's MMAs have retired once at most this one is in flight: its stage is free
+      wgmma_wait<1>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
     }
-    wgmma_commit();
-    // the previous k-block's MMAs have retired once at most this one is in flight: its stage is free
-    wgmma_wait<1>();
-    if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-    prev = stage;
-    if (++stage == Cfg::STAGES) { stage = 0; phase ^= 1; }
-  }
-  wgmma_wait<0>();
+    wgmma_wait<0>();
+    if (lane == 0) mbar_arrive(&empty_bar[prev]);   // the producer is already filling the ring for the next tile
 
-  const int r0 = m0 + cw * 64 + warp * 16 + (lane >> 2);
-  const EpiRow e0 = epi_row(p, r0, split), e1 = epi_row(p, r0 + 8, split);
+    const int r0 = c.m0 + cw * 64 + warp * 16 + (lane >> 2);
+    const EpiRow e0 = epi_row(p, r0, c.split), e1 = epi_row(p, r0 + 8, c.split);
 #pragma unroll
-  for (int j = 0; j < BN / 8; ++j) {
-    const int n = n0 + 8 * j + 2 * (lane & 3);
-    if (n >= p.N) break;
-    epi_pair(p, e0, n, acc[4 * j], acc[4 * j + 1]);
-    epi_pair(p, e1, n, acc[4 * j + 2], acc[4 * j + 3]);
+    for (int j = 0; j < BN / 8; ++j) {
+      const int n = c.n0 + 8 * j + 2 * (lane & 3);
+      if (n >= p.N) break;
+      epi_pair(p, e0, n, acc[4 * j], acc[4 * j + 1]);
+      epi_pair(p, e1, n, acc[4 * j + 2], acc[4 * j + 3]);
+    }
   }
 }
 
@@ -329,7 +359,7 @@ int launch_reduce_rows(const float* in, float* out, long long stride, int S, lon
 }
 
 template <int BN, int TA, int TB>
-static int launch_gemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& d, int num_m, cudaStream_t st) {
+static int launch_gemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& d, cudaStream_t st) {
   using Cfg = GemmCfg<BN>;
   static bool attr_set = false;  // benign race: idempotent
   if (!attr_set) {
@@ -337,7 +367,7 @@ static int launch_gemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const G
     VT_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(smem=%d) failed: %s", Cfg::SMEM_BYTES, cudaGetErrorString(e));
     attr_set = true;
   }
-  const dim3 grid((unsigned)((d.N + BN - 1) / BN), (unsigned)num_m, (unsigned)d.splits);
+  const int grid = d.tiles < persistent_sm_count() ? d.tiles : persistent_sm_count();
   gemm_wgmma_kernel<BN, TA, TB><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(tmA, tmB, d);
   return check_launch("gemm_wgmma_kernel");
 }
@@ -352,8 +382,11 @@ static int launch_gemm(const vt_gemm_params* q, GemmDev& d, cudaStream_t st) {
   if (!q->b_mn_major) rc = make_tmap_bf16_2d(&tmB, q->b, q->N, q->K, q->ldb, BN);
   else rc = make_tmap_bf16_2d(&tmB, q->b, q->K, q->N, q->ldb, BK);
   if (rc) return rc;
-  const int num_m = (q->M + BM - 1) / BM;
-  VT_REQUIRE(num_m <= 65535, "vt_gemm: M=%d too large", q->M);
+  d.num_m = (q->M + BM - 1) / BM;
+  d.num_n = (q->N + BN - 1) / BN;
+  const long long tiles = (long long)d.num_m * d.num_n * d.splits;
+  VT_REQUIRE(tiles < (1LL << 31), "vt_gemm: M=%d N=%d gives too many tiles", q->M, q->N);
+  d.tiles = (int)tiles;
   const long long tile_out = (long long)q->M * q->N;
   void* final_out = d.out;
   d.split_stride = 0;
@@ -362,10 +395,10 @@ static int launch_gemm(const vt_gemm_params* q, GemmDev& d, cudaStream_t st) {
     d.ldo = q->N;
     d.split_stride = tile_out;
   }
-  if (!q->a_mn_major && !q->b_mn_major) rc = launch_gemm_t<BN, 0, 0>(tmA, tmB, d, num_m, st);
-  else if (!q->a_mn_major) rc = launch_gemm_t<BN, 0, 1>(tmA, tmB, d, num_m, st);
-  else if (!q->b_mn_major) rc = launch_gemm_t<BN, 1, 0>(tmA, tmB, d, num_m, st);
-  else rc = launch_gemm_t<BN, 1, 1>(tmA, tmB, d, num_m, st);
+  if (!q->a_mn_major && !q->b_mn_major) rc = launch_gemm_t<BN, 0, 0>(tmA, tmB, d, st);
+  else if (!q->a_mn_major) rc = launch_gemm_t<BN, 0, 1>(tmA, tmB, d, st);
+  else if (!q->b_mn_major) rc = launch_gemm_t<BN, 1, 0>(tmA, tmB, d, st);
+  else rc = launch_gemm_t<BN, 1, 1>(tmA, tmB, d, st);
   if (rc) return rc;
   if (d.splits > 1) {
     VT_REQUIRE(q->ldo == q->N, "vt_gemm: split-K requires ldo == N");
@@ -382,7 +415,7 @@ int launch_gemm_rows(const vt_gemm_params* q, int m0, void* stream);   // vt_gem
 // M a few rows past a multiple of 128: tensor-core kernel on the full row tiles, CUDA-core dot products for the rest
 // (vt_gemm_rows.cu).  Plain row-major calls only; anything forced by a test goes through the one-kernel path.
 #ifndef VT_DEFAULT_ROWS_SPLIT
-#define VT_DEFAULT_ROWS_SPLIT true
+#define VT_DEFAULT_ROWS_SPLIT false   // off: with persistent CTAs the 8-row tail tile costs less than the extra launch
 #endif
 static int rows_split_point(const vt_gemm_params* q) {
   const int r = q->M % vt::BM;
@@ -459,9 +492,13 @@ static int gemm_dispatch(const vt_gemm_params* q, void* stream) {
     d.special_ld = q->map_special_stride;
   }
 
-  // Wave-quantisation aware configuration: cost ~ waves over the SMs x per-tile time, where a tile (x K split) costs
-  // (its k-blocks + a fixed prologue/epilogue overhead) x BN, with a small penalty for narrower tiles (they re-read A
-  // more often).  Splitting K is only possible for plain fp32 outputs with a workspace (weight gradients).
+  // Cost ~ tiles per CTA of the persistent grid (ceil(tiles / SMs)) x per-tile time, where a tile (x K split) costs (its
+  // k-blocks + a fixed epilogue overhead) x BN, with a small penalty for narrower tiles (they re-read A more often).
+  // Splitting K is only possible for plain fp32 outputs with a workspace (weight gradients).
+  // Short-K GEMMs without a split (K <= 1024: qkv, FC1 forward, FC2 data gradient, out-proj) take the 128-wide tile, which
+  // the model undervalues: measured on an H100 at B = 8 it is 20-35 % faster than the 256-wide tile on the wide-output
+  // ones (their register epilogue costs about as much as the 12-k-block mainloop) and within 4 % on the others.
+  const bool short_k = d.kblocks <= 16;
   const int sms = persistent_sm_count();
   const int num_m = (q->M + BM - 1) / BM;
   const bool can_split = q->epilogue == VT_EPI_F32 && q->workspace && !q->out_row && !q->aux && !q->row_scale && !q->bias &&
@@ -472,13 +509,14 @@ static int gemm_dispatch(const vt_gemm_params* q, void* stream) {
   int bn = 128, splits = 1;
   for (int i = 0; i < 3; ++i) {
     if (q->force_bn && cand[i] != q->force_bn) continue;
+    if (!q->force_bn && !can_split && short_k && cand[i] != 128) continue;
     const int num_n = (q->N + cand[i] - 1) / cand[i];
     const int smax = can_split ? 16 : 1;
     for (int sp = 1; sp <= smax; ++sp) {
       if (sp > 1 && (d.kblocks / sp < 4 || (long long)sp * q->M * q->N * 4 > q->workspace_bytes)) break;
       const long long tiles = (long long)num_m * num_n * sp;
-      const double waves = (double)((tiles + sms - 1) / sms);
-      const double cost = waves * ((double)d.kblocks / sp + 8.0) * cand[i] * penalty[i];
+      const double per_cta = (double)((tiles + sms - 1) / sms);
+      const double cost = per_cta * ((double)d.kblocks / sp + 8.0) * cand[i] * penalty[i];
       if (cost < best - 1e-9) { best = cost; bn = cand[i]; splits = sp; }
     }
   }
