@@ -95,7 +95,7 @@ XATTN_SHAPES = [(2, 2, 70, 37), (1, 1, 300, 393), (1, 4, 64, 16), (2, 1, 5, 1), 
                 (1, 2, 300, 700), (1, 1, 2300, 200), (3, 2, 128, 128)]
 
 
-@pytest.mark.parametrize('impl', [1, 2], ids=['simt', 'tcgen05'])
+@pytest.mark.parametrize('impl', [1, 2], ids=['simt', 'mma'])
 @pytest.mark.parametrize('B,H,Nq,Nk', XATTN_SHAPES)
 def test_xattn_fwd_bwd(B, H, Nq, Nk, impl):
     d = H * HD

@@ -1,4 +1,5 @@
-"""CPU walk-through of the index arithmetic and tiling of the MViT CUDA kernels (csrc/vt_mvit.cu).
+"""CPU walk-through of the index arithmetic and tiling of the MViT CUDA kernels (csrc/vt_mvit.cu) and of the tensor-core flash
+attention (csrc/vt_attention_mma.cu, modelled in tests/attn_mma_emu.py).
 
 There is no GPU in the build container, so the kernels' *algorithms* — row decoding, gather conditions of the adjoint
 kernels, tile masking, log2-domain softmax bookkeeping — are transcribed loop-for-loop into numpy here and compared
@@ -9,6 +10,7 @@ import numpy as np
 import pytest
 import torch
 
+from tests import attn_mma_emu as AE
 from tests.emu_kernels import EmuKernels
 
 HD = 96
@@ -535,109 +537,131 @@ def test_xattn_tile_algorithm(Nq, Nk):
         assert np.abs(mine - ref).max() < 1e-12 * max(1.0, np.abs(ref).max())
 
 
-# ---- tcgen05 pooling attention (vt_xattention_tc.cu): tile walk, two-warpgroup split + merge, garbage padding ---------
-def sim_xattn_tc_fwd(q, k, v, scale, garbage):
-    """128-query CTA tiles, 128-key tiles taken alternately by two warpgroups with private (m, l, O) states that are merged
-    at the end; rows / columns past Nq / Nk hold `garbage` (what TMA brings in from the neighbouring head or batch) and
-    must not influence the result."""
-    Nq, Nk = q.shape[0], k.shape[0]
-    nqt, nkt = -(-Nq // 128), -(-Nk // 128)
-    qp = np.concatenate([q, garbage((nqt * 128 - Nq, HD))])
-    kp = np.concatenate([k, garbage((nkt * 128 - Nk, HD))])
-    vp = np.concatenate([v, garbage((nkt * 128 - Nk, HD))])
-    sl2 = scale * LOG2E
-    out, lse = np.zeros((Nq, HD)), np.zeros(Nq)
-    for qt in range(nqt):
-        Q = qp[qt * 128:(qt + 1) * 128]
-        state = []
-        for wg in range(2):
-            m, l, acc = np.full(128, -np.inf), np.zeros(128), np.zeros((128, HD))
-            for j in range(wg, nkt, 2):
-                S = Q @ kp[j * 128:(j + 1) * 128].T
-                nvalid = min(128, Nk - j * 128)
-                mx = np.where(np.arange(128)[None, :] < nvalid, S, -np.inf).max(1)
-                mn = np.maximum(m, mx * sl2)
-                corr = np.exp2(m - mn)
-                e = np.where(np.arange(128)[None, :] < nvalid, np.exp2(S * sl2 - mn[:, None]), 0.0)
-                l = l * corr + e.sum(1)
-                acc = acc * corr[:, None] + e @ vp[j * 128:(j + 1) * 128]
-                m = mn
-            state.append((m, l, acc))
-        (m0, l0, a0), (m1, l1, a1) = state
-        mm = np.maximum(m0, m1)
-        f0, f1 = np.exp2(m0 - mm), np.exp2(m1 - mm)              # m1 = -inf when the second group had no tile
-        lt = l0 * f0 + l1 * f1
-        o = (a0 * f0[:, None] + a1 * f1[:, None]) / lt[:, None]
-        n = min(128, Nq - qt * 128)
-        out[qt * 128:qt * 128 + n] = o[:n]
-        lse[qt * 128:qt * 128 + n] = ((mm + np.log2(lt)) * LN2)[:n]
-    return out, lse
+# ---- tensor-core flash attention (vt_attention_mma.cu): the tile walk of tests/attn_mma_emu.py ------------------------
 
-
-def sim_xattn_tc_bwd(q, k, v, o, do, lse, scale, garbage, qtiles_per_chunk=2):
-    Nq, Nk = q.shape[0], k.shape[0]
-    nqt, nkt = -(-Nq // 128), -(-Nk // 128)
-    pad = lambda a, n: np.concatenate([a, garbage((n - a.shape[0], HD))])
-    qp, dop = pad(q, nqt * 128), pad(do, nqt * 128)
-    kp, vp = pad(k, nkt * 128), pad(v, nkt * 128)
-    sl2 = scale * LOG2E
-    lse2 = np.full(nqt * 128, np.inf)
-    lse2[:Nq] = lse * LOG2E                                      # rows past Nq: +inf => P = 0
-    delta = np.zeros(nqt * 128)
-    delta[:Nq] = (do * o).sum(1)
-    kcol = np.arange(128)[None, :]
-    # dQ kernel: one CTA per query tile, key tiles streamed
-    dq = np.zeros((Nq, HD))
-    for qt in range(nqt):
-        rows = slice(qt * 128, (qt + 1) * 128)
-        acc = np.zeros((128, HD))
-        for j in range(nkt):
-            K_, V_ = kp[j * 128:(j + 1) * 128], vp[j * 128:(j + 1) * 128]
-            S, dP = qp[rows] @ K_.T, dop[rows] @ V_.T
-            P = np.where(j * 128 + kcol < Nk, np.exp2(S * sl2 - lse2[rows, None]), 0.0)
-            dS = P * (dP - delta[rows, None]) * scale
-            acc += dS @ K_
-        n = min(128, Nq - qt * 128)
-        dq[qt * 128:qt * 128 + n] = acc[:n]
-    # dK/dV kernel: CTA = key tile x chunk of query tiles, chunks merged by atomics
-    dk, dv = np.zeros((Nk, HD)), np.zeros((Nk, HD))
-    for kt in range(nkt):
-        K_, V_ = kp[kt * 128:(kt + 1) * 128], vp[kt * 128:(kt + 1) * 128]
-        for c0 in range(0, nqt, qtiles_per_chunk):
-            dK, dV = np.zeros((128, HD)), np.zeros((128, HD))
-            for qt in range(c0, min(nqt, c0 + qtiles_per_chunk)):
-                rows = slice(qt * 128, (qt + 1) * 128)
-                S, dP = qp[rows] @ K_.T, dop[rows] @ V_.T
-                P = np.where(kt * 128 + kcol < Nk, np.exp2(S * sl2 - lse2[rows, None]), 0.0)
-                dS = P * (dP - delta[rows, None]) * scale
-                dK += dS.T @ qp[rows]
-                dV += P.T @ dop[rows]
-            n = min(128, Nk - kt * 128)
-            dk[kt * 128:kt * 128 + n] += dK[:n]
-            dv[kt * 128:kt * 128 + n] += dV[:n]
-    return dq, dk, dv
-
-
-@pytest.mark.parametrize('Nq,Nk', [(70, 37), (300, 393), (129, 128), (5, 1), (520, 260)])
-def test_xattn_tensor_core_tile_walk(Nq, Nk):
-    rng = np.random.default_rng(9)
-    garbage = lambda shape: rng.standard_normal(shape) * 7.0      # finite junk in every padded row
-    q, k, v = rng.standard_normal((Nq, HD)), rng.standard_normal((Nk, HD)), rng.standard_normal((Nk, HD))
-    scale = HD ** -0.5
-    s = (q @ k.T) * scale
-    mx = s.max(1, keepdims=True)
-    lse = (mx + np.log(np.exp(s - mx).sum(1, keepdims=True)))[:, 0]
-    p = np.exp(s - lse[:, None])
-    o = p @ v
-    so, slse = sim_xattn_tc_fwd(q, k, v, scale, garbage)
+@pytest.mark.parametrize('hd', [64, 96])
+@pytest.mark.parametrize('Nq,Nk', [(1, 1), (5, 1), (63, 65), (64, 64), (65, 129), (129, 63), (197, 197), (300, 393)])
+def test_attn_mma_model_exact(Nq, Nk, hd):
+    """The model in 'exact' mode (64-row tiles, online softmax in the log2 domain, masking, lse = +inf past Nq in the
+    backward) reproduces closed-form fp64 attention; finite junk in the rows past Nq / Nk (the next problem's rows in memory)
+    must not reach the result."""
+    rng = torch.Generator().manual_seed(9)
+    P, scale = 2, hd ** -0.5
+    pad = lambda x, n: torch.cat([x, torch.randn(P, 64 + 7, hd, generator=rng, dtype=torch.float64) * 7.0], 1)
+    q, k, v, do = (torch.randn(P, n, hd, generator=rng, dtype=torch.float64) for n in (Nq, Nk, Nk, Nq))
+    o, lse, dq, dk, dv = AE.reference(q, k, v, do, scale)
+    so, slse = AE.fwd(pad(q, Nq), pad(k, Nk), pad(v, Nk), scale, 'exact', Nq=Nq, Nk=Nk)
     assert rel(so, o) < 1e-12 and rel(slse, lse) < 1e-12
-    do = rng.standard_normal((Nq, HD))
-    dv = p.T @ do
-    ds = p * (do @ v.T - (do * o).sum(1, keepdims=True)) * scale
-    dq, dk = ds @ k, ds.T @ q
-    sdq, sdk, sdv = sim_xattn_tc_bwd(q, k, v, o, do, lse, scale, garbage)
-    for mine, ref in ((sdq, dq), (sdk, dk), (sdv, dv)):
-        assert np.abs(mine - ref).max() < 1e-11 * max(1.0, np.abs(ref).max())
+    sdq, sdk, sdv = AE.bwd(pad(q, Nq), pad(k, Nk), pad(v, Nk), pad(o, Nq), pad(do, Nq), slse, scale, 'exact', Nq=Nq, Nk=Nk)
+    for mine, ref in ((sdq, dq), (sdk, dk), (sdv, dv)):      # one key => dq, dk are exactly 0: compare absolutely
+        assert mine.shape == ref.shape
+        assert float((mine - ref).abs().max()) < 1e-11 * max(1.0, float(ref.abs().max()))
+
+
+@pytest.mark.parametrize('regime', AE.REGIMES)
+def test_attn_mma_model_bf16_noise(regime):
+    """The 'bf16' model rounds where the kernels do: its outputs are bf16 values (dK / dV only on the packed path), it lands a
+    few bf16 ulps from fp64, and the rounding of P and dS adds to the rounding of the outputs alone ('bf16_out')."""
+    hd, Nq, Nk, scale = 64, 129, 197, 0.125
+    q, k, v, do = AE.make_inputs(2, Nq, Nk, hd, scale, regime, seed=1)
+    o, lse, dq, dk, dv = AE.reference(q, k, v, do, scale)
+    if regime == 'uniform':
+        s = (q @ k.transpose(1, 2)) * scale
+        assert float((s - s[:, :, :1]).abs().max()) < 1e-9             # every logit of a row equal: P = 1 / Nk
+    if regime == 'max_last':
+        s = (q @ k.transpose(1, 2)) * scale
+        assert bool((s.argmax(-1) >= (Nk - 1) // 64 * 64).all()) and 26 < float(s.amax()) < 34
+    if regime == 'max_first':
+        s = (q @ k.transpose(1, 2)) * scale
+        assert float((s[:, :, 64:].amax(-1) - s[:, :, :64].amax(-1)).max()) < -90
+    b_o, _ = AE.fwd(q, k, v, scale, 'bf16_out')
+    m_o, m_lse = AE.fwd(q, k, v, scale, 'bf16')
+    assert torch.equal(AE.bf16(m_o), m_o)
+    assert float((m_lse - lse).abs().max()) < 1e-10                   # l is summed from the unrounded P
+    gq, gk, gv = AE.bwd(q, k, v, m_o, do, m_lse, scale, 'bf16', dkv_bf16=True)
+    fq, fk, fv = AE.bwd(q, k, v, m_o, do, m_lse, scale, 'bf16', dkv_bf16=False)
+    assert torch.equal(AE.bf16(gq), gq) and torch.equal(AE.bf16(gk), gk) and torch.equal(AE.bf16(gv), gv)
+    assert torch.equal(AE.bf16(fk), gk) and torch.equal(AE.bf16(fv), gv) and not torch.equal(fk, gk)
+    for got, ref in ((m_o, o), (gq, dq), (gk, dk), (gv, dv)):
+        e = AE.row_errors(got, ref)
+        assert 1e-4 < e.glob < 0.1, e
+    # rounding P costs accuracy on top of the output's rounding, except where P is exactly 1 (uniform rows: exp2(0))
+    assert AE.row_errors(b_o, o).glob < AE.row_errors(m_o, o).glob or regime == 'uniform'
+
+
+# ---- the per-row gate of the attention tests: faults it must catch --------------------------------------------------------
+def test_row_gate_catches_one_copied_query_row():
+    """At (Bp, N, H) = (64, 197, 12) one head's query row replaced by its neighbour's stays under the whole-tensor 5e-3 gate of
+    test_gpu_attention.py but fails the per-row gate against the bf16 model."""
+    Bp, N, H, hd, scale = 64, 197, 12, 64, 0.125
+    q, k, v, _ = AE.make_inputs(Bp * H, N, N, hd, scale, seed=2)
+    o = AE.reference(q, k, v, q, scale)[0]
+    model = AE.fwd(q, k, v, scale, 'bf16')[0]
+    bad = model.clone()
+    bad[5 * H + 7, 100] = bad[5 * H + 7, 101]
+    assert AE.within_budget(model, o, model)[0]
+    assert rel(bad, o) < 5e-3
+    ok, g, m = AE.within_budget(bad, o, model)
+    assert not ok and g.where == (5 * H + 7, 0, 100), (g, m)
+
+
+def test_row_gate_catches_one_wrong_key_tile_of_dk():
+    """One 64-key tile of dK 10 % too large at Nk = 1569 is within the 2e-2 whole-tensor gate of test_gpu_mvit.py's
+    tensor-core cases, and far outside the per-row gate."""
+    P, N, hd, scale = 2, 1569, 64, 0.125
+    q, k, v, do = AE.make_inputs(P, N, N, hd, scale, seed=3)
+    o, lse, dq, dk, dv = AE.reference(q, k, v, do, scale)
+    m_o, m_lse = AE.fwd(q, k, v, scale, 'bf16')
+    _, mk, _ = AE.bwd(q, k, v, m_o, do, m_lse, scale, 'bf16')
+    bad = mk.clone()
+    bad[1, 640:704] *= 1.1
+    assert AE.within_budget(mk, dk, mk)[0]
+    assert rel(bad, dk) < 2e-2
+    ok, g, _ = AE.within_budget(bad, dk, mk)
+    assert not ok and g.where[0] == 1 and 640 <= g.where[2] < 704
+
+
+def test_lse_gate_catches_a_shift_on_a_partial_query_tile():
+    """lse off by 1e-3 on the five rows of one problem's partial last query tile (N = 197) passes a whole-tensor 1e-5 gate."""
+    P, N, hd, scale = 48, 197, 64, 0.125
+    q, k, v, _ = AE.make_inputs(P, N, N, hd, scale, seed=4)
+    lse = AE.reference(q, k, v, q, scale)[1]
+    bad = lse.clone()
+    bad[3, 192:] += 1e-3
+    assert AE.lse_error(AE.fwd(q, k, v, scale, 'bf16')[1], lse)[0] < AE.LSE_TOL
+    assert rel(bad, lse) < 1e-5
+    e, i = AE.lse_error(bad, lse)
+    assert e > AE.LSE_TOL and i // N == 3 and i % N >= 192
+
+
+def test_row_gate_catches_scale_applied_twice_to_dk():
+    P, Nq, Nk, hd, scale = 2, 129, 197, 64, 0.125
+    q, k, v, do = AE.make_inputs(P, Nq, Nk, hd, scale, seed=5)
+    dk = AE.reference(q, k, v, do, scale)[3]
+    m_o, m_lse = AE.fwd(q, k, v, scale, 'bf16')
+    _, mk, _ = AE.bwd(q, k, v, m_o, do, m_lse, scale, 'bf16')
+    assert AE.within_budget(mk, dk, mk)[0]
+    assert not AE.within_budget(mk * scale, dk, mk)[0]
+
+
+def test_row_metric_locates_the_row():
+    g = torch.Generator().manual_seed(6)
+    ref = torch.randn(2, 3, 70, 8, generator=g, dtype=torch.float64)
+    got = ref.clone()
+    got[1, 2, 65, 3] += 0.5
+    e = AE.row_errors(got, ref)
+    assert e.where == (1, 2, 65)
+    assert abs(e.worst - 0.5 / float(ref[1, 2, 65].norm())) < 1e-12
+    assert abs(e.glob - 0.5 / float(ref.norm())) < 1e-12
+    small = ref.clone()
+    small[0, 0, 0] *= 1e-6                                             # a near-zero row is measured against the floor
+    bumped = small.clone()
+    bumped[0, 0, 0, 0] += 1e-3
+    rms = float(small.norm(dim=-1).square().mean().sqrt())
+    assert abs(AE.row_errors(bumped, small).worst - 1e-3 / (AE.ROW_FLOOR * rms)) < 1e-9
+    assert AE.row_errors(torch.full_like(ref, float('nan')), ref).worst == float('inf')
+    z = torch.zeros(1, 1, 4, 8, dtype=torch.float64)
+    assert AE.row_errors(z + 1e-7, z).worst < 1e-6                    # an all-zero reference is compared absolutely
 
 
 # ---------------------------------------------------------------------------------------------------------------------
