@@ -1,7 +1,8 @@
 // Warp-specialised, persistent bf16 GEMM for sm_90a:
 //   TMA (cp.async.bulk.tensor, 128B swizzle) -> shared-memory ring (mbarrier full / empty pairs) -> wgmma.mma_async
-//   (fp32 accumulators in registers) -> epilogue fused with bias / GELU / dGELU / residual / row maps, straight from
-//   the accumulator registers to global memory.
+//   (fp32 accumulators in registers) -> epilogue fused with bias / GELU / dGELU / residual / row maps.  The bf16-output
+//   forms on plain rows stage the tile in shared memory and write it with TMA stores that run under the next tile's
+//   MMAs; the others write straight from the accumulator registers to global memory.
 // Persistent: one CTA per SM walks a static sequence of 128 x BN output tiles (x K split), BN in {128, 192, 256}.  384
 // threads: warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = consumers, each owning 64 rows of every tile.  The
 // producer runs ahead across tile boundaries, so the next tile's first k-blocks load while the consumers run the epilogue.
@@ -42,14 +43,23 @@ struct GemmDev {
   long long special_ld;
 };
 
-template <int BN>
+// Epilogue kinds (kernel template parameter SE): 0 = from registers; 1 = one staged bf16 output (VT_EPI_BF16);
+// 2 = two staged bf16 tiles (VT_EPI_GELU: z and h; VT_EPI_DGELU: dz and the TMA-loaded z).
+constexpr int EPI_BOX_BYTES = 64 * 64 * 2;   // one 64-row x 64-column bf16 box, 128B-swizzled as TMA reads / writes it
+
+template <int BN, int SE>
 struct GemmCfg {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = (BN == 256) ? 4 : (BN == 192 ? 5 : 6);
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-  static_assert(SMEM_BYTES <= 232448, "shared memory budget");
+  static constexpr int EPI_TILE_BYTES = BM * BN * 2;    // one staged 128 x BN bf16 tile (both consumer halves)
+  static constexpr int EPI_BYTES = SE * EPI_TILE_BYTES;
+  static constexpr int SMEM_LIMIT = 232448, SMEM_EXTRA = 1024 /*align slack*/ + 256 /*barriers*/;
+  // the ring gives up stages to the staging tiles: 6 / 5 / 4 stages at BN = 128 / 192 / 256 without staging
+  static constexpr int STAGES_FIT = (SMEM_LIMIT - SMEM_EXTRA - EPI_BYTES) / STAGE_BYTES;
+  static constexpr int STAGES = STAGES_FIT < 6 ? STAGES_FIT : 6;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + SMEM_EXTRA;
+  static_assert(STAGES >= 2 && SMEM_BYTES <= SMEM_LIMIT, "shared memory budget");
 };
 
 template <int BN, int TA, int TB>
@@ -102,13 +112,28 @@ __device__ __forceinline__ EpiRow epi_row(const GemmDev& p, int row, int split) 
   return r;
 }
 
-// columns n, n + 1 of one row (n even, n + 1 < N since N % 8 == 0)
-__device__ __forceinline__ void epi_pair(const GemmDev& p, const EpiRow& r, int n, float v0, float v1) {
-  if (!r.out) return;
+// The per-element arithmetic of the bf16 forms, shared by the register and the staged epilogue so that both give the
+// same bits.
+__device__ __forceinline__ void add_bias(const GemmDev& p, int n, float& v0, float& v1) {
   if (p.bias) {
     const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
     v0 += b.x; v1 += b.y;
   }
+}
+// h from the bf16-rounded z: bit for bit what the stand-alone GELU kernel computes from the stored z
+__device__ __forceinline__ uint32_t gelu_pair(uint32_t z) {
+  const float2 zr = unpack_bf16x2(z);
+  return pack_bf16x2(gelu_fast(zr.x), gelu_fast(zr.y));
+}
+__device__ __forceinline__ uint32_t dgelu_pair(uint32_t zpair, float v0, float v1) {
+  const float2 z = unpack_bf16x2(zpair);
+  return pack_bf16x2(v0 * dgelu_fast(z.x), v1 * dgelu_fast(z.y));
+}
+
+// columns n, n + 1 of one row (n even, n + 1 < N since N % 8 == 0)
+__device__ __forceinline__ void epi_pair(const GemmDev& p, const EpiRow& r, int n, float v0, float v1) {
+  if (!r.out) return;
+  add_bias(p, n, v0, v1);
   if (p.epi == VT_EPI_BF16) {
     *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(r.out) + n) = pack_bf16x2(r.s * v0, r.s * v1);
   } else if (p.epi == VT_EPI_F32) {
@@ -120,14 +145,53 @@ __device__ __forceinline__ void epi_pair(const GemmDev& p, const EpiRow& r, int 
     }
     *reinterpret_cast<float2*>(reinterpret_cast<float*>(r.out) + n) = make_float2(fmaf(r.s, v0, a.x), fmaf(r.s, v1, a.y));
   } else if (p.epi == VT_EPI_GELU) {
-    // h from the bf16-rounded z: bit for bit what the stand-alone GELU kernel computes from the stored z
     const uint32_t z = pack_bf16x2(v0, v1);
-    const float2 zr = unpack_bf16x2(z);
     *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(r.out) + n) = z;
-    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(r.out2) + n) = pack_bf16x2(gelu_fast(zr.x), gelu_fast(zr.y));
+    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(r.out2) + n) = gelu_pair(z);
   } else {  // VT_EPI_DGELU
-    const float2 z = unpack_bf16x2(*reinterpret_cast<const uint32_t*>(reinterpret_cast<const __nv_bfloat16*>(r.aux) + n));
-    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(r.out) + n) = pack_bf16x2(v0 * dgelu_fast(z.x), v1 * dgelu_fast(z.y));
+    const uint32_t z = *reinterpret_cast<const uint32_t*>(reinterpret_cast<const __nv_bfloat16*>(r.aux) + n);
+    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(r.out) + n) = dgelu_pair(z, v0, v1);
+  }
+}
+
+// Staged epilogue of one consumer warpgroup: its 64 x BN half of the tile goes to shared memory as BN / 64 boxes of
+// 64 rows x 128 B in the SWIZZLE_128B layout (16-byte chunk c of row r at chunk c ^ (r % 8)).  A thread's column pair
+// of 8 rows of one warp lands in 8 different chunks: the 32 lanes hit 32 different banks.  Rows >= M and columns >= N
+// are left as they are; the TMA store clips them.  stage: this half's output tile; stage2: GELU's h, or DGELU's z as
+// loaded by the producer.
+template <int BN, int EPI>
+__device__ __forceinline__ void epi_stage(const GemmDev& p, const float (&acc)[BN / 2], uint8_t* stage, uint8_t* stage2,
+                                          int row0, int n0, int warp, int lane) {
+  const int r = warp * 16 + (lane >> 2);          // rows r and r + 8 of the 64-row half; r % 8 == lane / 4
+  float s[2] = {1.0f, 1.0f};
+  if (EPI == VT_EPI_BF16 && p.row_scale) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      if (row0 + r + 8 * h < p.M) s[h] = p.row_scale[row0 + r + 8 * h];
+  }
+  // a1 / a2: this thread's word of chunk r % 8 (r % 8 in address bits [4, 7)); xor with j % 8 there gives chunk j ^ r
+  const uint32_t a1 = smem_u32(stage) + r * 128 + 4 * (lane & 3) + ((lane >> 2) << 4);
+  const uint32_t a2 = smem_u32(stage2) + r * 128 + 4 * (lane & 3) + ((lane >> 2) << 4);
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int n = n0 + 8 * j + 2 * (lane & 3);
+    if (n >= p.N) break;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t off = (j >> 3) * EPI_BOX_BYTES + h * 8 * 128;
+      const uint32_t o = (a1 ^ ((j & 7) << 4)) + off, o2 = (a2 ^ ((j & 7) << 4)) + off;
+      float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+      add_bias(p, n, v0, v1);
+      if (EPI == VT_EPI_BF16) {
+        st_shared_u32(o, pack_bf16x2(s[h] * v0, s[h] * v1));
+      } else if (EPI == VT_EPI_GELU) {
+        const uint32_t z = pack_bf16x2(v0, v1);
+        st_shared_u32(o, z);
+        st_shared_u32(o2, gelu_pair(z));
+      } else {  // VT_EPI_DGELU
+        st_shared_u32(o, dgelu_pair(ld_shared_u32(o2), v0, v1));
+      }
+    }
   }
 }
 
@@ -154,24 +218,39 @@ __device__ __forceinline__ Tile tile_at(const GemmDev& p, int t) {
 // through one shared-memory ring whose stage / phase count runs on across tiles, so barrier set-up, register hand-over and
 // the tensor-map prefetch happen once per CTA and the ring refills during each epilogue.  The walk is static: a tile's
 // result depends only on the tile, not on the grid size.
-template <int BN, int TA, int TB>
+// SE > 0 (staged epilogue): each consumer warpgroup writes its half of the tile into its own staging boxes, and one of its
+// threads stores them with TMA (tmC: out; tmD: GELU's out2) and goes straight on to the next tile's MMAs; before the
+// boxes are rewritten, that thread waits until the previous store has read them.  For DGELU the producer TMA-loads the
+// tile's z (tmD) into the second staging tile after issuing the tile's last k-block, guarded by a z full / z empty
+// mbarrier pair.
+template <int BN, int TA, int TB, int SE>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmDev p) {
-  using Cfg = GemmCfg<BN>;
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmD, const GemmDev p) {
+  using Cfg = GemmCfg<BN, SE>;
   constexpr int STAGES = Cfg::STAGES;
+  constexpr int HALF_BYTES = Cfg::EPI_TILE_BYTES / 2;   // one consumer warpgroup's 64 x BN part of a staged tile
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
+  uint8_t* epi_smem = smem + STAGES * Cfg::STAGE_BYTES;   // staged tiles (1024-byte aligned), SE x EPI_TILE_BYTES
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_smem + Cfg::EPI_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* zfull_bar = empty_bar + STAGES;
+  uint64_t* zempty_bar = zfull_bar + 1;
+  const bool load_z = SE == 2 && p.epi == VT_EPI_DGELU;
 
   const int wg = threadIdx.x >> 7;
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if (SE > 0) tma_prefetch_desc(&tmC);
+    if (SE == 2) tma_prefetch_desc(&tmD);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 8);   // one arrive per consumer warp
     }
+    mbar_init(zfull_bar, 1);
+    mbar_init(zempty_bar, 2);        // one arrive per consumer warpgroup
     fence_barrier_init();
   }
   __syncthreads();
@@ -180,7 +259,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
       uint32_t it = 0;   // ring position: k-blocks loaded so far by this CTA
-      for (int t = blockIdx.x; t < p.tiles; t += gridDim.x) {
+      uint32_t tj = 0;   // tiles of this CTA so far
+      for (int t = blockIdx.x; t < p.tiles; t += gridDim.x, ++tj) {
         const Tile c = tile_at<BN>(p, t);
         for (int kb = c.kb0; kb < c.kb1; ++kb, ++it) {
           const int stage = (int)(it % STAGES);
@@ -201,6 +281,16 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
             for (int ch = 0; ch < BN / 64; ++ch) tma_load_2d(sB + ch * CHUNK_BYTES, &tmB, &full_bar[stage], c.n0 + ch * 64, kb * BK);
           }
         }
+        if (load_z) {   // the tile's z into the second staging tile, once the consumers have read the previous tile's
+          mbar_wait(zempty_bar, (tj & 1) ^ 1);
+          mbar_arrive_expect_tx(zfull_bar, Cfg::EPI_TILE_BYTES);   // out-of-bounds parts are zero-filled and counted
+          uint8_t* zt = epi_smem + Cfg::EPI_TILE_BYTES;
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int b = 0; b < BN / 64; ++b)
+              tma_load_2d(zt + h * HALF_BYTES + b * EPI_BOX_BYTES, &tmD, zfull_bar, c.n0 + 64 * b, c.m0 + 64 * h);
+        }
       }
     }
     return;
@@ -209,8 +299,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   setmaxnreg_inc<232>();
   const int cw = wg - 1;                       // consumer: rows [64 cw, 64 cw + 64) of every tile
   const int warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
-  uint32_t it = 0;
-  for (int t = blockIdx.x; t < p.tiles; t += gridDim.x) {
+  const bool leader = (threadIdx.x & 127) == 0;   // issues this warpgroup's TMA stores
+  uint8_t* stage = epi_smem + cw * HALF_BYTES;
+  uint8_t* stage2 = stage + Cfg::EPI_TILE_BYTES;
+  uint32_t it = 0, tj = 0;
+  for (int t = blockIdx.x; t < p.tiles; t += gridDim.x, ++tj) {
     const Tile c = tile_at<BN>(p, t);
     float acc[BN / 2];
 #pragma unroll
@@ -237,16 +330,41 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     wgmma_wait<0>();
     if (lane == 0) mbar_arrive(&empty_bar[prev]);   // the producer is already filling the ring for the next tile
 
-    const int r0 = c.m0 + cw * 64 + warp * 16 + (lane >> 2);
-    const EpiRow e0 = epi_row(p, r0, c.split), e1 = epi_row(p, r0 + 8, c.split);
+    if constexpr (SE > 0) {
+      const int row0 = c.m0 + cw * 64;
+      if (load_z) mbar_wait(zfull_bar, tj & 1);
+      if (leader) tma_store_wait_read_all();       // the previous tile's store has read the staging boxes
+      named_bar_sync(1 + cw, 128);
+      if (SE == 1) epi_stage<BN, VT_EPI_BF16>(p, acc, stage, stage2, row0, c.n0, warp, lane);
+      else if (p.epi == VT_EPI_GELU) epi_stage<BN, VT_EPI_GELU>(p, acc, stage, stage2, row0, c.n0, warp, lane);
+      else epi_stage<BN, VT_EPI_DGELU>(p, acc, stage, stage2, row0, c.n0, warp, lane);
+      fence_proxy_async_smem();
+      named_bar_sync(1 + cw, 128);
+      if (leader) {
+        if (load_z) mbar_arrive(zempty_bar);
+        if (row0 < p.M) {
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int n = c.n0 + 8 * j + 2 * (lane & 3);
-      if (n >= p.N) break;
-      epi_pair(p, e0, n, acc[4 * j], acc[4 * j + 1]);
-      epi_pair(p, e1, n, acc[4 * j + 2], acc[4 * j + 3]);
+          for (int b = 0; b < BN / 64; ++b) {
+            if (c.n0 + 64 * b >= p.N) break;
+            tma_store_2d(&tmC, stage + b * EPI_BOX_BYTES, c.n0 + 64 * b, row0);
+            if (SE == 2 && p.epi == VT_EPI_GELU) tma_store_2d(&tmD, stage2 + b * EPI_BOX_BYTES, c.n0 + 64 * b, row0);
+          }
+        }
+        tma_store_commit();
+      }
+    } else {
+      const int r0 = c.m0 + cw * 64 + warp * 16 + (lane >> 2);
+      const EpiRow e0 = epi_row(p, r0, c.split), e1 = epi_row(p, r0 + 8, c.split);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int n = c.n0 + 8 * j + 2 * (lane & 3);
+        if (n >= p.N) break;
+        epi_pair(p, e0, n, acc[4 * j], acc[4 * j + 1]);
+        epi_pair(p, e1, n, acc[4 * j + 2], acc[4 * j + 3]);
+      }
     }
   }
+  if (SE > 0 && leader) tma_store_wait_read_all();   // shared memory stays valid until the last store has read it
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -358,23 +476,48 @@ int launch_reduce_rows(const float* in, float* out, long long stride, int S, lon
   return check_launch("reduce_rows_kernel");
 }
 
-template <int BN, int TA, int TB>
-static int launch_gemm_t(const CUtensorMap& tmA, const CUtensorMap& tmB, const GemmDev& d, cudaStream_t st) {
-  using Cfg = GemmCfg<BN>;
+// tm: A, B, and for the staged epilogue the output and GELU's out2 / DGELU's z
+template <int BN, int TA, int TB, int SE>
+static int launch_gemm_t(const CUtensorMap (&tm)[4], const GemmDev& d, cudaStream_t st) {
+  using Cfg = GemmCfg<BN, SE>;
   static bool attr_set = false;  // benign race: idempotent
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, TA, TB>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, TA, TB, SE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
     VT_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(smem=%d) failed: %s", Cfg::SMEM_BYTES, cudaGetErrorString(e));
     attr_set = true;
   }
   const int grid = d.tiles < persistent_sm_count() ? d.tiles : persistent_sm_count();
-  gemm_wgmma_kernel<BN, TA, TB><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(tmA, tmB, d);
+  gemm_wgmma_kernel<BN, TA, TB, SE><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(tm[0], tm[1], tm[2], tm[3], d);
   return check_launch("gemm_wgmma_kernel");
+}
+
+template <int BN, int SE>
+static int launch_layout(const vt_gemm_params* q, const CUtensorMap (&tm)[4], const GemmDev& d, cudaStream_t st) {
+  if (!q->a_mn_major && !q->b_mn_major) return launch_gemm_t<BN, 0, 0, SE>(tm, d, st);
+  if (!q->a_mn_major) return launch_gemm_t<BN, 0, 1, SE>(tm, d, st);
+  if (!q->b_mn_major) return launch_gemm_t<BN, 1, 0, SE>(tm, d, st);
+  return launch_gemm_t<BN, 1, 1, SE>(tm, d, st);
+}
+
+#ifndef VT_DEFAULT_STAGED_EPI
+#define VT_DEFAULT_STAGED_EPI true
+#endif
+// Staged epilogue kind for this call (see GemmCfg): the bf16-output forms on plain rows, whose outputs (and DGELU's z)
+// TMA can address as [M, N] tensors.  VT_GEMM_STAGED_EPI=0 keeps every form on the register epilogue.
+static int staged_kind(const vt_gemm_params* q) {
+  if (q->epilogue == VT_EPI_F32 || q->out_row) return 0;
+  if (!feature_on("VT_GEMM_STAGED_EPI", VT_DEFAULT_STAGED_EPI)) return 0;
+  if (q->epilogue == VT_EPI_BF16) return 1;
+  // GELU's out2 is not checked by the register path's alignment rule; TMA needs it 16-byte aligned
+  if (q->epilogue == VT_EPI_GELU && ((reinterpret_cast<uintptr_t>(q->out2) & 15) || (q->ldo2 * 2) % 16)) return 0;
+  return 2;
 }
 
 template <int BN>
 static int launch_gemm(const vt_gemm_params* q, GemmDev& d, cudaStream_t st) {
-  CUtensorMap tmA, tmB;
+  CUtensorMap tm[4];
+  memset(tm, 0, sizeof(tm));
+  CUtensorMap &tmA = tm[0], &tmB = tm[1];
   int rc;
   if (!q->a_mn_major) rc = make_tmap_bf16_2d(&tmA, q->a, q->M, q->K, q->lda, BM);
   else rc = make_tmap_bf16_2d(&tmA, q->a, q->K, q->M, q->lda, BK);
@@ -395,10 +538,16 @@ static int launch_gemm(const vt_gemm_params* q, GemmDev& d, cudaStream_t st) {
     d.ldo = q->N;
     d.split_stride = tile_out;
   }
-  if (!q->a_mn_major && !q->b_mn_major) rc = launch_gemm_t<BN, 0, 0>(tmA, tmB, d, st);
-  else if (!q->a_mn_major) rc = launch_gemm_t<BN, 0, 1>(tmA, tmB, d, st);
-  else if (!q->b_mn_major) rc = launch_gemm_t<BN, 1, 0>(tmA, tmB, d, st);
-  else rc = launch_gemm_t<BN, 1, 1>(tmA, tmB, d, st);
+  const int se = d.splits > 1 ? 0 : staged_kind(q);
+  if (se > 0) {
+    rc = make_tmap_bf16_2d(&tm[2], q->out, q->M, q->N, q->ldo, 64);
+    if (!rc && q->epilogue == VT_EPI_GELU) rc = make_tmap_bf16_2d(&tm[3], q->out2, q->M, q->N, q->ldo2, 64);
+    if (!rc && q->epilogue == VT_EPI_DGELU) rc = make_tmap_bf16_2d(&tm[3], q->aux, q->M, q->N, q->ldaux, 64);
+    if (rc) return rc;
+  }
+  if (se == 1) rc = launch_layout<BN, 1>(q, tm, d, st);
+  else if (se == 2) rc = launch_layout<BN, 2>(q, tm, d, st);
+  else rc = launch_layout<BN, 0>(q, tm, d, st);
   if (rc) return rc;
   if (d.splits > 1) {
     VT_REQUIRE(q->ldo == q->N, "vt_gemm: split-K requires ldo == N");
@@ -497,8 +646,11 @@ static int gemm_dispatch(const vt_gemm_params* q, void* stream) {
   // Splitting K is only possible for plain fp32 outputs with a workspace (weight gradients).
   // Short-K GEMMs without a split (K <= 1024: qkv, FC1 forward, FC2 data gradient, out-proj) take the 128-wide tile, which
   // the model undervalues: measured on an H100 at B = 8 it is 20-35 % faster than the 256-wide tile on the wide-output
-  // ones (their register epilogue costs about as much as the 12-k-block mainloop) and within 4 % on the others.
+  // ones with the register epilogue, and the staged GELU / dGELU forms lose ring stages to their two staging tiles at
+  // wider tiles.  The one-output staged form may also take the 192-wide tile (4 stages), which the model picks for qkv
+  // (81 vs 92 us) and the projection's data gradient (29 vs 33 us).
   const bool short_k = d.kblocks <= 16;
+  const bool one_staged = staged_kind(q) == 1;
   const int sms = persistent_sm_count();
   const int num_m = (q->M + BM - 1) / BM;
   const bool can_split = q->epilogue == VT_EPI_F32 && q->workspace && !q->out_row && !q->aux && !q->row_scale && !q->bias &&
@@ -509,7 +661,7 @@ static int gemm_dispatch(const vt_gemm_params* q, void* stream) {
   int bn = 128, splits = 1;
   for (int i = 0; i < 3; ++i) {
     if (q->force_bn && cand[i] != q->force_bn) continue;
-    if (!q->force_bn && !can_split && short_k && cand[i] != 128) continue;
+    if (!q->force_bn && !can_split && short_k && cand[i] != 128 && !(one_staged && cand[i] == 192)) continue;
     const int num_n = (q->N + cand[i] - 1) / cand[i];
     const int smax = can_split ? 16 : 1;
     for (int sp = 1; sp <= smax; ++sp) {
