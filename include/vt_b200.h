@@ -427,6 +427,25 @@ typedef struct {
 } vt_im2col_u8_mix_params;
 int vt_im2col_u8_mix_bf16(const vt_im2col_u8_mix_params* p, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Bicubic resize of a positional-embedding grid (TimeSformer.interpolate_pos_encoding, video_transformer.py:171-191:
+ * F.interpolate(mode='bicubic', align_corners=False, scale_factor=(scale_h, scale_w)) on the patch rows of pos_embed).
+ * fp32 token-major rows, D contiguous: grid cell (y, x) of a gh x gw grid is row y * gw + x, read where it lies.
+ *   vt_pos_resize_fwd: src = the gh x gw grid, dst = the oh x ow output (oh = floor(gh * scale_h), ow likewise).
+ *   vt_pos_resize_bwd: src = the gradient of the oh x ow output, dst = the gradient of the gh x gw grid (every row
+ *                      written; the exact adjoint, gathered per input cell: no atomics, deterministic).
+ * Source coordinate (dst + 0.5) / scale - 0.5 (PyTorch's scale-factor form), cubic convolution A = -0.75, 4 x 4 taps
+ * clamped to the grid, fp32 accumulation.  lds / ldd: row strides in elements.  oh + ow <= 8192.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct {
+  const float* src; int64_t lds;
+  float* dst; int64_t ldd;
+  int32_t gh, gw, oh, ow, D;
+  double scale_h, scale_w;
+} vt_pos_resize_params;
+int vt_pos_resize_fwd(const vt_pos_resize_params* p, void* stream);
+int vt_pos_resize_bwd(const vt_pos_resize_params* p, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

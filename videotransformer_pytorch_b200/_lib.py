@@ -214,6 +214,12 @@ class Im2colU8MixParams(C.Structure):
                 ('C', c_i32), ('H', c_i32), ('W', c_i32), ('tube', c_i32), ('ph', c_i32), ('pw', c_i32)]
 
 
+class PosResizeParams(C.Structure):
+    _fields_ = [('src', c_vp), ('lds', c_i64), ('dst', c_vp), ('ldd', c_i64),
+                ('gh', c_i32), ('gw', c_i32), ('oh', c_i32), ('ow', c_i32), ('D', c_i32),
+                ('scale_h', C.c_double), ('scale_w', C.c_double)]
+
+
 EXPORTS = ['vt_version', 'vt_last_error', 'vt_sm_count', 'vt_set_reserved_sms', 'vt_launch_count', 'vt_gemm', 'vt_layernorm_fwd', 'vt_ln_bwd_blocks',
            'vt_layernorm_bwd', 'vt_reduce_rows', 'vt_colsum_chunks', 'vt_colsum_bf16', 'vt_cast_f32_bf16',
            'vt_cls_rows', 'vt_gather_cast_colsum_blocks', 'vt_gather_cast_colsum_bf16', 'vt_gelu_bwd_colsum_blocks', 'vt_gelu_bwd_colsum_bf16',
@@ -222,7 +228,7 @@ EXPORTS = ['vt_version', 'vt_last_error', 'vt_sm_count', 'vt_set_reserved_sms', 
            'vt_maxpool_bwd', 'vt_im2col3d_bf16', 'vt_mvit_tokens_fwd', 'vt_mvit_tokens_bwd', 'vt_mse_blocks',
            'vt_mse_fwd', 'vt_mse_bwd', 'vt_opt_norm2', 'vt_opt_sgd', 'vt_opt_adamw',
            'vt_linear_small_fwd', 'vt_linear_small_bwd', 'vt_softmax_ce', 'vt_scale_by_scalar', 'vt_attn_probs',
-           'vt_im2col_u8_mix_bf16']
+           'vt_im2col_u8_mix_bf16', 'vt_pos_resize_fwd', 'vt_pos_resize_bwd']
 
 _dll = None
 
@@ -705,6 +711,39 @@ class CudaKernels:
         p.B, p.T, p.C, p.H, p.W, p.tube, p.ph, p.pw = B, T, Cc, H, W, tube, ph, pw
         _check(lib.vt_col2im_f32(C.byref(p), _stream()), 'vt_col2im_f32')
         return dx
+
+    # -- positional-embedding resize -------------------------------------------------------------
+    def _pos_resize(self, fn, src, out, n_in, n_out, grid, out_grid, scales):
+        """n_in / n_out: rows of src / out; grid / out_grid: the (rows, cols) of the table before / after the resize."""
+        lib = load_library()
+        _rows2d(_req(src, torch.float32, fn + '.src'), fn + '.src')
+        D = src.shape[1]
+        if src.shape[0] != n_in:
+            raise RuntimeError(f'{fn}: expected {n_in} source rows, got {src.shape[0]}')
+        if out is None:
+            out = torch.empty((n_out, D), dtype=torch.float32, device=src.device)
+        _rows2d(_req(out, torch.float32, fn + '.out'), fn + '.out')
+        if tuple(out.shape) != (n_out, D):
+            raise RuntimeError(f'{fn}: out must be [{n_out}, {D}], got {tuple(out.shape)}')
+        p = PosResizeParams()
+        p.src, p.lds, p.dst, p.ldd = src.data_ptr(), src.stride(0), out.data_ptr(), out.stride(0)
+        p.gh, p.gw = grid
+        p.oh, p.ow = out_grid
+        p.D = D
+        p.scale_h, p.scale_w = float(scales[0]), float(scales[1])
+        _check(getattr(lib, fn)(C.byref(p), _stream()), fn)
+        return out
+
+    def pos_resize_fwd(self, src, grid, out_grid, scales, out=None):
+        """Bicubic resize (F.interpolate, align_corners=False, scale_factor=scales) of the grid whose cell (y, x) is row
+        y * grid[1] + x of src (fp32 [gh*gw, D], unit inner stride) -> fp32 [oh*ow, D] (or written into `out`)."""
+        return self._pos_resize('vt_pos_resize_fwd', src, out, grid[0] * grid[1], out_grid[0] * out_grid[1],
+                                grid, out_grid, scales)
+
+    def pos_resize_bwd(self, dout, grid, out_grid, scales, out=None):
+        """Adjoint of pos_resize_fwd: dout fp32 [oh*ow, D] -> fp32 [gh*gw, D] (or written into `out`)."""
+        return self._pos_resize('vt_pos_resize_bwd', dout, out, out_grid[0] * out_grid[1], grid[0] * grid[1],
+                                grid, out_grid, scales)
 
     # -- HOG ------------------------------------------------------------------------------------
     def hog(self, frames, lut, want_bins=False):

@@ -9,6 +9,7 @@ C-ABI kernel launches (see _lib.K):
   FFNFn           <- FFNWithPreNorm.forward                        (transformer.py:516-523)
   PatchTokensFn   <- PatchEmbed.forward + TimeSformer/ViViT.prepare_tokens
                      (transformer.py:138-151, video_transformer.py:193-240 / :455-475)
+  PosResizeFn     <- the bicubic resize of TimeSformer.interpolate_pos_encoding (video_transformer.py:171-191)
   ClsNormFn       <- final nn.LayerNorm(eps=1e-6) + cls select     (video_transformer.py:251-254)
   AttentionCoreFn <- Attention.forward (stand-alone use)            (transformer.py:165-177)
 
@@ -310,7 +311,14 @@ class SpatialAttnFn(torch.autograd.Function):
         hd = D // H
         xn, mean, rstd = k.ln_fwd(x2, ln_w, ln_b, eps, in_row=maps['sp_in'], rows=Ms)
         qkv = k.gemm(xn, qkv_wh, Ms, 3 * D, D, bias=qkv_b, epi='bf16', tag='qkv')
-        cx, lse, _ = k.attn_fwd(qkv, B * T, P + 1, H, hd, hd ** -0.5)
+        if P + 1 <= ATTN_SINGLE_PASS_MAX:
+            cx, lse, _ = k.attn_fwd(qkv, B * T, P + 1, H, hd, hd ** -0.5)
+        else:
+            # frames of 256 patches or more (inputs larger than 256 x 256 at patch 16): streaming tensor-core kernel,
+            # q/k/v read in place from the packed projection
+            q4, k4, v4 = _packed_heads(qkv, B * T, P + 1, H, hd)
+            cx, lse = k.xattn_fwd(q4, k4, v4, hd ** -0.5)
+            cx = cx.view(Ms, D)
         ybig = torch.empty((R + B * T, D), dtype=torch.float32, device=x.device)
         k.gemm(cx, proj_wh, Ms, D, D, bias=proj_b, epi='f32', aux=x2, aux_row=maps['sp_aux'], out=ybig,
                out_row=maps['sp_out'], row_scale=dp, row_map=affine_row_maps(B, T, P, D)['spatial'], tag='proj')
@@ -335,7 +343,10 @@ class SpatialAttnFn(torch.autograd.Function):
         g, d_proj_b = _cast_with_colsum(k, dy2, in_row=maps['sp_in'], row_scale=_mul_opt(dp, maps['sp_cls_scale']), rows=Ms)
         d_proj_w = _wgrad(g, cx, D, D, Ms, tag='proj', wptr=ctx.wptrs[1])
         dcx = _dgrad(g, proj_wh, Ms, D, D, epi='bf16', tag='proj')
-        dqkv = k.attn_bwd(qkv, cx, dcx, lse, B * T, P + 1, H, hd, hd ** -0.5)
+        if P + 1 <= ATTN_SINGLE_PASS_MAX:
+            dqkv = k.attn_bwd(qkv, cx, dcx, lse, B * T, P + 1, H, hd, hd ** -0.5)
+        else:
+            dqkv = _streaming_attn_bwd(k, qkv, cx, dcx, lse, B * T, P + 1, H, hd)
         d_qkv_w = _wgrad(dqkv, xn, 3 * D, D, Ms, tag='qkv', wptr=ctx.wptrs[0])
         d_qkv_b = k.colsum(dqkv)
         dxn = _dgrad(dqkv, qkv_wh, Ms, D, 3 * D, epi='bf16', tag='qkv')
@@ -466,6 +477,13 @@ class PatchTokensFn(torch.autograd.Function):
         k = K()
         D = w.shape[0]
         ph, pw = w.shape[-2], w.shape[-1]
+        T, Himg, Wimg = (x.shape[1], x.shape[2], x.shape[3]) if x.dtype == torch.uint8 else (x.shape[1], x.shape[3], x.shape[4])
+        n_pos, n_time = (Himg // ph) * (Wimg // pw), T // tube
+        # the epilogue reads table rows through aux_row without bounds: the tables must cover this input's grid
+        if pos_embed.numel() != (1 + n_pos) * D:
+            raise ValueError(f'pos_embed has {pos_embed.numel() // D} rows but a {Himg}x{Wimg} input needs 1 + {n_pos}')
+        if mode == 'timesformer' and (time_embed is None or time_embed.numel() != n_time * D):
+            raise ValueError(f'time_embed must have {n_time} rows for a clip of {T} frames')
         if x.dtype == torch.uint8:
             # decoder output [B, T, H, W, C]: ToTensor + Normalize are folded into the operand kernel (norm = (scale, shift)),
             # and with a mix plan (mixup.Mixup) the batch-level Mixup / CutMix of mixup.py:102-114 as well
@@ -534,6 +552,38 @@ class PatchTokensFn(torch.autograd.Function):
             dx = k.col2im(dcols, xshape, tube, wshape[-2], wshape[-1])
         # small grads are returned as fresh contiguous tensors (not views) so autograd can adopt them in place
         return dx, dw.contiguous(), db, dcls.reshape(cshape).clone(), dpos.contiguous(), dtime, None, None, None, None, None
+
+
+# --------------------------------------------------------------------------------------------------
+class PosResizeFn(torch.autograd.Function):
+    """The resize of TimeSformer.interpolate_pos_encoding (video_transformer.py:176-191): pos [1, 1 + gh*gw, D] ->
+    [1, 1 + oh*ow, D].  Row 0 (cls) passes through; the patch rows, a gh x gw grid flattened row-major, are resized by
+    bicubic interpolation with PyTorch's scale-factor coordinates (vt_pos_resize_fwd) and stay row-major flattened.
+    The gradient flows back through the exact adjoint (vt_pos_resize_bwd)."""
+
+    @staticmethod
+    def forward(ctx, pos, grid, out_grid, scales):
+        k = K()
+        D = pos.shape[-1]
+        src = pos.reshape(-1, D)
+        if src.shape[0] != 1 + grid[0] * grid[1]:
+            raise ValueError(f'pos table has {src.shape[0]} rows, expected 1 + {grid[0]} x {grid[1]}')
+        out = torch.empty((1 + out_grid[0] * out_grid[1], D), dtype=torch.float32, device=pos.device)
+        out[0] = src[0]
+        k.pos_resize_fwd(src[1:], grid, out_grid, scales, out=out[1:])
+        ctx.geom = (tuple(grid), tuple(out_grid), tuple(scales), tuple(pos.shape))
+        return out.view(1, -1, D)
+
+    @staticmethod
+    def backward(ctx, dout):
+        k = K()
+        grid, out_grid, scales, pshape = ctx.geom
+        D = pshape[-1]
+        d = dout.reshape(-1, D).contiguous()
+        dpos = torch.empty((1 + grid[0] * grid[1], D), dtype=torch.float32, device=d.device)
+        dpos[0] = d[0]
+        k.pos_resize_bwd(d[1:], grid, out_grid, scales, out=dpos[1:])
+        return dpos.view(pshape), None, None, None
 
 
 # --------------------------------------------------------------------------------------------------

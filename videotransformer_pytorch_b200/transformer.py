@@ -186,8 +186,9 @@ class PatchEmbed(nn.Module):
         D = self.projection.weight.shape[0]
         dev = x.device
         zeros = lambda *s: torch.zeros(*s, device=dev)
+        n = (x.shape[-2] // self.patch_size[0]) * (x.shape[-1] // self.patch_size[1])     # patches of this input
         tok = ops.PatchTokensFn.apply(x, _f32(self.projection.weight), _f32(self.projection.bias), zeros(1, 1, D),
-                                      zeros(1, self.num_patches + 1, D), None, self.shadow(), 'frames', self.tube)
+                                      zeros(1, n + 1, D), None, self.shadow(), 'frames', self.tube)
         return tok[:, 1:, :]
 
 

@@ -4,10 +4,13 @@ sm_90a kernels.
 
 Covered configurations (SURVEY.md §8a, §8f rank 4): TimeSformer `divided_space_time`, `space_only` (197-token joint
 attention per frame) and `joint_space_time` (one 1569-token attention per clip, streaming tensor-core kernel); ViViT
-`fact_encoder` (model 2), `joint_space_time` (model 1) and `divided_space_time` (model 3).  Nothing falls back to eager
+`fact_encoder` (model 2), `joint_space_time` (model 1) and `divided_space_time` (model 3).  TimeSformer also takes clips
+whose patch grid differs from img_size's (interpolate_pos_encoding, reference :171-191).  Nothing falls back to eager
 PyTorch.
 """
 from __future__ import annotations
+
+import math
 
 import torch
 import torch.nn as nn
@@ -124,11 +127,28 @@ class TimeSformer(_ByteClipInput, nn.Module):
         return {'pos_embed', 'cls_token', 'mask_token'}
 
     def interpolate_pos_encoding(self, x, w, h):
-        npatch = x.shape[1] - 1
-        N = self.pos_embed.shape[1] - 1
+        """reference video_transformer.py:171-191.  x: the tokens, or any tensor whose dim 1 is 1 + the input's patch
+        count; w, h: the clip's width and height."""
+        return self._interpolate(self.pos_embed, x.shape[1] - 1, w, h)
+
+    def _interpolate(self, pos, npatch, w, h):
+        """pos unchanged when the input has the training grid, else its patch rows (a sqrt(N) x sqrt(N) grid) resized
+        bicubically to (w // p) rows x (h // p) columns with the reference's scale factors ((n + 0.1) / sqrt(N)).  The
+        resized grid is flattened row-major and added to patch tokens in Conv2d order (h // p rows of w // p): for w != h
+        token i takes cell (i // (h // p), i % (h // p)), the reference's axis order, reproduced as is."""
+        N = pos.shape[1] - 1
         if npatch == N and w == h:
-            return self.pos_embed
-        raise NotImplementedError('bicubic pos-embed interpolation (img_size != training size) is outside the hot path')
+            return pos
+        g = math.isqrt(N)
+        if g * g != N:
+            raise ValueError(f'pos_embed holds {N} patch rows, which is not a square grid: it cannot be interpolated')
+        p = self.patch_embed.patch_size[0]
+        w0, h0 = w // p, h // p
+        scales = ((w0 + 0.1) / math.sqrt(N), (h0 + 0.1) / math.sqrt(N))
+        out_grid = (math.floor(g * scales[0]), math.floor(g * scales[1]))      # F.interpolate's output size
+        if out_grid != (w0, h0) or w0 < 1 or h0 < 1:
+            raise ValueError(f'cannot resize the {g}x{g} position grid to {w0}x{h0}')
+        return ops.PosResizeFn.apply(pos, (g, g), out_grid, scales)
 
     def _embeds(self, x):
         pos = self.pos_embed
@@ -144,10 +164,13 @@ class TimeSformer(_ByteClipInput, nn.Module):
             b, t, h, w, c = x.shape
         else:
             b, t, c, h, w = x.shape
-        P = self.patch_embed.num_patches
-        if (h // self.patch_embed.patch_size[0]) * (w // self.patch_embed.patch_size[1]) != P or w != h:
-            raise NotImplementedError('input size must match img_size (no pos-embed interpolation on the hot path)')
+        ps = self.patch_embed.patch_size
+        if h % ps[0] or w % ps[1]:
+            raise ValueError(f'clip sides {h}x{w} must be multiples of the patch size {ps[0]}x{ps[1]}')
+        if self.attention_type != 'space_only' and t != self.num_frames:
+            raise ValueError(f'{self.attention_type} model of {self.num_frames} frames fed a clip of {t} frames')
         pos, tim = self._embeds(x)
+        pos = self._interpolate(pos, (h // ps[0]) * (w // ps[1]), w, h)
         pe = self.patch_embed
         mode = 'frames' if self.attention_type == 'space_only' else 'timesformer'   # space_only: per-frame tokens
         tok = ops.PatchTokensFn.apply(x, _f32(pe.projection.weight), _f32(pe.projection.bias), self.cls_token, pos, tim,
@@ -257,6 +280,11 @@ class ViViT(_ByteClipInput, nn.Module):
     def prepare_tokens(self, x):
         x, norm, plan = self._unwrap_clip(x)
         b = x.shape[0]
+        h, w = (x.shape[2], x.shape[3]) if norm is not None else (x.shape[3], x.shape[4])
+        ps = self.patch_embed.patch_size
+        if (h // ps[0]) * (w // ps[1]) != self.patch_embed.num_patches:
+            # no pos_embed interpolation in ViViT: the reference fails on `x + self.pos_embed` (:464-473)
+            raise ValueError(f'ViViT built for img_size {self.patch_embed.img_size} got a {h}x{w} clip')
         pos = self.pos_embed if self.use_learnable_pos_emb else self.pos_embed.to(x.device).detach()
         pe = self.patch_embed
         if self.attention_type == 'fact_encoder':
