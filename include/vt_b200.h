@@ -55,6 +55,8 @@ int vt_launch_count(void);
  *                  (residual add / pos+time-embed add / fp32 gradients)
  *   VT_EPI_GELU  : out_bf16[m,n] = z = acc + bias[n];  out2_bf16[m,n] = gelu_erf(z)     (transformer.py:501-503)
  *   VT_EPI_DGELU : out_bf16[m,n] = acc * gelu_erf'(aux_bf16[m,n])                        (autograd of nn.GELU)
+ *   VT_EPI_GELU_H: out_bf16[orow(m), n] = gelu_erf(bf16(s(m) * (acc + bias[n])))  — forward-only FC1: h alone, z is not
+ *                  written.  Bit for bit VT_EPI_BF16 followed by vt_gelu_fwd_bf16 (same per-element code, same tiles).
  * orow(m) = out_row ? out_row[m] : m  (negative => row skipped);  arow likewise (negative => no addend);  s(m) = row_scale ? row_scale[m] : 1
  * (row_scale carries DropPath's per-row mask/keep factor, transformer.py:34-42, and the 1/T of the cls mean :371-373).
  *
@@ -62,7 +64,7 @@ int vt_launch_count(void);
  * K = tokens), K is split; partial tiles go to the fp32 workspace and are summed by a second kernel.
  * Only with VT_EPI_F32, no row maps.
  * ------------------------------------------------------------------------------------------- */
-enum { VT_EPI_BF16 = 0, VT_EPI_F32 = 1, VT_EPI_GELU = 2, VT_EPI_DGELU = 3 };
+enum { VT_EPI_BF16 = 0, VT_EPI_F32 = 1, VT_EPI_GELU = 2, VT_EPI_DGELU = 3, VT_EPI_GELU_H = 4 };
 
 typedef struct {
   const void* a;      /* bf16 */
@@ -111,6 +113,7 @@ int vt_gemm(const vt_gemm_params* p, void* stream);
  * is the normalised row in_row[m] of x, so '(b t) p' / '(b p) t' orders and the per-frame cls copy
  * cost no separate pass.
  *   y_bf16[m,:] = (x[in_row ? in_row[m] : m, :] - mean) * rstd * gamma + beta ;  mean/rstd saved.
+ * mean / rstd may both be NULL: not written (forward-only calls; only the backward reads them).
  * D must be a multiple of 128 and <= 1024.
  * ------------------------------------------------------------------------------------------- */
 typedef struct {
@@ -198,7 +201,8 @@ int vt_gelu_bwd_colsum_bf16(const vt_gelu_bwd_colsum_params* p, void* stream);
  * Multi-head softmax attention core on a packed qkv tensor (no projection):
  *   qkv bf16 [Bp, N, 3, H, hd] (the layout produced by transformer.py:167's reshape), hd = 64
  *   ctx bf16 [Bp, N, H*hd] = softmax(q k^T * scale) v      (transformer.py:170-174)
- *   lse fp32 [Bp, H, N]   (saved for backward);  probs fp32 [Bp,H,N,N] optional (Attention returns it, :177)
+ *   lse fp32 [Bp, H, N]   (saved for backward; NULL = not written, for every implementation);
+ *   probs fp32 [Bp,H,N,N] optional (Attention returns it, :177)
  * Three kernels behind one entry point: a tensor-core flash kernel for the spatial pass (N = 197; mma.sync bf16 with
  * fp32 accumulators, K/V tiles in shared memory, vt_attention_mma.cu), a warp-per-problem kernel for the temporal pass
  * (N = 8, 18 816 problems/layer), and a generic warp-per-query kernel for any other N <= 256 (ViViT N = 9, probs output).
@@ -253,7 +257,8 @@ int vt_hog(const vt_hog_params* p, void* stream);
  *   1.. are the (T,Hin,Win) tokens, t-major) — i.e. a q/k/v slice of the fused projection output is read in place.
  *   pooled fp32 [B,H,1+Lo,hd] = cls row copied, other rows conv3d(kernel 3x3x3, stride (st,sh,sw), padding 1, groups=hd)
  *   out    bf16 [B,H,1+Lo,hd] = LayerNorm(pooled; gamma, beta, eps) over hd;  mean/rstd [B*H*(1+Lo)] saved.
- * Lo = To*Ho*Wo with To = (T + 2 - 3)/st + 1 etc.   w: fp32 [hd, 27] (nn.Conv3d weight [hd,1,3,3,3]). */
+ * Lo = To*Ho*Wo with To = (T + 2 - 3)/st + 1 etc.   w: fp32 [hd, 27] (nn.Conv3d weight [hd,1,3,3,3]).
+ * pooled, mean and rstd are only read by vt_pool_bwd: all three NULL = none written (forward-only calls). */
 typedef struct {
   const void* in; int64_t in_bs, in_rs;
   const float* w; const float* gamma; const float* beta;
@@ -280,7 +285,7 @@ int vt_pool_bwd(const vt_pool_bwd_params* p, void* stream);
 
 /* Softmax attention with separate, strided Q / K / V and Nq != Nk (pooling attention):
  *   element (b, h, n, c) of q at q[b*q_bs + h*q_hs + n*q_rs + c] (bf16), same for k, v, o (and dout, dq).
- *   o = softmax(scale * q k^T) v ;  lse fp32 [B,H,Nq] = log sum exp(scale * q k^T).
+ *   o = softmax(scale * q k^T) v ;  lse fp32 [B,H,Nq] = log sum exp(scale * q k^T)  (NULL = not written, both kernels).
  * Two implementations, head dim 64 or 96: tensor-core flash kernels (vt_attention_mma.cu, VT_XATTN_TCGEN05 — the name is
  * kept for ABI compatibility) and CUDA-core kernels for arbitrary strides (two threads per query row, K/V tiles staged in
  * shared memory). */
@@ -306,7 +311,8 @@ int vt_xattn_bwd(const vt_xattn_bwd_params* p, void* stream);
 
 /* Skip-path MaxPool3d on the fp32 token stream (pytorchvideo MultiScaleBlock.pool_skip: kernel s+1, stride s, padding
  * k//2 per axis; cls row copied).  x [B,1+T*H*W,D] -> y [B,1+To*Ho*Wo,D]; idx u8 same shape as y = winning tap
- * ((dt*kh+dh)*kw+dw, first maximum in scan order like torch).  Backward routes dy to the winners. */
+ * ((dt*kh+dh)*kw+dw, first maximum in scan order like torch).  Backward routes dy to the winners.  idx NULL = winners not
+ * recorded (forward-only calls). */
 typedef struct {
   const float* x; float* y; uint8_t* idx;
   int32_t B, D, T, H, W, kt, kh, kw, st, sh, sw, To, Ho, Wo;
@@ -411,6 +417,25 @@ int vt_softmax_ce(const vt_softmax_ce_params* p, void* stream);
 /* out[i] = in[i] * scalar[0] (device scalar: chain rule through the loss inside a captured graph) */
 typedef struct { const float* in; const float* scalar; float* out; int64_t n; } vt_scale_params;
 int vt_scale_by_scalar(const vt_scale_params* p, void* stream);
+
+/* Top-k accuracy counters of an evaluation step (model_trainer.py validation_step / test_step):
+ *   logits fp32 [B*V, C], row b*V + v = view v of clip b;  labels int64 [B]
+ *   mean[b, :] = (sum_v logits[b*V + v, :]) * (1.0f / V)   (views summed in order, then scaled by the fp32 factor 1/V,
+ *                which is how torch forms preds.view(-1, V, C).mean(1))
+ *   probs fp32 [B, C] = softmax(mean[b, :])  (optional, NULL = not written)
+ *   rank(b) = #{c : mean[b, c] > mean[b, label_b]};  hits[i] += #{b : rank(b) < k[i]} for i < n_k (n_k <= 4);  samples[0] += B
+ * Counters are int64 device values accumulated with integer atomics (deterministic, graph-capturable).  A label outside
+ * [0, C) or a NaN label score counts as a miss.  Against torch's test step (mean, softmax, topk on the probabilities) the
+ * count can differ in two ways, both confined to near-ties: where two probabilities round to the same float, torch.topk
+ * breaks the tie by index while this count ranks the label first among its equals; and where a reduction that sums the
+ * views in another order gives a mean one ulp away, a class within that ulp of the label can change sides.  C <= 12000. */
+typedef struct {
+  const float* logits; const int64_t* labels; float* probs;
+  int64_t* hits; int64_t* samples;
+  int32_t B, V, C;
+  int32_t n_k; int32_t k[4];
+} vt_topk_hits_params;
+int vt_topk_hits(const vt_topk_hits_params* p, void* stream);
 
 /* probs[bp,h,i,j] = softmax_j(q_i . k_j * scale) for any N that fits 8 rows of scores in shared memory (N <= ~6000),
  * q/k read in place from the packed projection bf16 [Bp, N, 3, H, 64].  Serves get_last_selfattention

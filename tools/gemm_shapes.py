@@ -10,6 +10,9 @@ this one process: the columns give the median of each, its spread (max - min ove
 staged.  The rate columns are the staged path's.  For the plain shapes it times torch.matmul (cuBLAS, bf16) as well: the
 rate this card reaches at its power limit.
 
+The evaluation forward's FC1 is timed both ways: 'gelu_h' (h alone from the epilogue) against the split form it replaces,
+the 'bf16' GEMM that writes z plus the stand-alone GELU kernel (its own row, "gelu kernel").
+
 --k-sweep times the wide-output GEMMs (qkv forward, FC1 forward with GELU, FC2 data gradient with dGELU) at their M x N
 with K = 768, 1536, 3072 and 6144 and BN = 128, and fits the time per wave of tiles, t_tile = a * k-blocks + e: e is the
 per-tile cost that does not scale with K (epilogue, pipeline fill), printed for both epilogues.
@@ -97,6 +100,8 @@ def cases(dev):
          dict(epi='f32', bias=bias_d, aux=stream, out=stream, aux_row=maps['sp_aux'], out_row=maps['sp_out'],
               row_map=aff['spatial']), 8, False),
         ('fc1 fwd (gelu)', M_TOK, HID, D, (0, 0), dict(epi='gelu', bias=bias_h), 4, False),
+        ('fc1 fwd eval (gelu_h)', M_TOK, HID, D, (0, 0), dict(epi='gelu_h', bias=bias_h), 2, False),
+        ('fc1 fwd split (bf16; + gelu kernel)', M_TOK, HID, D, (0, 0), dict(epi='bf16', bias=bias_h), 2, False),
         ('fc2 fwd (f32 residual)', M_TOK, D, HID, (0, 0), dict(epi='f32', bias=bias_d, aux=stream[:M_TOK]), 8, False),
         ('fc2 dgrad (dgelu)', M_TOK, HID, D, (0, 1), dict(epi='dgelu', aux=z), 4, False),
         ('fc1 dgrad', M_TOK, D, HID, (0, 1), dict(epi='bf16'), 2, True),
@@ -149,6 +154,14 @@ def shapes(K, dev, args, rows):
             rows.append(r)
             print(f'{name:38s} {M:6d} {N:5d} {Kd:6d} {"cublas":>6s} {"":>8s} {"":>5s} {us:8.1f} {"":>5s} {"":>7s} '
                   f'{r["tflops"]:8.1f} {"":>7s} {r["over_floor"]:7.2f}')
+        if name.startswith('fc1 fwd split'):
+            # the rest of the split form: vt_gelu_fwd_bf16 reads z and writes h (2 x M x N bf16)
+            z = torch.randn(M, N, device=dev).bfloat16()
+            us = 1e3 * events_ms(lambda: K.gelu(z), args.reps, args.warmup)
+            r = dict(gemm='gelu kernel (after fc1 split)', M=M, N=N, K=0, tile='-', us=us, gbs=4.0 * M * N / us * 1e-3)
+            rows.append(r)
+            print(f'{r["gemm"]:38s} {M:6d} {N:5d} {0:6d} {"-":>6s} {"":>8s} {"":>5s} {us:8.1f} {"":>5s} {"":>7s} '
+                  f'{"":>8s} {r["gbs"]:7.0f}')
 
 
 def k_sweep(K, dev, args, sms, rows):

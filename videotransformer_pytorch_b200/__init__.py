@@ -14,5 +14,6 @@ from .video_transformer import TimeSformer, ViViT, get_vit_base_patch16_224  # n
 from .maskfeat import MaskFeat  # noqa: F401
 from .mixup import MixedClip, Mixup  # noqa: F401
 from .ops import cross_entropy  # noqa: F401
+from .metrics import TopKAccuracy  # noqa: F401
 
 __version__ = '0.1.0'

@@ -15,7 +15,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libvt_b200.so')
 
-EPI = {'bf16': 0, 'f32': 1, 'gelu': 2, 'dgelu': 3}
+EPI = {'bf16': 0, 'f32': 1, 'gelu': 2, 'dgelu': 3, 'gelu_h': 4}
 
 c_i32, c_i64, c_f32, c_vp = C.c_int32, C.c_int64, C.c_float, C.c_void_p
 
@@ -209,6 +209,11 @@ class AttnProbsParams(C.Structure):
     _fields_ = [('qkv', c_vp), ('probs', c_vp), ('Bp', c_i32), ('N', c_i32), ('H', c_i32), ('hd', c_i32), ('scale', c_f32)]
 
 
+class TopkHitsParams(C.Structure):
+    _fields_ = [('logits', c_vp), ('labels', c_vp), ('probs', c_vp), ('hits', c_vp), ('samples', c_vp),
+                ('B', c_i32), ('V', c_i32), ('C', c_i32), ('n_k', c_i32), ('k', c_i32 * 4)]
+
+
 class Im2colU8MixParams(C.Structure):
     _fields_ = [('x', c_vp), ('scale', c_vp), ('shift', c_vp), ('plan', c_vp), ('cols', c_vp), ('B', c_i32), ('T', c_i32),
                 ('C', c_i32), ('H', c_i32), ('W', c_i32), ('tube', c_i32), ('ph', c_i32), ('pw', c_i32)]
@@ -228,7 +233,7 @@ EXPORTS = ['vt_version', 'vt_last_error', 'vt_sm_count', 'vt_set_reserved_sms', 
            'vt_maxpool_bwd', 'vt_im2col3d_bf16', 'vt_mvit_tokens_fwd', 'vt_mvit_tokens_bwd', 'vt_mse_blocks',
            'vt_mse_fwd', 'vt_mse_bwd', 'vt_opt_norm2', 'vt_opt_sgd', 'vt_opt_adamw',
            'vt_linear_small_fwd', 'vt_linear_small_bwd', 'vt_softmax_ce', 'vt_scale_by_scalar', 'vt_attn_probs',
-           'vt_im2col_u8_mix_bf16', 'vt_pos_resize_fwd', 'vt_pos_resize_bwd']
+           'vt_im2col_u8_mix_bf16', 'vt_pos_resize_fwd', 'vt_pos_resize_bwd', 'vt_topk_hits']
 
 _dll = None
 
@@ -283,6 +288,9 @@ class CudaKernels:
     """Tensor-level wrappers; every method enqueues on torch's current CUDA stream."""
 
     name = 'cuda'
+    # the forward-only forms ops.run dispatches to: the 'gelu_h' GEMM epilogue and stats=False / want_lse=False /
+    # want_idx=False (backward-only outputs not written)
+    inference_forms = True
 
     def __init__(self):
         self._ws = {}
@@ -363,19 +371,20 @@ class CudaKernels:
         return (out, out2) if epi == 'gelu' else out
 
     # -- LayerNorm ----------------------------------------------------------------------------
-    def ln_fwd(self, x2d, gamma, beta, eps, in_row=None, rows=None, out_fp32=False):
+    def ln_fwd(self, x2d, gamma, beta, eps, in_row=None, rows=None, out_fp32=False, stats=True):
+        """-> (y, mean, rstd); stats=False: the statistics are not written and come back as None."""
         lib = load_library()
         _rows2d(_req(x2d, torch.float32, 'ln_fwd.x'), 'ln_fwd.x')
         rows = x2d.shape[0] if rows is None else rows
         D = x2d.shape[1]
         y = torch.empty((rows, D), dtype=torch.float32 if out_fp32 else torch.bfloat16, device=x2d.device)
-        mean = torch.empty(rows, dtype=torch.float32, device=x2d.device)
-        rstd = torch.empty_like(mean)
+        mean = torch.empty(rows, dtype=torch.float32, device=x2d.device) if stats else None
+        rstd = torch.empty_like(mean) if stats else None
         p = LnFwdParams()
         p.x, p.ldx = x2d.data_ptr(), x2d.stride(0)
         p.in_row = _ptr(None if in_row is None else _req(in_row, torch.int32, 'ln_fwd.in_row'))
         p.gamma, p.beta = _req(gamma, torch.float32, 'gamma').data_ptr(), _req(beta, torch.float32, 'beta').data_ptr()
-        p.y, p.mean, p.rstd = y.data_ptr(), mean.data_ptr(), rstd.data_ptr()
+        p.y, p.mean, p.rstd = y.data_ptr(), _ptr(mean), _ptr(rstd)
         p.rows, p.D, p.eps, p.y_fp32 = rows, D, eps, int(out_fp32)
         _check(lib.vt_layernorm_fwd(C.byref(p), _stream()), 'vt_layernorm_fwd')
         return y, mean, rstd
@@ -538,16 +547,17 @@ class CudaKernels:
         return out
 
     # -- attention ----------------------------------------------------------------------------
-    def attn_fwd(self, qkv, Bp, N, H, hd, scale, want_probs=False, impl=0):
+    def attn_fwd(self, qkv, Bp, N, H, hd, scale, want_probs=False, impl=0, want_lse=True):
+        """-> (ctx, lse, probs); lse is None with want_lse=False (not written), probs None unless want_probs."""
         lib = load_library()
         _req(qkv, torch.bfloat16, 'attn.qkv')
         if not qkv.is_contiguous() or qkv.numel() != Bp * N * 3 * H * hd:
             raise RuntimeError('attn_fwd: qkv must be contiguous [Bp, N, 3, H, hd]')
         ctx = torch.empty((Bp * N, H * hd), dtype=torch.bfloat16, device=qkv.device)
-        lse = torch.empty((Bp, H, N), dtype=torch.float32, device=qkv.device)
+        lse = torch.empty((Bp, H, N), dtype=torch.float32, device=qkv.device) if want_lse else None
         probs = torch.empty((Bp, H, N, N), dtype=torch.float32, device=qkv.device) if want_probs else None
         p = AttnFwdParams()
-        p.qkv, p.ctx, p.lse, p.probs = qkv.data_ptr(), ctx.data_ptr(), lse.data_ptr(), _ptr(probs)
+        p.qkv, p.ctx, p.lse, p.probs = qkv.data_ptr(), ctx.data_ptr(), _ptr(lse), _ptr(probs)
         p.Bp, p.N, p.H, p.hd, p.scale, p.impl = Bp, N, H, hd, scale, impl
         _check(lib.vt_attn_fwd(C.byref(p), _stream()), 'vt_attn_fwd')
         return ctx, lse, probs
@@ -644,6 +654,35 @@ class CudaKernels:
         p.M, p.N = M, N
         _check(lib.vt_softmax_ce(C.byref(p), _stream()), 'vt_softmax_ce')
         return loss, dz, row
+
+    def topk_hits(self, logits, labels, views, ks, hits, samples, probs=None):
+        """Adds to the int64 device counters hits[i] the clips of this batch whose label ranks below ks[i] on the mean of
+        its `views` logit rows, and the clip count to samples[0]; probs (fp32 [B, C] or None) receives softmax(mean)."""
+        lib = load_library()
+        _req(logits, torch.float32, 'topk_hits.logits')
+        _req(labels, torch.int64, 'topk_hits.labels')
+        for t, n in ((hits, 'hits'), (samples, 'samples')):
+            _req(t, torch.int64, 'topk_hits.' + n)
+        if logits.dim() != 2 or not logits.is_contiguous() or not labels.is_contiguous():
+            raise RuntimeError('topk_hits: logits must be a contiguous [B*V, C] matrix and labels contiguous')
+        BV, Cn = logits.shape
+        B = labels.numel()
+        if BV != B * views:
+            raise RuntimeError(f'topk_hits: {BV} logit rows for {B} labels x {views} views')
+        ks = tuple(int(k) for k in ks)
+        if len(ks) > 4 or hits.numel() < len(ks):
+            raise RuntimeError('topk_hits: at most 4 k values, one hit counter each')
+        p = TopkHitsParams()
+        p.logits, p.labels, p.hits, p.samples = logits.data_ptr(), labels.data_ptr(), hits.data_ptr(), samples.data_ptr()
+        if probs is not None:
+            _req(probs, torch.float32, 'topk_hits.probs')
+            if not probs.is_contiguous() or tuple(probs.shape) != (B, Cn):
+                raise RuntimeError('topk_hits: probs must be a contiguous [B, C] matrix')
+            p.probs = probs.data_ptr()
+        p.B, p.V, p.C, p.n_k = B, views, Cn, len(ks)
+        for i, k in enumerate(ks):
+            p.k[i] = k
+        _check(lib.vt_topk_hits(C.byref(p), _stream()), 'vt_topk_hits')
 
     def scale_by_scalar(self, t, scalar):
         lib = load_library()
@@ -774,8 +813,9 @@ class CudaKernels:
             raise RuntimeError(f'{name}: expected a [B, N, H*hd] view with unit last stride, got {tuple(t.shape)} {t.stride()}')
         return t
 
-    def pool_fwd(self, src, H, hd, thw, stride, w, gamma, beta, eps):
-        """src: [B, 1+T*Hin*Win, H*hd] bf16 view -> (out bf16 [B,H,1+Lo,hd], pooled fp32, mean, rstd, out_thw)"""
+    def pool_fwd(self, src, H, hd, thw, stride, w, gamma, beta, eps, stats=True):
+        """src: [B, 1+T*Hin*Win, H*hd] bf16 view -> (out bf16 [B,H,1+Lo,hd], pooled fp32, mean, rstd, out_thw);
+        stats=False: pooled / mean / rstd are not written and come back as None."""
         lib = load_library()
         B = src.shape[0]
         self._tok_view(src, 'pool_fwd.src', B, H, hd)
@@ -785,15 +825,15 @@ class CudaKernels:
         To, Ho, Wo = self.pool_out_thw(thw, stride)
         Lo1 = 1 + To * Ho * Wo
         dev = src.device
-        pooled = torch.empty((B, H, Lo1, hd), dtype=torch.float32, device=dev)
+        pooled = torch.empty((B, H, Lo1, hd), dtype=torch.float32, device=dev) if stats else None
         out = torch.empty((B, H, Lo1, hd), dtype=torch.bfloat16, device=dev)
-        mean = torch.empty(B * H * Lo1, dtype=torch.float32, device=dev)
-        rstd = torch.empty_like(mean)
+        mean = torch.empty(B * H * Lo1, dtype=torch.float32, device=dev) if stats else None
+        rstd = torch.empty_like(mean) if stats else None
         p = PoolFwdParams()
         p.inp, p.in_bs, p.in_rs = src.data_ptr(), src.stride(0), src.stride(1)
         p.w = _req(w, torch.float32, 'pool_fwd.w').contiguous().data_ptr()
         p.gamma, p.beta = _req(gamma, torch.float32, 'gamma').data_ptr(), _req(beta, torch.float32, 'beta').data_ptr()
-        p.pooled, p.out, p.mean, p.rstd = pooled.data_ptr(), out.data_ptr(), mean.data_ptr(), rstd.data_ptr()
+        p.pooled, p.out, p.mean, p.rstd = _ptr(pooled), out.data_ptr(), _ptr(mean), _ptr(rstd)
         p.B, p.H, p.hd, p.T, p.Hin, p.Win = B, H, hd, T, Hin, Win
         p.st, p.sh, p.sw = stride
         p.To, p.Ho, p.Wo, p.eps = To, Ho, Wo, eps
@@ -841,19 +881,19 @@ class CudaKernels:
             raise RuntimeError(f'{name}: expected a [B,H,N,hd] view with unit last stride')
         return t.data_ptr(), t.stride(0), t.stride(1), t.stride(2)
 
-    def xattn_fwd(self, q, k, v, scale, impl=0):
-        """q [B,H,Nq,hd], k/v [B,H,Nk,hd] bf16 views -> (o bf16 [B, Nq, H*hd], lse fp32 [B,H,Nq])"""
+    def xattn_fwd(self, q, k, v, scale, impl=0, want_lse=True):
+        """q [B,H,Nq,hd], k/v [B,H,Nk,hd] bf16 views -> (o bf16 [B, Nq, H*hd], lse fp32 [B,H,Nq] | None if not want_lse)"""
         lib = load_library()
         B, H, Nq, hd = q.shape
         Nk = k.shape[2]
         o = torch.empty((B, Nq, H * hd), dtype=torch.bfloat16, device=q.device)
-        lse = torch.empty((B, H, Nq), dtype=torch.float32, device=q.device)
+        lse = torch.empty((B, H, Nq), dtype=torch.float32, device=q.device) if want_lse else None
         p = XattnFwdParams()
         p.q, p.q_bs, p.q_hs, p.q_rs = self._bhnd(q, 'xattn.q')
         p.k, p.k_bs, p.k_hs, p.k_rs = self._bhnd(k, 'xattn.k')
         p.v, p.v_bs, p.v_hs, p.v_rs = self._bhnd(v, 'xattn.v')
         p.o, p.o_bs, p.o_hs, p.o_rs = o.data_ptr(), Nq * H * hd, hd, H * hd
-        p.lse = lse.data_ptr()
+        p.lse = _ptr(lse)
         p.B, p.H, p.Nq, p.Nk, p.hd, p.scale, p.impl = B, H, Nq, Nk, hd, scale, impl
         _check(lib.vt_xattn_fwd(C.byref(p), _stream()), 'vt_xattn_fwd')
         return o, lse
@@ -894,8 +934,8 @@ class CudaKernels:
         p.st, p.sh, p.sw = stride
         p.To, p.Ho, p.Wo = self.maxpool_out_thw(thw, kernel, stride)
 
-    def maxpool_fwd(self, x, thw, kernel, stride):
-        """x fp32 [B, 1+T*H*W, D] -> (y fp32 [B, 1+Lo, D], idx u8, out_thw)"""
+    def maxpool_fwd(self, x, thw, kernel, stride, want_idx=True):
+        """x fp32 [B, 1+T*H*W, D] -> (y fp32 [B, 1+Lo, D], idx u8 | None if not want_idx, out_thw)"""
         lib = load_library()
         x = _req(x, torch.float32, 'maxpool.x')
         if not x.is_contiguous() or x.shape[1] != 1 + thw[0] * thw[1] * thw[2]:
@@ -904,9 +944,9 @@ class CudaKernels:
         out_thw = self.maxpool_out_thw(thw, kernel, stride)
         Lo1 = 1 + out_thw[0] * out_thw[1] * out_thw[2]
         y = torch.empty((B, Lo1, D), dtype=torch.float32, device=x.device)
-        idx = torch.empty((B, Lo1, D), dtype=torch.uint8, device=x.device)
+        idx = torch.empty((B, Lo1, D), dtype=torch.uint8, device=x.device) if want_idx else None
         p = MaxpoolFwdParams()
-        p.x, p.y, p.idx = x.data_ptr(), y.data_ptr(), idx.data_ptr()
+        p.x, p.y, p.idx = x.data_ptr(), y.data_ptr(), _ptr(idx)
         self._mp_dims(p, B, D, thw, kernel, stride)
         _check(lib.vt_maxpool_fwd(C.byref(p), _stream()), 'vt_maxpool_fwd')
         return y, idx, out_thw

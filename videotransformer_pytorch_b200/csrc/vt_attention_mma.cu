@@ -72,7 +72,8 @@ __device__ __forceinline__ void stage_row_stats(float* lse_s, float* del_s, cons
 }
 
 // ------------------------------------------------------------------------------------------------ forward
-template <int HD>
+// LSE = false: p.lse is not written (forward-only calls); a template flag, so the saving form's code is unchanged
+template <int HD, bool LSE>
 __global__ void __launch_bounds__(MMA_THREADS) attn_mma_fwd_kernel(const MmaAttn p) {
   constexpr int P = HD + 8, NB = HD / 8, KC = HD / 16;
   __shared__ __align__(16) __nv_bfloat16 Qs[MT * P];
@@ -159,7 +160,7 @@ __global__ void __launch_bounds__(MMA_THREADS) attn_mma_fwd_kernel(const MmaAttn
     if (r0 < p.Nq) *reinterpret_cast<uint32_t*>(ob + (long long)r0 * p.o_rs + nb * 8 + 2 * t) = pack_bf16x2(o[nb][0] * inv0, o[nb][1] * inv0);
     if (r1 < p.Nq) *reinterpret_cast<uint32_t*>(ob + (long long)r1 * p.o_rs + nb * 8 + 2 * t) = pack_bf16x2(o[nb][2] * inv1, o[nb][3] * inv1);
   }
-  if (t == 0) {
+  if (LSE && t == 0) {
     if (r0 < p.Nq) p.lse[(long long)bh * p.Nq + r0] = (m0 + log2f(l0)) * MMA_LN2;
     if (r1 < p.Nq) p.lse[(long long)bh * p.Nq + r1] = (m1 + log2f(l1)) * MMA_LN2;
   }
@@ -384,8 +385,9 @@ int attn_mma_fwd(const MmaAttn& a, int B, int hd, cudaStream_t st) {
   VT_REQUIRE(hd == 64 || hd == 96, "tensor-core attention: head dim %d unsupported (64 or 96)", hd);
   VT_REQUIRE((long long)B * a.H <= 65535, "tensor-core attention: B*H too large");
   const dim3 grid((a.Nq + MT - 1) / MT, B * a.H);
-  if (hd == 64) attn_mma_fwd_kernel<64><<<grid, MMA_THREADS, 0, st>>>(a);
-  else attn_mma_fwd_kernel<96><<<grid, MMA_THREADS, 0, st>>>(a);
+  const bool lse = a.lse != nullptr;
+  if (hd == 64) (lse ? attn_mma_fwd_kernel<64, true> : attn_mma_fwd_kernel<64, false>)<<<grid, MMA_THREADS, 0, st>>>(a);
+  else (lse ? attn_mma_fwd_kernel<96, true> : attn_mma_fwd_kernel<96, false>)<<<grid, MMA_THREADS, 0, st>>>(a);
   return check_launch("attn_mma_fwd_kernel");
 }
 

@@ -82,7 +82,7 @@ attn8_fwd_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
     const float inv = 1.0f / l;
     Ps[i * 9 + 2 * g] = e0 * inv;
     Ps[i * 9 + 2 * g + 1] = e1 * inv;
-    if (g == 0) lse[(long long)prob * SM_N + i] = m + __logf(l);
+    if (g == 0 && lse) lse[(long long)prob * SM_N + i] = m + __logf(l);
     __syncwarp();
     float acc[16];
 #pragma unroll

@@ -97,7 +97,7 @@ ln_fwd_kernel(const float* __restrict__ x, long long ldx, const int* __restrict_
       ss += (a * a + bb * bb) + (c * c + d * d);
     }
     const float rs = rsqrtf(warp_sum(ss) * (1.0f / D) + eps);
-    if (lane == 0) {
+    if (lane == 0 && mean) {   // mean / rstd NULL: not written
       mean[m] = mu;
       rstd[m] = rs;
     }
@@ -749,7 +749,8 @@ extern "C" int vt_set_reserved_sms(int n) {
 extern "C" int vt_launch_count(void) { return (int)(__atomic_load_n(&g_launches, __ATOMIC_RELAXED) & 0x7fffffffull); }
 
 extern "C" int vt_layernorm_fwd(const vt_ln_fwd_params* p, void* stream) {
-  VT_REQUIRE(p && p->x && p->gamma && p->beta && p->y && p->mean && p->rstd, "vt_layernorm_fwd: null pointer");
+  VT_REQUIRE(p && p->x && p->gamma && p->beta && p->y, "vt_layernorm_fwd: null pointer");
+  VT_REQUIRE((p->mean == nullptr) == (p->rstd == nullptr), "vt_layernorm_fwd: mean and rstd are both given or both NULL");
   VT_REQUIRE(p->rows > 0, "vt_layernorm_fwd: rows=%d", p->rows);
   if (p->D % 128 != 0) return layernorm_fwd_small(p, stream);
   VT_REQUIRE(p->D % 128 == 0 && p->D >= 128 && p->D <= 1024, "vt_layernorm_fwd: D=%d unsupported (multiple of 128, <=1024)", p->D);

@@ -43,7 +43,7 @@ struct GemmDev {
   long long special_ld;
 };
 
-// Epilogue kinds (kernel template parameter SE): 0 = from registers; 1 = one staged bf16 output (VT_EPI_BF16);
+// Epilogue kinds (kernel template parameter SE): 0 = from registers; 1 = one staged bf16 output (VT_EPI_BF16, VT_EPI_GELU_H);
 // 2 = two staged bf16 tiles (VT_EPI_GELU: z and h; VT_EPI_DGELU: dz and the TMA-loaded z).
 constexpr int EPI_BOX_BYTES = 64 * 64 * 2;   // one 64-row x 64-column bf16 box, 128B-swizzled as TMA reads / writes it
 
@@ -144,6 +144,8 @@ __device__ __forceinline__ void epi_pair(const GemmDev& p, const EpiRow& r, int 
       a.x += b2.x; a.y += b2.y;
     }
     *reinterpret_cast<float2*>(reinterpret_cast<float*>(r.out) + n) = make_float2(fmaf(r.s, v0, a.x), fmaf(r.s, v1, a.y));
+  } else if (p.epi == VT_EPI_GELU_H) {
+    *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(r.out) + n) = gelu_pair(pack_bf16x2(r.s * v0, r.s * v1));
   } else if (p.epi == VT_EPI_GELU) {
     const uint32_t z = pack_bf16x2(v0, v1);
     *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(r.out) + n) = z;
@@ -164,7 +166,7 @@ __device__ __forceinline__ void epi_stage(const GemmDev& p, const float (&acc)[B
                                           int row0, int n0, int warp, int lane) {
   const int r = warp * 16 + (lane >> 2);          // rows r and r + 8 of the 64-row half; r % 8 == lane / 4
   float s[2] = {1.0f, 1.0f};
-  if (EPI == VT_EPI_BF16 && p.row_scale) {
+  if ((EPI == VT_EPI_BF16 || EPI == VT_EPI_GELU_H) && p.row_scale) {
 #pragma unroll
     for (int h = 0; h < 2; ++h)
       if (row0 + r + 8 * h < p.M) s[h] = p.row_scale[row0 + r + 8 * h];
@@ -184,6 +186,8 @@ __device__ __forceinline__ void epi_stage(const GemmDev& p, const float (&acc)[B
       add_bias(p, n, v0, v1);
       if (EPI == VT_EPI_BF16) {
         st_shared_u32(o, pack_bf16x2(s[h] * v0, s[h] * v1));
+      } else if (EPI == VT_EPI_GELU_H) {
+        st_shared_u32(o, gelu_pair(pack_bf16x2(s[h] * v0, s[h] * v1)));
       } else if (EPI == VT_EPI_GELU) {
         const uint32_t z = pack_bf16x2(v0, v1);
         st_shared_u32(o, z);
@@ -335,7 +339,8 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       if (load_z) mbar_wait(zfull_bar, tj & 1);
       if (leader) tma_store_wait_read_all();       // the previous tile's store has read the staging boxes
       named_bar_sync(1 + cw, 128);
-      if (SE == 1) epi_stage<BN, VT_EPI_BF16>(p, acc, stage, stage2, row0, c.n0, warp, lane);
+      if (SE == 1 && p.epi == VT_EPI_GELU_H) epi_stage<BN, VT_EPI_GELU_H>(p, acc, stage, stage2, row0, c.n0, warp, lane);
+      else if (SE == 1) epi_stage<BN, VT_EPI_BF16>(p, acc, stage, stage2, row0, c.n0, warp, lane);
       else if (p.epi == VT_EPI_GELU) epi_stage<BN, VT_EPI_GELU>(p, acc, stage, stage2, row0, c.n0, warp, lane);
       else epi_stage<BN, VT_EPI_DGELU>(p, acc, stage, stage2, row0, c.n0, warp, lane);
       fence_proxy_async_smem();
@@ -507,7 +512,7 @@ static int launch_layout(const vt_gemm_params* q, const CUtensorMap (&tm)[4], co
 static int staged_kind(const vt_gemm_params* q) {
   if (q->epilogue == VT_EPI_F32 || q->out_row) return 0;
   if (!feature_on("VT_GEMM_STAGED_EPI", VT_DEFAULT_STAGED_EPI)) return 0;
-  if (q->epilogue == VT_EPI_BF16) return 1;
+  if (q->epilogue == VT_EPI_BF16 || q->epilogue == VT_EPI_GELU_H) return 1;
   // GELU's out2 is not checked by the register path's alignment rule; TMA needs it 16-byte aligned
   if (q->epilogue == VT_EPI_GELU && ((reinterpret_cast<uintptr_t>(q->out2) & 15) || (q->ldo2 * 2) % 16)) return 0;
   return 2;
@@ -602,7 +607,7 @@ static int gemm_dispatch(const vt_gemm_params* q, void* stream) {
   VT_REQUIRE(q->M > 0 && q->N > 0 && q->K > 0, "vt_gemm: bad shape M=%d N=%d K=%d", q->M, q->N, q->K);
   VT_REQUIRE(q->N % 8 == 0, "vt_gemm: N must be a multiple of 8 (got %d)", q->N);
   VT_REQUIRE(q->a && q->b && q->out, "vt_gemm: null operand");
-  VT_REQUIRE(q->epilogue >= VT_EPI_BF16 && q->epilogue <= VT_EPI_DGELU, "vt_gemm: bad epilogue %d", q->epilogue);
+  VT_REQUIRE(q->epilogue >= VT_EPI_BF16 && q->epilogue <= VT_EPI_GELU_H, "vt_gemm: bad epilogue %d", q->epilogue);
   if (q->epilogue == VT_EPI_GELU) VT_REQUIRE(q->out2 != nullptr, "vt_gemm: VT_EPI_GELU needs out2");
   if (q->epilogue == VT_EPI_DGELU) VT_REQUIRE(q->aux != nullptr, "vt_gemm: VT_EPI_DGELU needs aux (z)");
   const int esz = (q->epilogue == VT_EPI_F32) ? 4 : 2;

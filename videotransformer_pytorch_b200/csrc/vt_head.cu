@@ -3,6 +3,7 @@
 //   * softmax cross-entropy (hard labels or soft targets) forward + gradient in one launch
 //   * attention probabilities softmax(q k^T * scale) for long sequences (get_last_selfattention of the joint variants)
 //   * uint8 clip -> normalised bf16 patch operand with Mixup / CutMix of the flipped batch folded in
+//   * top-k hit counters of an evaluation step (view mean, optional softmax, rank of the label)
 // All are latency / bandwidth bound warp-primitive kernels (no tensor cores: M <= 64 rows or one-off visualisation work).
 #include "vt_common.cuh"
 
@@ -362,6 +363,89 @@ extern "C" int vt_im2col_u8_mix_bf16(const vt_im2col_u8_mix_params* p, void* str
       p->x, p->scale, p->shift, p->plan, static_cast<__nv_bfloat16*>(p->cols), p->B, p->T, p->C, p->H, p->W, p->tube, p->ph,
       p->pw, total8);
   return check_launch("im2col_u8_mix_kernel");
+}
+
+// ------------------------------------------------------------------------------------------------
+// Top-k hits of one evaluation batch: one CTA per clip.  The clip's V view rows are averaged into shared memory (summed
+// in view order, then scaled by 1/V as torch's mean does: preds.view(-1, V, C).mean(1)); rank = number of classes whose mean is strictly
+// greater than the label's; counter i gains 1 when rank < k[i].  Integer atomics: the totals do not depend on the order
+// the CTAs finish in, and nothing is allocated or synchronised, so the kernel can be captured in a CUDA graph.
+// ------------------------------------------------------------------------------------------------
+namespace vt {
+constexpr int TK_THREADS = 256;
+
+__global__ void __launch_bounds__(TK_THREADS)
+topk_hits_kernel(const float* __restrict__ logits, const int64_t* __restrict__ labels, float* __restrict__ probs,
+                 unsigned long long* __restrict__ hits, unsigned long long* __restrict__ samples, int B, int V, int C,
+                 int4 ks, int n_k) {
+  extern __shared__ float tk_mean[];
+  __shared__ float red_f[TK_THREADS / 32];
+  __shared__ int red_i[TK_THREADS / 32];
+  const int b = blockIdx.x, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const float* z = logits + (long long)b * V * C;
+  const float inv_v = 1.0f / (float)V;
+  for (int c = threadIdx.x; c < C; c += TK_THREADS) {
+    float m = z[c];
+    for (int v = 1; v < V; ++v) m += z[(long long)v * C + c];
+    tk_mean[c] = m * inv_v;
+  }
+  __syncthreads();
+  const long long lab = labels[b];
+  const bool lab_ok = lab >= 0 && lab < C;
+  const float ml = lab_ok ? tk_mean[lab] : 0.f;
+  int above = 0;
+  for (int c = threadIdx.x; c < C; c += TK_THREADS) above += tk_mean[c] > ml;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) above += __shfl_xor_sync(0xffffffffu, above, o);
+  if (lane == 0) red_i[warp] = above;
+  if (probs) {
+    float mx = -INFINITY;
+    for (int c = threadIdx.x; c < C; c += TK_THREADS) mx = fmaxf(mx, tk_mean[c]);
+    mx = warp_max(mx);
+    if (lane == 0) red_f[warp] = mx;
+    __syncthreads();
+    mx = red_f[0];
+#pragma unroll
+    for (int i = 1; i < TK_THREADS / 32; ++i) mx = fmaxf(mx, red_f[i]);
+    float se = 0.f;
+    for (int c = threadIdx.x; c < C; c += TK_THREADS) se += expf(tk_mean[c] - mx);
+    se = warp_sum(se);
+    __syncthreads();
+    if (lane == 0) red_f[warp] = se;
+    __syncthreads();
+    se = red_f[0];
+#pragma unroll
+    for (int i = 1; i < TK_THREADS / 32; ++i) se += red_f[i];
+    const float inv = 1.0f / se;
+    for (int c = threadIdx.x; c < C; c += TK_THREADS) probs[(long long)b * C + c] = expf(tk_mean[c] - mx) * inv;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int rank = 0;
+#pragma unroll
+    for (int i = 0; i < TK_THREADS / 32; ++i) rank += red_i[i];
+    if (!lab_ok || ml != ml) rank = C;             // label out of range or NaN score: a miss for every k
+    const int kk[4] = {ks.x, ks.y, ks.z, ks.w};
+    for (int i = 0; i < n_k; ++i)
+      if (rank < kk[i]) atomicAdd(hits + i, 1ull);
+    if (b == 0) atomicAdd(samples, (unsigned long long)B);
+  }
+}
+}  // namespace vt
+
+extern "C" int vt_topk_hits(const vt_topk_hits_params* p, void* stream) {
+  using namespace vt;
+  VT_REQUIRE(p && p->logits && p->labels && p->hits && p->samples, "vt_topk_hits: null pointer");
+  VT_REQUIRE(p->B > 0 && p->V > 0 && p->C > 0, "vt_topk_hits: bad shape B=%d V=%d C=%d", p->B, p->V, p->C);
+  VT_REQUIRE(p->C <= 12000, "vt_topk_hits: C=%d classes unsupported (<= 12000)", p->C);   // the means fit 48 KiB of shared memory
+  VT_REQUIRE(p->n_k >= 0 && p->n_k <= 4, "vt_topk_hits: n_k=%d (0..4)", p->n_k);
+  VT_REQUIRE(((reinterpret_cast<uintptr_t>(p->hits) | reinterpret_cast<uintptr_t>(p->samples)) & 7) == 0,
+             "vt_topk_hits: counters must be 8-byte aligned");
+  const int4 ks = make_int4(p->k[0], p->k[1], p->k[2], p->k[3]);
+  topk_hits_kernel<<<p->B, TK_THREADS, p->C * sizeof(float), static_cast<cudaStream_t>(stream)>>>(
+      p->logits, p->labels, p->probs, reinterpret_cast<unsigned long long*>(p->hits),
+      reinterpret_cast<unsigned long long*>(p->samples), p->B, p->V, p->C, ks, p->n_k);
+  return check_launch("topk_hits_kernel");
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -32,7 +32,8 @@ __device__ __forceinline__ float bf2f(const __nv_bfloat16* p) { return __bfloat1
 // LayerNorm for narrow rows: D = 32*E, one warp per row, lane owns columns lane + 32*i (coalesced 128-B segments).
 // Same contract as ln_fwd_kernel / ln_bwd_kernel of vt_elementwise.cu without row maps.
 // ================================================================================================
-template <int E>
+// STATS = false: mean / rstd are not written (forward-only calls); a template flag, so the saving form's code is unchanged
+template <int E, bool STATS>
 __global__ void __launch_bounds__(ROW_WARPS * 32)
 ln_small_fwd_kernel(const float* __restrict__ x, long long ldx, const float* __restrict__ gamma,
                     const float* __restrict__ beta, void* __restrict__ y, float* __restrict__ mean,
@@ -54,7 +55,8 @@ ln_small_fwd_kernel(const float* __restrict__ x, long long ldx, const float* __r
       v[i] = xr[lane + 32 * i];
       s += v[i];
     }
-    const float mu = warp_sum(s) * (1.0f / D);
+    // rounded before use (never contracted into the subtractions below), so both STATS forms give the same bits
+    const float mu = __fmul_rn(warp_sum(s), 1.0f / D);
     float ss = 0.f;
 #pragma unroll
     for (int i = 0; i < E; ++i) {
@@ -62,7 +64,7 @@ ln_small_fwd_kernel(const float* __restrict__ x, long long ldx, const float* __r
       ss += d * d;
     }
     const float rs = rsqrtf(warp_sum(ss) * (1.0f / D) + eps);
-    if (lane == 0) {
+    if (STATS && lane == 0) {
       mean[m] = mu;
       rstd[m] = rs;
     }
@@ -141,7 +143,8 @@ struct PoolDims {
   int B, H, T, Hin, Win, st, sh, sw, To, Ho, Wo;
 };
 
-template <int E>
+// STATS = false: pooled / mean / rstd are not written (forward-only calls)
+template <int E, bool STATS>
 __global__ void __launch_bounds__(ROW_WARPS * 32)
 pool_ln_fwd_kernel(const __nv_bfloat16* __restrict__ in, long long in_bs, long long in_rs,
                    const float* __restrict__ w, const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -215,7 +218,7 @@ pool_ln_fwd_kernel(const __nv_bfloat16* __restrict__ in, long long in_bs, long l
     float s = 0.f;
 #pragma unroll
     for (int i = 0; i < E; ++i) s += acc[i];
-    const float mu = warp_sum(s) * (1.0f / HD);
+    const float mu = __fmul_rn(warp_sum(s), 1.0f / HD);   // rounded before use, as in ln_small_fwd_kernel
     float ss = 0.f;
 #pragma unroll
     for (int i = 0; i < E; ++i) {
@@ -223,13 +226,13 @@ pool_ln_fwd_kernel(const __nv_bfloat16* __restrict__ in, long long in_bs, long l
       ss += c * c;
     }
     const float rs = rsqrtf(warp_sum(ss) * (1.0f / HD) + eps);
-    if (lane == 0) {
+    if (STATS && lane == 0) {
       mean[r] = mu;
       rstd[r] = rs;
     }
 #pragma unroll
     for (int i = 0; i < E; ++i) {
-      pooled[(long long)r * HD + lane + 32 * i] = acc[i];
+      if (STATS) pooled[(long long)r * HD + lane + 32 * i] = acc[i];
       out[(long long)r * HD + lane + 32 * i] = __float2bfloat16_rn((acc[i] - mu) * rs * g[i] + bt[i]);
     }
   }
@@ -608,7 +611,7 @@ __device__ __forceinline__ void stage_rows(float* __restrict__ dst, const __nv_b
   }
 }
 
-template <int HD>
+template <int HD, bool LSE>   // LSE = false: lse is not written (forward-only calls)
 __global__ void __launch_bounds__(2 * XA_QPB)
 xattn_fwd_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ k,
                  const __nv_bfloat16* __restrict__ v, __nv_bfloat16* __restrict__ o, float* __restrict__ lse,
@@ -687,7 +690,7 @@ xattn_fwd_kernel(const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __res
 #pragma unroll
     for (int d2 = 0; d2 < HALF / 2; ++d2)
       *reinterpret_cast<uint32_t*>(op + 2 * d2) = pack_bf16x2(acc[2 * d2] * inv, acc[2 * d2 + 1] * inv);
-    if (half == 0) lse[(long long)bh * Nq + qi] = (m + log2f(l)) * LN2;
+    if (LSE && half == 0) lse[(long long)bh * Nq + qi] = (m + log2f(l)) * LN2;
   }
 }
 
@@ -878,6 +881,7 @@ struct MpDims {
 };
 
 // four channels per thread: the window walk (divisions, bounds) is shared by a float4 of channels
+template <bool IDX>   // IDX = false: the winners are not recorded (forward-only calls)
 __global__ void maxpool_fwd_kernel(const float* __restrict__ x, float* __restrict__ y, uint8_t* __restrict__ idx, MpDims d) {
   const int Lo1 = 1 + d.To * d.Ho * d.Wo, L1 = 1 + d.T * d.H * d.W;
   const int D4 = d.D / 4;
@@ -892,7 +896,7 @@ __global__ void maxpool_fwd_kernel(const float* __restrict__ x, float* __restric
     uchar4* io = reinterpret_cast<uchar4*>(idx) + e;
     if (l == 0) {
       *yo = xb[0];
-      *io = make_uchar4(0, 0, 0, 0);
+      if (IDX) *io = make_uchar4(0, 0, 0, 0);
       continue;
     }
     const int o = l - 1;
@@ -918,7 +922,7 @@ __global__ void maxpool_fwd_kernel(const float* __restrict__ x, float* __restric
       }
     }
     *yo = best;
-    *io = make_uchar4((unsigned char)ax, (unsigned char)ay, (unsigned char)az, (unsigned char)aw);
+    if (IDX) *io = make_uchar4((unsigned char)ax, (unsigned char)ay, (unsigned char)az, (unsigned char)aw);
   }
 }
 
@@ -1176,8 +1180,8 @@ int vt::layernorm_fwd_small(const vt_ln_fwd_params* p, void* stream) {
   const int blocks = row_blocks(p->rows, 4);
 #define VT_CASE(E)                                                                                                    \
   case E:                                                                                                             \
-    ln_small_fwd_kernel<E><<<blocks, ROW_WARPS * 32, 0, st>>>(p->x, p->ldx, p->gamma, p->beta, p->y, p->mean, p->rstd, \
-                                                              p->rows, p->eps, p->y_fp32);                            \
+    (p->mean ? ln_small_fwd_kernel<E, true> : ln_small_fwd_kernel<E, false>)<<<blocks, ROW_WARPS * 32, 0, st>>>(          \
+        p->x, p->ldx, p->gamma, p->beta, p->y, p->mean, p->rstd, p->rows, p->eps, p->y_fp32);                          \
     break;
   switch (p->D / 32) { VT_CASE(1) VT_CASE(2) VT_CASE(3) VT_CASE(4) VT_CASE(5) VT_CASE(6) VT_CASE(7) VT_CASE(8) }
 #undef VT_CASE
@@ -1213,14 +1217,17 @@ static int pool_dims_ok(int T, int Hin, int Win, int st, int sh, int sw, int To,
 }
 
 extern "C" int vt_pool_fwd(const vt_pool_fwd_params* p, void* stream) {
-  VT_REQUIRE(p && p->in && p->w && p->gamma && p->beta && p->pooled && p->out && p->mean && p->rstd, "vt_pool_fwd: null pointer");
+  VT_REQUIRE(p && p->in && p->w && p->gamma && p->beta && p->out, "vt_pool_fwd: null pointer");
+  VT_REQUIRE((p->pooled == nullptr) == (p->mean == nullptr) && (p->mean == nullptr) == (p->rstd == nullptr),
+             "vt_pool_fwd: pooled, mean and rstd are all given or all NULL");
   VT_REQUIRE(p->hd == 96, "vt_pool_fwd: head dim %d unsupported (96 only)", p->hd);
   VT_REQUIRE(p->B > 0 && p->H > 0 && p->T > 0 && p->Hin > 0 && p->Win > 0, "vt_pool_fwd: bad dims");
   VT_REQUIRE(pool_dims_ok(p->T, p->Hin, p->Win, p->st, p->sh, p->sw, p->To, p->Ho, p->Wo), "vt_pool_fwd: output dims inconsistent");
   const PoolDims d{p->B, p->H, p->T, p->Hin, p->Win, p->st, p->sh, p->sw, p->To, p->Ho, p->Wo};
   const long long rows = (long long)p->B * p->H * (1 + (long long)p->To * p->Ho * p->Wo);
   VT_REQUIRE(rows < 0x7fffffffll, "vt_pool_fwd: too many rows");
-  pool_ln_fwd_kernel<3><<<row_blocks(rows, 8), ROW_WARPS * 32, 0, static_cast<cudaStream_t>(stream)>>>(
+  (p->pooled ? pool_ln_fwd_kernel<3, true> : pool_ln_fwd_kernel<3, false>)<<<row_blocks(rows, 8), ROW_WARPS * 32, 0,
+                                                                             static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(p->in), p->in_bs, p->in_rs, p->w, p->gamma, p->beta, p->pooled,
       static_cast<__nv_bfloat16*>(p->out), p->mean, p->rstd, d, p->eps);
   return check_launch("pool_ln_fwd_kernel");
@@ -1337,7 +1344,7 @@ static int xa_strides_ok(const long long* s, int n) {
 }
 
 extern "C" int vt_xattn_fwd(const vt_xattn_fwd_params* p, void* stream) {
-  VT_REQUIRE(p && p->q && p->k && p->v && p->o && p->lse, "vt_xattn_fwd: null pointer");
+  VT_REQUIRE(p && p->q && p->k && p->v && p->o, "vt_xattn_fwd: null pointer");   // lse may be NULL (not written)
   VT_REQUIRE(p->hd == 96 || p->hd == 64, "vt_xattn_fwd: head dim %d unsupported (64 or 96)", p->hd);
   VT_REQUIRE(p->B > 0 && p->H > 0 && p->Nq > 0 && p->Nk > 0 && (long long)p->B * p->H <= 65535, "vt_xattn_fwd: bad dims");
   VT_REQUIRE(p->impl >= VT_XATTN_AUTO && p->impl <= VT_XATTN_TCGEN05, "vt_xattn_fwd: bad impl %d", p->impl);
@@ -1353,7 +1360,8 @@ extern "C" int vt_xattn_fwd(const vt_xattn_fwd_params* p, void* stream) {
   VT_REQUIRE(((uintptr_t)p->q | (uintptr_t)p->k | (uintptr_t)p->v | (uintptr_t)p->o) % 4 == 0, "vt_xattn_fwd: pointers must be 4-byte aligned");
   const XaStrides s{p->q_bs, p->q_hs, p->q_rs, p->k_bs, p->k_hs, p->k_rs, p->v_bs, p->v_hs, p->v_rs, p->o_bs, p->o_hs, p->o_rs, 0, 0, 0};
   dim3 grid((p->Nq + XA_QPB - 1) / XA_QPB, p->B * p->H);
-  auto kern = p->hd == 96 ? xattn_fwd_kernel<96> : xattn_fwd_kernel<64>;
+  auto kern = p->hd == 96 ? (p->lse ? xattn_fwd_kernel<96, true> : xattn_fwd_kernel<96, false>)
+                          : (p->lse ? xattn_fwd_kernel<64, true> : xattn_fwd_kernel<64, false>);
   kern<<<grid, 2 * XA_QPB, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const __nv_bfloat16*>(p->q), static_cast<const __nv_bfloat16*>(p->k), static_cast<const __nv_bfloat16*>(p->v),
       static_cast<__nv_bfloat16*>(p->o), p->lse, s, p->H, p->Nq, p->Nk, p->scale);
@@ -1417,11 +1425,12 @@ static int mp_dims_ok(const MpDims& d) {
 }
 
 extern "C" int vt_maxpool_fwd(const vt_maxpool_fwd_params* p, void* stream) {
-  VT_REQUIRE(p && p->x && p->y && p->idx && p->B > 0 && p->D > 0 && p->D % 4 == 0, "vt_maxpool_fwd: bad params (D %% 4 == 0 required)");
+  VT_REQUIRE(p && p->x && p->y && p->B > 0 && p->D > 0 && p->D % 4 == 0, "vt_maxpool_fwd: bad params (D %% 4 == 0 required)");
   const MpDims d{p->B, p->D, p->T, p->H, p->W, p->kt, p->kh, p->kw, p->st, p->sh, p->sw, p->To, p->Ho, p->Wo};
   VT_REQUIRE(mp_dims_ok(d), "vt_maxpool_fwd: inconsistent geometry");
   const long long n = (long long)p->B * (1 + (long long)p->To * p->Ho * p->Wo) * (p->D / 4);
-  maxpool_fwd_kernel<<<flat_blocks(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(p->x, p->y, p->idx, d);
+  (p->idx ? maxpool_fwd_kernel<true> : maxpool_fwd_kernel<false>)<<<flat_blocks(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
+      p->x, p->y, p->idx, d);
   return check_launch("maxpool_fwd_kernel");
 }
 

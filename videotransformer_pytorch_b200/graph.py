@@ -1,4 +1,5 @@
-"""CUDA-graph capture of one training step (forward + backward [+ gradient all-reduce]).
+"""CUDA-graph capture of one training step (forward + backward [+ gradient all-reduce]), and of one forward alone
+(`GraphedForward`: validation / test steps).
 
 A TimeSformer-B step is ~850 kernel launches of 5-150 us each; issued one by one from Python they make the
 step launch-bound long before the kernels are.  `GraphedTrainStep` records the whole step once and replays
@@ -17,7 +18,7 @@ from typing import Callable, Optional, Sequence
 
 import torch
 
-from . import ops
+from . import metrics, ops
 
 
 class MaskArena:
@@ -163,3 +164,55 @@ class GraphedTrainStep:
                 if p_.grad is not g_:
                     p_.grad = g_
         return self.static_loss
+
+
+class _NoMasks:
+    """Mask arena of GraphedForward: a forward that would draw DropPath masks (training mode) is refused."""
+    recording = True
+
+    def register(self, n0: int, keep: float):
+        raise RuntimeError('GraphedForward: the forward draws DropPath masks; put the model in eval mode')
+
+
+class GraphedForward:
+    """out = fwd(*inputs): replays  `with torch.no_grad(): out = fn(*static_inputs)`  as one CUDA graph.
+
+    For evaluation: the model must be in eval mode (a captured forward that draws DropPath masks is refused).  The module
+    forwards take their forward-only form under no_grad (ops.run), and the bf16 weight shadows are re-cast from the fp32
+    parameters inside the graph, so training steps between two replays are picked up.  `fn` may also update device-side
+    metrics (metrics.TopKAccuracy.update) from its inputs; those launches are replayed with the rest.  The eager warm-up
+    runs on the example inputs leave those metrics as they found them, so after construction they count the replayed
+    batches only.  The returned output is a static tensor, rewritten by the next replay.
+    """
+
+    def __init__(self, fn: Callable, example_inputs: Sequence[torch.Tensor], warmup: int = 2):
+        self.fn = fn
+        dev = example_inputs[0].device
+        if dev.type != 'cuda':
+            raise RuntimeError('GraphedForward needs CUDA tensors')
+        self.static_inputs = [t.clone() for t in example_inputs]
+        side = torch.cuda.Stream(device=dev)
+        from . import _lib
+        ops.set_mask_arena(_NoMasks())
+        try:
+            side.wait_stream(torch.cuda.current_stream(dev))
+            with torch.cuda.stream(side), torch.no_grad(), metrics.restored_after():
+                for _ in range(max(warmup, 1)):  # eager warm-up: kernel attributes, index maps, allocator, metric counters
+                    fn(*self.static_inputs)
+            torch.cuda.current_stream(dev).wait_stream(side)
+            torch.cuda.synchronize(dev)
+            self.graph = torch.cuda.CUDAGraph()
+            launches_before = _lib.launch_count()
+            with torch.cuda.graph(self.graph, stream=side), torch.no_grad():
+                self.static_output = fn(*self.static_inputs)
+        finally:
+            ops.set_mask_arena(None)
+        # libvt_b200 kernels recorded in the graph == launched by every replay
+        self.kernels_per_replay = _lib.launch_count() - launches_before
+
+    def __call__(self, *inputs):
+        for dst, src in zip(self.static_inputs, inputs):
+            if dst.data_ptr() != src.data_ptr():
+                dst.copy_(src, non_blocking=True)
+        self.graph.replay()
+        return self.static_output

@@ -18,7 +18,7 @@ from __future__ import annotations
 import torch
 import torch.nn as nn
 
-from . import mvit_ops
+from . import mvit_ops, ops
 from .ops import RowsNormFn
 from .transformer import ShadowWeights, _f32
 
@@ -142,14 +142,14 @@ class MultiScaleBlock(nn.Module):
         f = _f32
         pq = (f(a.pool_q.weight), f(a.norm_q.weight), f(a.norm_q.bias)) if self.stride_q is not None else (None, None, None)
         meta = (a.num_heads, tuple(thw), self.stride_q, self.stride_kv, self.norm1.eps, a.norm_k.eps)
-        x = mvit_ops.PoolAttnFn.apply(
-            x, f(self.norm1.weight), f(self.norm1.bias), f(a.q.weight), f(a.q.bias), f(a.k.weight), f(a.k.bias),
+        x = ops.run(
+            mvit_ops.PoolAttnFn, x, f(self.norm1.weight), f(self.norm1.bias), f(a.q.weight), f(a.q.bias), f(a.k.weight), f(a.k.bias),
             f(a.v.weight), f(a.v.bias), f(a.proj.weight), f(a.proj.bias), *pq,
             f(a.pool_k.weight), f(a.norm_k.weight), f(a.norm_k.bias), f(a.pool_v.weight), f(a.norm_v.weight), f(a.norm_v.bias),
             qkv_wh, sh.get('proj', a.proj.weight), meta)
         has_proj = self.dim != self.dim_out
-        x = mvit_ops.MlpFn.apply(
-            x, f(self.norm2.weight), f(self.norm2.bias), f(self.mlp.fc1.weight), f(self.mlp.fc1.bias),
+        x = ops.run(
+            mvit_ops.MlpFn, x, f(self.norm2.weight), f(self.norm2.bias), f(self.mlp.fc1.weight), f(self.mlp.fc1.bias),
             f(self.mlp.fc2.weight), f(self.mlp.fc2.bias),
             f(self.proj.weight) if has_proj else None, f(self.proj.bias) if has_proj else None,
             sh.get('fc1', self.mlp.fc1.weight), sh.get('fc2', self.mlp.fc2.weight),
@@ -171,7 +171,7 @@ class MultiscaleVisionTransformers(nn.Module):
         for blk in self.blocks:
             x, thw = blk(x, thw)
         B, N, D = x.shape
-        y = RowsNormFn.apply(x, _f32(self.norm_embed.weight), _f32(self.norm_embed.bias), self.norm_embed.eps, None)
+        y = ops.run(RowsNormFn, x, _f32(self.norm_embed.weight), _f32(self.norm_embed.bias), self.norm_embed.eps, None)
         return y.view(B, N, D)
 
 
@@ -256,8 +256,8 @@ class MaskFeat(nn.Module):
             wmask = dense.reshape(B, T * H * W).to(device=x.device, dtype=torch.float32).contiguous()
         kreal = conv.weight[0].numel()
         kpad = (kreal + 63) // 64 * 64
-        x0 = mvit_ops.ConvTokensFn.apply(
-            x, _f32(conv.weight), _f32(conv.bias), _f32(self.mask_token), _f32(pos.cls_token), _f32(pos.pos_embed_spatial),
+        x0 = ops.run(
+            mvit_ops.ConvTokensFn, x, _f32(conv.weight), _f32(conv.bias), _f32(self.mask_token), _f32(pos.cls_token), _f32(pos.pos_embed_spatial),
             _f32(pos.pos_embed_temporal), _f32(pos.pos_embed_class), wmask,
             self._shadow.get_padded('conv', conv.weight, kpad), (self.kernel, self.stride, self.padding))
         return self.mvit(x0)

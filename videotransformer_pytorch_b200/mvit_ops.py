@@ -10,6 +10,8 @@ Data layout: the token stream stays fp32 [B, 1+T*H*W, dim] (cls first, tokens t-
 q/k/v projection writes one bf16 [B*N, 3*dim] buffer; pooling and attention read their q/k/v slices of it in place
 through strides, and the backward kernels write the matching slices of the gradient buffer, so the reference's
 reshape/permute/contiguous copies (pytorchvideo _attention_pool) never materialise.
+
+Forward-only calls go through ops.run like the transformer blocks: ctx=None, no statistics, FC1 through 'gelu_h'.
 """
 from __future__ import annotations
 
@@ -17,7 +19,7 @@ import torch
 
 from . import _lib
 from . import ops as _ops
-from .ops import _cast_with_colsum, _dgrad, _wgrad
+from .ops import _cast_with_colsum, _dgrad, _lse, _stats, _wgrad
 
 
 def K():
@@ -51,6 +53,8 @@ class ConvTokensFn(torch.autograd.Function):
         t = k.gemm(cols, conv_wh, M, C0, kpad, bias=conv_b, epi='f32')
         x0 = k.mvit_tokens_fwd(t, wmask, mask_token.reshape(C0), cls_token.reshape(C0), pos_s.reshape(-1, C0),
                                pos_t.reshape(-1, C0), pos_cls.reshape(C0), B, To, Ho * Wo)
+        if ctx is None:
+            return x0
         ctx.save_for_backward(cols, wmask if wmask is not None else torch.empty(0, device=x.device))
         ctx.meta = (tuple(conv_w.shape), tuple(mask_token.shape), tuple(cls_token.shape), tuple(pos_s.shape),
                     tuple(pos_t.shape), tuple(pos_cls.shape), wmask is not None, B, To, Ho * Wo)
@@ -97,25 +101,30 @@ class PoolAttnFn(torch.autograd.Function):
         M = B * N1
         scale = hd ** -0.5
         x2 = x.view(M, d)
-        xn, mean, rstd = k.ln_fwd(x2, n1w, n1b, eps_block)
+        save = ctx is not None
+        st = _stats(save)
+        xn, mean, rstd = k.ln_fwd(x2, n1w, n1b, eps_block, **st)
         qkv = k.gemm(xn, qkv_wh, M, 3 * d, d, bias=torch.cat([qb, kb, vb]), epi='bf16')
         sq, sk, sv = _slots(qkv, B, N1, d)
         if stride_q is not None:
-            q4, q_pooled, q_mean, q_rstd, q_thw = k.pool_fwd(sq, H, hd, thw, stride_q, pq_w.reshape(hd, 27), nq_w, nq_b, eps_pool)
+            q4, q_pooled, q_mean, q_rstd, q_thw = k.pool_fwd(sq, H, hd, thw, stride_q, pq_w.reshape(hd, 27), nq_w, nq_b, eps_pool,
+                                                             **st)
         else:
             q4, q_thw = _bhnd(sq, H, hd), tuple(thw)
             q_pooled = q_mean = q_rstd = torch.empty(0, device=x.device)
-        k4, k_pooled, k_mean, k_rstd, _ = k.pool_fwd(sk, H, hd, thw, stride_kv, pk_w.reshape(hd, 27), nk_w, nk_b, eps_pool)
-        v4, v_pooled, v_mean, v_rstd, _ = k.pool_fwd(sv, H, hd, thw, stride_kv, pv_w.reshape(hd, 27), nv_w, nv_b, eps_pool)
-        o, lse = k.xattn_fwd(q4, k4, v4, scale)
+        k4, k_pooled, k_mean, k_rstd, _ = k.pool_fwd(sk, H, hd, thw, stride_kv, pk_w.reshape(hd, 27), nk_w, nk_b, eps_pool, **st)
+        v4, v_pooled, v_mean, v_rstd, _ = k.pool_fwd(sv, H, hd, thw, stride_kv, pv_w.reshape(hd, 27), nv_w, nv_b, eps_pool, **st)
+        o, lse = k.xattn_fwd(q4, k4, v4, scale, **_lse(save))
         Nq = q4.shape[2]
         Mq = B * Nq
         if stride_q is not None:
             kernel_skip = tuple(s + 1 if s > 1 else s for s in stride_q)
-            x_res, idx, _ = k.maxpool_fwd(x, thw, kernel_skip, stride_q)
+            x_res, idx, _ = k.maxpool_fwd(x, thw, kernel_skip, stride_q, **({} if save else {'want_idx': False}))
         else:
             x_res, idx = x, torch.empty(0, device=x.device)
         y = k.gemm(o.view(Mq, d), proj_wh, Mq, d, d, bias=pb, epi='f32', aux=x_res.view(Mq, d))
+        if not save:
+            return y.view(B, Nq, d)
         ctx.save_for_backward(x, n1w, mean, rstd, xn, qkv, o, lse, idx, q4 if stride_q is not None else torch.empty(0, device=x.device),
                               q_pooled, q_mean, q_rstd, k4, k_pooled, k_mean, k_rstd, v4, v_pooled, v_mean, v_rstd,
                               pq_w if stride_q is not None else torch.empty(0, device=x.device), nq_w if stride_q is not None else torch.empty(0, device=x.device),
@@ -182,12 +191,18 @@ class MlpFn(torch.autograd.Function):
         M = B * N
         Dh, do = w1h.shape[0], w2h.shape[0]
         x2 = x.view(M, d)
-        xn, mean, rstd = k.ln_fwd(x2, n2w, n2b, eps)
-        z = k.gemm(xn, w1h, M, Dh, d, bias=b1, epi='bf16')
-        h = k.gelu(z)
+        save = ctx is not None
+        xn, mean, rstd = k.ln_fwd(x2, n2w, n2b, eps, **_stats(save))
+        if save:
+            z = k.gemm(xn, w1h, M, Dh, d, bias=b1, epi='bf16')
+            h = k.gelu(z)
+        else:
+            z, h = None, k.gemm(xn, w1h, M, Dh, d, bias=b1, epi='gelu_h')
         has_proj = pjh is not None
         r = k.gemm(xn, pjh, M, do, d, bias=pjb, epi='f32') if has_proj else x2
         y = k.gemm(h, w2h, M, do, Dh, bias=b2, epi='f32', aux=r)
+        if not save:
+            return y.view(B, N, do)
         ctx.save_for_backward(x, n2w, mean, rstd, xn, z, h, w1h, w2h, pjh if has_proj else torch.empty(0, device=x.device))
         ctx.has_proj = has_proj
         return y.view(B, N, do)

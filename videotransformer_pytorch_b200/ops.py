@@ -13,6 +13,11 @@ C-ABI kernel launches (see _lib.K):
   ClsNormFn       <- final nn.LayerNorm(eps=1e-6) + cls select     (video_transformer.py:251-254)
   AttentionCoreFn <- Attention.forward (stand-alone use)            (transformer.py:165-177)
 
+Forward-only calls: when autograd will not record a call (grad mode off, or no input or parameter requires grad), `run`
+executes the same forward body with ctx=None instead of Function.apply.  The launch sequence is the same, in the forms
+that write nothing the backward alone reads: FC1 writes h directly (epilogue 'gelu_h' instead of z + a GELU kernel),
+LayerNorm, attention, pooling and max-pool skip their statistics, and nothing is saved.
+
 Data layout: the residual stream stays fp32 `[B, 1+P*T, D]` exactly as in the reference (token
 n = 1 + p*T + t).  The einops regroupings ('b (p t) d -> (b p) t d', '-> (b t) p d', cls replication /
 mean) never materialise: LayerNorm reads rows through an index map and the last GEMM of each
@@ -50,6 +55,16 @@ FUSED_COLSUM = _os.environ.get('VT_FUSED_COLSUM', '1') == '1'
 MERGE_TEMPORAL_FC = _os.environ.get('VT_MERGE_TEMPORAL_FC', '1') == '1'
 
 
+def run(fn, *args):
+    """fn.apply(*args) when autograd records the call; otherwise fn.forward(None, *args), the forward-only form of the
+    same launch sequence (module docstring).  Kernel tables without the forward-only forms (`inference_forms`) always
+    take fn.apply."""
+    if not getattr(K(), 'inference_forms', False) or (
+            torch.is_grad_enabled() and any(isinstance(a, torch.Tensor) and a.requires_grad for a in args)):
+        return fn.apply(*args)
+    return fn.forward(None, *args)
+
+
 def set_mask_arena(arena):
     """Installed by graph.GraphedTrainStep while a step is being captured."""
     global _MASK_ARENA
@@ -61,6 +76,13 @@ def set_mask_arena(arena):
 # --------------------------------------------------------------------------------------------------
 @functools.lru_cache(maxsize=64)
 def token_maps(B: int, T: int, P: int, device: str):
+    # built outside inference mode whatever the caller's mode: the cached maps outlive the call, and a training forward
+    # saves some of them for backward, which autograd refuses for inference tensors
+    with torch.inference_mode(False):
+        return _token_maps(B, T, P, device)
+
+
+def _token_maps(B, T, P, device):
     dev = torch.device(device)
     S = 1 + P * T
     R = B * S
@@ -105,13 +127,15 @@ def affine_row_maps(B: int, T: int, P: int, D: int):
 
 @functools.lru_cache(maxsize=64)
 def frame_maps(BT: int, P: int, device: str):
-    """ViViT spatial encoder tokens: rows (bt, n); patch-embed GEMM rows (bt, p) -> bt*(P+1)+1+p."""
-    dev = torch.device(device)
-    m = torch.arange(BT * P, device=dev, dtype=torch.int64)
-    bt, p = m // P, m % P
-    out = bt * (P + 1) + 1 + p
-    aux = 1 + p
-    return dict(emb_out=out.to(torch.int32).contiguous(), emb_aux=aux.to(torch.int32).contiguous())
+    """ViViT spatial encoder tokens: rows (bt, n); patch-embed GEMM rows (bt, p) -> bt*(P+1)+1+p.
+    Built outside inference mode, like token_maps."""
+    with torch.inference_mode(False):
+        dev = torch.device(device)
+        m = torch.arange(BT * P, device=dev, dtype=torch.int64)
+        bt, p = m // P, m % P
+        out = bt * (P + 1) + 1 + p
+        aux = 1 + p
+        return dict(emb_out=out.to(torch.int32).contiguous(), emb_aux=aux.to(torch.int32).contiguous())
 
 
 def drop_path_scale(p: float, training: bool, n0: int, repeat: int, device):
@@ -200,6 +224,27 @@ def _cast_with_colsum(k, src2d, in_row=None, row_scale=None, rows=None):
     return g, k.colsum(g)
 
 
+def _stats(save):
+    """LayerNorm / pooling keyword for a forward that saves (default form) or one that does not (statistics not written)."""
+    return {} if save else {'stats': False}
+
+
+def _lse(save):
+    return {} if save else {'want_lse': False}
+
+
+def _fc1_gelu(k, xn, w1h, b1, M, Dh, D, save):
+    """(z, h) of h = gelu(z), z = xn W1^T + b1, both bf16.  Saving forward: z is kept for backward — fused 'gelu' epilogue
+    or 'bf16' GEMM + GELU kernel per FUSED_GELU_FWD.  Forward-only: the 'gelu_h' epilogue writes h alone (z is None), bit
+    for bit the split form's h."""
+    if not save:
+        return None, k.gemm(xn, w1h, M, Dh, D, bias=b1, epi='gelu_h')
+    if FUSED_GELU_EPILOGUE or FUSED_GELU_FWD:
+        return k.gemm(xn, w1h, M, Dh, D, bias=b1, epi='gelu')
+    z = k.gemm(xn, w1h, M, Dh, D, bias=b1, epi='bf16')
+    return z, k.gelu(z)
+
+
 def _mul_opt(a, b):
     if a is None:
         return b
@@ -220,14 +265,15 @@ class TemporalAttnFn(torch.autograd.Function):
         maps = token_maps(B, T, P, str(x.device))
         x2 = x.reshape(B * S, D)
         Mt = B * P * T
-        xn, mean, rstd = k.ln_fwd(x2, ln_w, ln_b, eps, in_row=maps['temporal'], rows=Mt)
+        save = ctx is not None
+        xn, mean, rstd = k.ln_fwd(x2, ln_w, ln_b, eps, in_row=maps['temporal'], rows=Mt, **_stats(save))
         qkv = k.gemm(xn, qkv_wh, Mt, 3 * D, D, bias=qkv_b, epi='bf16', tag='qkv')
         hd = D // H
-        cx, lse, _ = k.attn_fwd(qkv, B * P, T, H, hd, hd ** -0.5)
+        cx, lse, _ = k.attn_fwd(qkv, B * P, T, H, hd, hd ** -0.5, **_lse(save))
         y = torch.empty_like(x)
         y2 = y.view(B * S, D)
-        ctx.merged = MERGE_TEMPORAL_FC
-        if ctx.merged:
+        merged = MERGE_TEMPORAL_FC
+        if merged:
             # y = s (W_f (W_p c + b_p)) + b_f + x = s (W_c c + b_c) + b_f + x,  W_c = W_f W_p,  b_c = W_f b_p
             # (transformer.py:261-267: two nn.Linear with only DropPath's per-sample scale between them)
             wc = k.gemm(fc_wh, proj_wh, D, D, D, b_mn=True, epi='bf16')
@@ -240,10 +286,12 @@ class TemporalAttnFn(torch.autograd.Function):
             k.gemm(a, fc_wh, Mt, D, D, bias=fc_b, epi='f32', aux=x2, aux_row=maps['temporal'], out=y2,
                    out_row=maps['temporal'], row_map=affine_row_maps(B, T, P, D)['temporal'])
         k.cls_rows(y[:, 0], x[:, 0])
-        ctx.save_for_backward(x, ln_w, mean, rstd, xn, qkv, cx, lse, a, qkv_wh, proj_wh, fc_wh, dp,
-                              fc_w if ctx.merged else None, proj_b if ctx.merged else None)
-        ctx.geom = (B, S, D, T, H, P)
-        ctx.wptrs = (qkv_w.data_ptr(), proj_w.data_ptr(), fc_w.data_ptr())
+        if save:
+            ctx.merged = merged
+            ctx.save_for_backward(x, ln_w, mean, rstd, xn, qkv, cx, lse, a, qkv_wh, proj_wh, fc_wh, dp,
+                                  fc_w if merged else None, proj_b if merged else None)
+            ctx.geom = (B, S, D, T, H, P)
+            ctx.wptrs = (qkv_w.data_ptr(), proj_w.data_ptr(), fc_w.data_ptr())
         return y
 
     @staticmethod
@@ -309,24 +357,26 @@ class SpatialAttnFn(torch.autograd.Function):
         R, Ms = B * S, B * T * (P + 1)
         x2 = x.reshape(R, D)
         hd = D // H
-        xn, mean, rstd = k.ln_fwd(x2, ln_w, ln_b, eps, in_row=maps['sp_in'], rows=Ms)
+        save = ctx is not None
+        xn, mean, rstd = k.ln_fwd(x2, ln_w, ln_b, eps, in_row=maps['sp_in'], rows=Ms, **_stats(save))
         qkv = k.gemm(xn, qkv_wh, Ms, 3 * D, D, bias=qkv_b, epi='bf16', tag='qkv')
         if P + 1 <= ATTN_SINGLE_PASS_MAX:
-            cx, lse, _ = k.attn_fwd(qkv, B * T, P + 1, H, hd, hd ** -0.5)
+            cx, lse, _ = k.attn_fwd(qkv, B * T, P + 1, H, hd, hd ** -0.5, **_lse(save))
         else:
             # frames of 256 patches or more (inputs larger than 256 x 256 at patch 16): streaming tensor-core kernel,
             # q/k/v read in place from the packed projection
             q4, k4, v4 = _packed_heads(qkv, B * T, P + 1, H, hd)
-            cx, lse = k.xattn_fwd(q4, k4, v4, hd ** -0.5)
+            cx, lse = k.xattn_fwd(q4, k4, v4, hd ** -0.5, **_lse(save))
             cx = cx.view(Ms, D)
         ybig = torch.empty((R + B * T, D), dtype=torch.float32, device=x.device)
         k.gemm(cx, proj_wh, Ms, D, D, bias=proj_b, epi='f32', aux=x2, aux_row=maps['sp_aux'], out=ybig,
                out_row=maps['sp_out'], row_scale=dp, row_map=affine_row_maps(B, T, P, D)['spatial'], tag='proj')
         y = ybig[:R].view(B, S, D)
         k.cls_rows(y[:, 0], x[:, 0], extra=ybig[R:].view(B, T, D), scale=1.0 / T)
-        ctx.save_for_backward(x, ln_w, mean, rstd, xn, qkv, cx, lse, qkv_wh, proj_wh, dp)
-        ctx.geom = (B, S, D, T, H, P)
-        ctx.wptrs = (qkv_w.data_ptr(), proj_w.data_ptr())
+        if save:
+            ctx.save_for_backward(x, ln_w, mean, rstd, xn, qkv, cx, lse, qkv_wh, proj_wh, dp)
+            ctx.geom = (B, S, D, T, H, P)
+            ctx.wptrs = (qkv_w.data_ptr(), proj_w.data_ptr())
         return y
 
     @staticmethod
@@ -368,21 +418,23 @@ class JointAttnFn(torch.autograd.Function):
         M = Bp * N
         x2 = x.reshape(M, D)
         hd = D // H
-        xn, mean, rstd = k.ln_fwd(x2, ln_w, ln_b, eps)
+        save = ctx is not None
+        xn, mean, rstd = k.ln_fwd(x2, ln_w, ln_b, eps, **_stats(save))
         qkv = k.gemm(xn, qkv_wh, M, 3 * D, D, bias=qkv_b, epi='bf16', tag='qkv')
         if N <= ATTN_SINGLE_PASS_MAX:
-            cx, lse, _ = k.attn_fwd(qkv, Bp, N, H, hd, hd ** -0.5)
+            cx, lse, _ = k.attn_fwd(qkv, Bp, N, H, hd, hd ** -0.5, **_lse(save))
         else:
             # long sequences (joint space-time attention: 1 + P*T = 1569 tokens): streaming tensor-core kernel, q/k/v read in
             # place from the packed projection
             q4, k4, v4 = _packed_heads(qkv, Bp, N, H, hd)
-            cx, lse = k.xattn_fwd(q4, k4, v4, hd ** -0.5)
+            cx, lse = k.xattn_fwd(q4, k4, v4, hd ** -0.5, **_lse(save))
             cx = cx.view(M, D)
         y = torch.empty_like(x)
         k.gemm(cx, proj_wh, M, D, D, bias=proj_b, epi='f32', aux=x2, out=y.view(M, D), row_scale=dp, tag='proj')
-        ctx.save_for_backward(x, ln_w, mean, rstd, xn, qkv, cx, lse, qkv_wh, proj_wh, dp)
-        ctx.geom = (Bp, N, D, H)
-        ctx.wptrs = (qkv_w.data_ptr(), proj_w.data_ptr())
+        if save:
+            ctx.save_for_backward(x, ln_w, mean, rstd, xn, qkv, cx, lse, qkv_wh, proj_wh, dp)
+            ctx.geom = (Bp, N, D, H)
+            ctx.wptrs = (qkv_w.data_ptr(), proj_w.data_ptr())
         return y
 
     @staticmethod
@@ -421,16 +473,14 @@ class FFNFn(torch.autograd.Function):
         M = x.numel() // D
         Dh = w1h.shape[0]
         x2 = x.reshape(M, D)
-        xn, mean, rstd = k.ln_fwd(x2, ln_w, ln_b, eps)
-        if FUSED_GELU_EPILOGUE or FUSED_GELU_FWD:
-            z, h = k.gemm(xn, w1h, M, Dh, D, bias=b1, epi='gelu')
-        else:
-            z = k.gemm(xn, w1h, M, Dh, D, bias=b1, epi='bf16')
-            h = k.gelu(z)
+        save = ctx is not None
+        xn, mean, rstd = k.ln_fwd(x2, ln_w, ln_b, eps, **_stats(save))
+        z, h = _fc1_gelu(k, xn, w1h, b1, M, Dh, D, save)
         y = torch.empty_like(x)
         k.gemm(h, w2h, M, D, Dh, bias=b2, epi='f32', aux=x2, out=y.view(M, D), row_scale=dp)
-        ctx.save_for_backward(x, ln_w, mean, rstd, xn, z, h, w1h, w2h, dp)
-        ctx.wptrs = (w1.data_ptr(), w2.data_ptr())
+        if save:
+            ctx.save_for_backward(x, ln_w, mean, rstd, xn, z, h, w1h, w2h, dp)
+            ctx.wptrs = (w1.data_ptr(), w2.data_ptr())
         return y
 
     @staticmethod
@@ -515,10 +565,11 @@ class PatchTokensFn(torch.autograd.Function):
         k.gemm(cols, wh.reshape(D, Kc), M, D, Kc, bias=b, epi='f32', aux=table, aux_row=aux_row,
                out=out.view(-1, D), out_row=out_row)
         out[:, 0] = cls_token.reshape(D).float() + pos[0]
-        ctx.save_for_backward(cols, wh)
-        ctx.meta = (mode, tube, (B, T, C, Himg, Wimg), tuple(w.shape), tuple(cls_token.shape), tuple(pos_embed.shape),
-                    None if time_embed is None else tuple(time_embed.shape), P, Tp,
-                    ctx.needs_input_grad[0] and x.dtype != torch.uint8)
+        if ctx is not None:
+            ctx.save_for_backward(cols, wh)
+            ctx.meta = (mode, tube, (B, T, C, Himg, Wimg), tuple(w.shape), tuple(cls_token.shape), tuple(pos_embed.shape),
+                        None if time_embed is None else tuple(time_embed.shape), P, Tp,
+                        ctx.needs_input_grad[0] and x.dtype != torch.uint8)
         return out
 
     @staticmethod
@@ -597,9 +648,11 @@ class RowsNormFn(torch.autograd.Function):
         D = x.shape[-1]
         x2 = x.reshape(-1, D)
         n = x2.shape[0] if rows is None else rows.numel()
-        y, mean, rstd = k.ln_fwd(x2, w, b, eps, in_row=rows, rows=n, out_fp32=True)
-        ctx.save_for_backward(x, w, mean, rstd, rows if rows is not None else torch.empty(0))
-        ctx.has_rows = rows is not None
+        save = ctx is not None
+        y, mean, rstd = k.ln_fwd(x2, w, b, eps, in_row=rows, rows=n, out_fp32=True, **_stats(save))
+        if save:
+            ctx.save_for_backward(x, w, mean, rstd, rows if rows is not None else torch.empty(0))
+            ctx.has_rows = rows is not None
         return y
 
     @staticmethod
@@ -675,9 +728,10 @@ class LinearSmallFn(torch.autograd.Function):
         k = K()
         x2 = x.reshape(-1, x.shape[-1]).float().contiguous()
         y = k.linear_small_fwd(x2, w.contiguous(), b)
-        ctx.save_for_backward(x2, w)
-        ctx.has_bias = b is not None
-        ctx.xshape = tuple(x.shape)
+        if ctx is not None:
+            ctx.save_for_backward(x2, w)
+            ctx.has_bias = b is not None
+            ctx.xshape = tuple(x.shape)
         return y.view(*x.shape[:-1], w.shape[0])
 
     @staticmethod

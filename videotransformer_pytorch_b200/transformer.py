@@ -31,7 +31,9 @@ def get_sine_cosine_pos_emb(n_position, d_hid):
 
 class ShadowWeights:
     """bf16 shadows of fp32 parameters, refreshed when the parameter is modified (optimizer step,
-    load_state_dict).  Owned by the module (SURVEY.md §8b 'Ownership')."""
+    load_state_dict).  Owned by the module (SURVEY.md §8b 'Ownership').  Shadows are cast outside inference mode even
+    when the forward runs under torch.inference_mode(): a cached shadow is saved for backward by the next training
+    forward, which autograd refuses for inference tensors."""
 
     def __init__(self):
         self._cache = {}
@@ -42,7 +44,7 @@ class ShadowWeights:
         capturing = param.is_cuda and torch.cuda.is_current_stream_capturing()
         if hit is not None and hit[0] == key and not capturing:
             return hit[1]
-        with torch.no_grad():
+        with torch.no_grad(), torch.inference_mode(False):
             w = param.detach()
             if w.dtype != torch.float32:
                 w = w.float()
@@ -60,7 +62,7 @@ class ShadowWeights:
         capturing = params[0].is_cuda and torch.cuda.is_current_stream_capturing()
         if hit is not None and hit[0] == key and not capturing:
             return hit[1]
-        with torch.no_grad():
+        with torch.no_grad(), torch.inference_mode(False):
             w = torch.cat([_f32(p.detach()).reshape(p.shape[0], -1) for p in params], dim=0)
             sh = _lib.K.cast_bf16(w.contiguous())
         self._cache[name] = (key, sh)
@@ -74,7 +76,7 @@ class ShadowWeights:
         capturing = param.is_cuda and torch.cuda.is_current_stream_capturing()
         if hit is not None and hit[0] == key and not capturing:
             return hit[1]
-        with torch.no_grad():
+        with torch.no_grad(), torch.inference_mode(False):
             w = _f32(param.detach()).reshape(param.shape[0], -1)
             w = torch.nn.functional.pad(w, (0, kpad - w.shape[1]))
             sh = _lib.K.cast_bf16(w.contiguous())
@@ -140,7 +142,7 @@ class ClassificationHead(nn.Module):
             constant_init_(module.bias, constant_value=0)
 
     def forward(self, x):
-        return ops.LinearSmallFn.apply(x, _f32(self.cls_head.weight), None if self.cls_head.bias is None else _f32(self.cls_head.bias))
+        return ops.run(ops.LinearSmallFn, x, _f32(self.cls_head.weight), None if self.cls_head.bias is None else _f32(self.cls_head.bias))
 
     def loss(self, x, target):
         """mean cross-entropy of the head's logits: int64 labels (nn.CrossEntropyLoss, model_trainer.py:91, :207-208) or
@@ -187,7 +189,7 @@ class PatchEmbed(nn.Module):
         dev = x.device
         zeros = lambda *s: torch.zeros(*s, device=dev)
         n = (x.shape[-2] // self.patch_size[0]) * (x.shape[-1] // self.patch_size[1])     # patches of this input
-        tok = ops.PatchTokensFn.apply(x, _f32(self.projection.weight), _f32(self.projection.bias), zeros(1, 1, D),
+        tok = ops.run(ops.PatchTokensFn, x, _f32(self.projection.weight), _f32(self.projection.bias), zeros(1, 1, D),
                                       zeros(1, n + 1, D), None, self.shadow(), 'frames', self.tube)
         return tok[:, 1:, :]
 
@@ -270,13 +272,13 @@ class DividedTemporalAttentionWithPreNorm(_DividedBase):
         P = (S - 1) // T
         if return_attention:
             maps = ops.token_maps(B, T, P, str(x.device))
-            xn = ops.RowsNormFn.apply(x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, maps['temporal'])
+            xn = ops.run(ops.RowsNormFn, x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, maps['temporal'])
             return self.attn(xn.view(B * P, T, D))[1]
         dp = _dp_scale(self.layer_drop, B * P, T, x.device)
         qh, ph = self.attn.shadows()
         fh = self.attn._shadow.get('temporal_fc', self.temporal_fc.weight)
-        return ops.TemporalAttnFn.apply(
-            x, _f32(self.norm.weight), _f32(self.norm.bias), _f32(self.attn.qkv.weight), _f32(self.attn.qkv.bias),
+        return ops.run(
+            ops.TemporalAttnFn, x, _f32(self.norm.weight), _f32(self.norm.bias), _f32(self.attn.qkv.weight), _f32(self.attn.qkv.bias),
             _f32(self.attn.proj.weight), _f32(self.attn.proj.bias), _f32(self.temporal_fc.weight),
             _f32(self.temporal_fc.bias), qh, ph, fh, dp, T, self.num_heads, self.norm.eps)
 
@@ -304,12 +306,12 @@ class DividedSpatialAttentionWithPreNorm(_DividedBase):
         P = (S - 1) // T
         if return_attention:
             maps = ops.token_maps(B, T, P, str(x.device))
-            xn = ops.RowsNormFn.apply(x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, maps['sp_in'])
+            xn = ops.run(ops.RowsNormFn, x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, maps['sp_in'])
             return self.attn(xn.view(B * T, P + 1, D))[1]
         dp = _dp_scale(self.layer_drop, B * T, P + 1, x.device)
         qh, ph = self.attn.shadows()
-        return ops.SpatialAttnFn.apply(
-            x, _f32(self.norm.weight), _f32(self.norm.bias), _f32(self.attn.qkv.weight), _f32(self.attn.qkv.bias),
+        return ops.run(
+            ops.SpatialAttnFn, x, _f32(self.norm.weight), _f32(self.norm.bias), _f32(self.attn.qkv.weight), _f32(self.attn.qkv.bias),
             _f32(self.attn.proj.weight), _f32(self.attn.proj.bias), qh, ph, dp, T, self.num_heads, self.norm.eps)
 
 
@@ -335,12 +337,12 @@ class MultiheadAttentionWithPreNorm(nn.Module):
         x = _f32(query).contiguous()
         Bp, N, D = x.shape
         if return_attention:
-            xn = ops.RowsNormFn.apply(x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, None)
+            xn = ops.run(ops.RowsNormFn, x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, None)
             return self.attn(xn.view(Bp, N, D))[1]
         dp = _dp_scale(self.layer_drop, Bp, N, x.device)
         qh, ph = self.attn.shadows()
-        return ops.JointAttnFn.apply(
-            x, _f32(self.norm.weight), _f32(self.norm.bias), _f32(self.attn.qkv.weight), _f32(self.attn.qkv.bias),
+        return ops.run(
+            ops.JointAttnFn, x, _f32(self.norm.weight), _f32(self.norm.bias), _f32(self.attn.qkv.weight), _f32(self.attn.qkv.bias),
             _f32(self.attn.proj.weight), _f32(self.attn.proj.bias), qh, ph, dp, self.num_heads, self.norm.eps)
 
 
@@ -368,7 +370,7 @@ class FFNWithPreNorm(nn.Module):
         fc1, fc2 = self.layers[0][0], self.layers[1]
         n0 = x.shape[0]
         dp = _dp_scale(self.layer_drop, n0, x.numel() // (n0 * x.shape[-1]), x.device)
-        return ops.FFNFn.apply(x, _f32(self.norm.weight), _f32(self.norm.bias), _f32(fc1.weight), _f32(fc1.bias),
+        return ops.run(ops.FFNFn, x, _f32(self.norm.weight), _f32(self.norm.bias), _f32(fc1.weight), _f32(fc1.bias),
                                _f32(fc2.weight), _f32(fc2.bias), self._shadow.get('w1', fc1.weight),
                                self._shadow.get('w2', fc2.weight), dp, self.norm.eps)
 

@@ -173,7 +173,7 @@ class TimeSformer(_ByteClipInput, nn.Module):
         pos = self._interpolate(pos, (h // ps[0]) * (w // ps[1]), w, h)
         pe = self.patch_embed
         mode = 'frames' if self.attention_type == 'space_only' else 'timesformer'   # space_only: per-frame tokens
-        tok = ops.PatchTokensFn.apply(x, _f32(pe.projection.weight), _f32(pe.projection.bias), self.cls_token, pos, tim,
+        tok = ops.run(ops.PatchTokensFn, x, _f32(pe.projection.weight), _f32(pe.projection.bias), self.cls_token, pos, tim,
                                       pe.shadow(), mode, 1, norm, plan)
         return tok, b
 
@@ -186,10 +186,10 @@ class TimeSformer(_ByteClipInput, nn.Module):
         if self.return_cls_token:
             if self.attention_type == 'space_only':
                 rows = (torch.arange(b, device=x.device, dtype=torch.int32) * S).contiguous()
-                return ops.RowsNormFn.apply(x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, rows)
+                return ops.run(ops.RowsNormFn, x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, rows)
             rows = ops.token_maps(b, self.num_frames, (S - 1) // self.num_frames, str(x.device))['cls_rows']
-            return ops.RowsNormFn.apply(x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, rows)
-        y = ops.RowsNormFn.apply(x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, None)
+            return ops.run(ops.RowsNormFn, x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, rows)
+        y = ops.run(ops.RowsNormFn, x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, None)
         return y.view(b, S, -1)[:, 1:].mean(1)
 
     def get_last_selfattention(self, x):
@@ -288,13 +288,13 @@ class ViViT(_ByteClipInput, nn.Module):
         pos = self.pos_embed if self.use_learnable_pos_emb else self.pos_embed.to(x.device).detach()
         pe = self.patch_embed
         if self.attention_type == 'fact_encoder':
-            tok = ops.PatchTokensFn.apply(x, _f32(pe.projection.weight), _f32(pe.projection.bias), self.cls_token, pos, None,
+            tok = ops.run(ops.PatchTokensFn, x, _f32(pe.projection.weight), _f32(pe.projection.bias), self.cls_token, pos, None,
                                           pe.shadow(), 'frames', self.tube_size, norm, plan)
         else:
             # reference :476-499 with use_cls_token_temporal False == TimeSformer's assembly on tubelets: one cls,
             # tokens 'b (p t) d', pos_embed per patch + time_embed per tubelet (fused into the patch GEMM epilogue)
             tim = self.time_embed if self.use_learnable_pos_emb else self.time_embed.to(x.device).detach()
-            tok = ops.PatchTokensFn.apply(x, _f32(pe.projection.weight), _f32(pe.projection.bias), self.cls_token, pos, tim,
+            tok = ops.run(ops.PatchTokensFn, x, _f32(pe.projection.weight), _f32(pe.projection.bias), self.cls_token, pos, tim,
                                           pe.shadow(), 'timesformer', self.tube_size, norm, plan)
         cls_tokens = self.cls_token.expand(tok.shape[0], -1, -1)
         return tok, cls_tokens, b
@@ -319,8 +319,8 @@ class ViViT(_ByteClipInput, nn.Module):
         if self.return_cls_token:
             S = x.shape[1]
             rows = (torch.arange(b, device=x.device, dtype=torch.int32) * S).contiguous()
-            return ops.RowsNormFn.apply(x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, rows)
-        y = ops.RowsNormFn.apply(x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, None)
+            return ops.run(ops.RowsNormFn, x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, rows)
+        y = ops.run(ops.RowsNormFn, x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, None)
         return y.view(x.shape)[:, 1:].mean(1)
 
     def get_last_selfattention(self, x):
