@@ -471,6 +471,53 @@ typedef struct {
 int vt_pos_resize_fwd(const vt_pos_resize_params* p, void* stream);
 int vt_pos_resize_bwd(const vt_pos_resize_params* p, void* stream);
 
+/* ---------------------------------------------------------------------------------------------
+ * Clip transforms on decode-resolution uint8 frames (the reference's DataLoader transforms, data_transform.py:495-615 and
+ * data_trainer.py:75-115, as torchvision applies them to a uint8 T C H W clip).  Frames are HWC uint8.
+ *
+ * vt_resized_crop_u8: out [n, T, S, S, 3] uint8.  Output clip k reads the clip of desc[k]: frame t of it starts at byte
+ * src + src_offset + t * H * pitch.  The crop box is resized to RH x RW with torchvision's antialiased filter (PIL's
+ * formulation: bicubic a = -0.5 with support 2 * max(scale, 1), or bilinear with support max(scale, 1); weights computed
+ * in fp32 and normalised by their sum, taps clamped at the crop box), width pass first with an fp32 intermediate, then
+ * clamped and rounded half to even: what torchvision's resized_crop / resize give on uint8.  Only the S x S window at
+ * (oy, ox) of the resized image is computed, mirrored left-right when flip is set.  An axis may need at most
+ * VT_CROP_MAX_TAPS taps (2 * ceil(support) + 1 <= 32: bicubic downscale <= 7.5, bilinear <= 15).  A descriptor that
+ * breaks a bound (taps, source bytes, window) makes its clip all zeros and sets *err (if given) to 1.
+ * Launch: grid (n * T, ceil(S / 8)), 256 threads; S <= 512.
+ *
+ * vt_color_jitter_u8: torchvision ColorJitter on uint8, in place on frames [n, T, S, S, 3], one CTA per frame with the
+ * frame resident in shared memory (S <= 256).  Clip k applies desc[k].op[0 .. n_ops) in order (0 brightness, 1 contrast,
+ * 2 saturation), each _blend(x, y, r) = trunc(clamp(r * x + (1 - r) * y, 0, 255)) with the products and the sum rounded
+ * separately in fp32; y is 0, the per-frame mean of the grayscale image (an exact integer sum, then one fp32 division),
+ * or the grayscale image (0.2989 r + 0.587 g + 0.114 b, truncated).  one_minus[i] = fp32(1.0 - (double)factor[i]).
+ * ------------------------------------------------------------------------------------------- */
+#define VT_CROP_MAX_TAPS 32
+typedef struct {
+  int64_t src_offset;                      /* bytes from vt_resized_crop_params.src to frame 0 of the clip */
+  int32_t H, W, pitch;                     /* source frame size; row pitch in bytes (>= 3 W), frames H * pitch apart */
+  int32_t crop_y, crop_x, crop_h, crop_w;  /* crop box inside the source frame */
+  int32_t RH, RW;                          /* size the crop box is resized to */
+  int32_t oy, ox;                          /* top-left of the S x S output window inside the RH x RW image */
+  int32_t flip;                            /* 1: mirror the window left-right */
+  int32_t filter;                          /* 0 bicubic, 1 bilinear */
+  int32_t reserved;
+} vt_crop_desc;
+typedef struct {
+  const uint8_t* src; int64_t src_bytes;   /* every byte a descriptor reads lies in [src, src + src_bytes) */
+  const vt_crop_desc* desc;                /* device table, one per output clip */
+  uint8_t* out;
+  int32_t* err;                            /* optional device flag */
+  int32_t n, T, S;
+} vt_resized_crop_params;
+int vt_resized_crop_u8(const vt_resized_crop_params* p, void* stream);
+
+typedef struct {
+  int32_t n_ops, op[3];
+  float factor[3], one_minus[3];
+} vt_jitter_desc;
+typedef struct { uint8_t* frames; const vt_jitter_desc* desc; int32_t n, T, S; } vt_color_jitter_params;
+int vt_color_jitter_u8(const vt_color_jitter_params* p, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -225,6 +225,24 @@ class PosResizeParams(C.Structure):
                 ('scale_h', C.c_double), ('scale_w', C.c_double)]
 
 
+class CropDesc(C.Structure):
+    _fields_ = [('src_offset', c_i64)] + [(n, c_i32) for n in (
+        'H', 'W', 'pitch', 'crop_y', 'crop_x', 'crop_h', 'crop_w', 'RH', 'RW', 'oy', 'ox', 'flip', 'filter', 'reserved')]
+
+
+class JitterDesc(C.Structure):
+    _fields_ = [('n_ops', c_i32), ('op', c_i32 * 3), ('factor', c_f32 * 3), ('one_minus', c_f32 * 3)]
+
+
+class ResizedCropParams(C.Structure):
+    _fields_ = [('src', c_vp), ('src_bytes', c_i64), ('desc', c_vp), ('out', c_vp), ('err', c_vp),
+                ('n', c_i32), ('T', c_i32), ('S', c_i32)]
+
+
+class ColorJitterParams(C.Structure):
+    _fields_ = [('frames', c_vp), ('desc', c_vp), ('n', c_i32), ('T', c_i32), ('S', c_i32)]
+
+
 EXPORTS = ['vt_version', 'vt_last_error', 'vt_sm_count', 'vt_set_reserved_sms', 'vt_launch_count', 'vt_gemm', 'vt_layernorm_fwd', 'vt_ln_bwd_blocks',
            'vt_layernorm_bwd', 'vt_reduce_rows', 'vt_colsum_chunks', 'vt_colsum_bf16', 'vt_cast_f32_bf16',
            'vt_cls_rows', 'vt_gather_cast_colsum_blocks', 'vt_gather_cast_colsum_bf16', 'vt_gelu_bwd_colsum_blocks', 'vt_gelu_bwd_colsum_bf16',
@@ -233,7 +251,8 @@ EXPORTS = ['vt_version', 'vt_last_error', 'vt_sm_count', 'vt_set_reserved_sms', 
            'vt_maxpool_bwd', 'vt_im2col3d_bf16', 'vt_mvit_tokens_fwd', 'vt_mvit_tokens_bwd', 'vt_mse_blocks',
            'vt_mse_fwd', 'vt_mse_bwd', 'vt_opt_norm2', 'vt_opt_sgd', 'vt_opt_adamw',
            'vt_linear_small_fwd', 'vt_linear_small_bwd', 'vt_softmax_ce', 'vt_scale_by_scalar', 'vt_attn_probs',
-           'vt_im2col_u8_mix_bf16', 'vt_pos_resize_fwd', 'vt_pos_resize_bwd', 'vt_topk_hits']
+           'vt_im2col_u8_mix_bf16', 'vt_pos_resize_fwd', 'vt_pos_resize_bwd', 'vt_topk_hits',
+           'vt_resized_crop_u8', 'vt_color_jitter_u8']
 
 _dll = None
 
@@ -783,6 +802,41 @@ class CudaKernels:
         """Adjoint of pos_resize_fwd: dout fp32 [oh*ow, D] -> fp32 [gh*gw, D] (or written into `out`)."""
         return self._pos_resize('vt_pos_resize_bwd', dout, out, out_grid[0] * out_grid[1], grid[0] * grid[1],
                                 grid, out_grid, scales)
+
+    # -- clip transforms (vt_augment.cu) ---------------------------------------------------------
+    def resized_crop_u8(self, src, desc, out, err=None):
+        """src: flat uint8 device buffer of decode-resolution clips; desc: uint8 device bytes holding out.shape[0]
+        CropDesc; out: uint8 [n, T, S, S, 3], written; err: optional int32 [1] set to 1 by a descriptor out of bounds."""
+        lib = load_library()
+        _req(src, torch.uint8, 'resized_crop.src')
+        _req(out, torch.uint8, 'resized_crop.out')
+        if not src.is_contiguous() or not out.is_contiguous() or out.dim() != 5 or out.shape[2] != out.shape[3] or out.shape[4] != 3:
+            raise RuntimeError('resized_crop_u8: src must be contiguous and out a contiguous [n, T, S, S, 3] tensor')
+        n, T, S = out.shape[:3]
+        if desc.numel() < n * C.sizeof(CropDesc):
+            raise RuntimeError(f'resized_crop_u8: desc holds fewer than {n} descriptors')
+        p = ResizedCropParams()
+        p.src, p.src_bytes = src.data_ptr(), src.numel()
+        p.desc = _req(desc, torch.uint8, 'resized_crop.desc').data_ptr()
+        p.out, p.err = out.data_ptr(), _ptr(None if err is None else _req(err, torch.int32, 'resized_crop.err'))
+        p.n, p.T, p.S = n, T, S
+        _check(lib.vt_resized_crop_u8(C.byref(p), _stream()), 'vt_resized_crop_u8')
+        return out
+
+    def color_jitter_u8(self, frames, desc):
+        """ColorJitter in place on uint8 [n, T, S, S, 3] with one JitterDesc per clip (uint8 device bytes)."""
+        lib = load_library()
+        _req(frames, torch.uint8, 'color_jitter.frames')
+        if not frames.is_contiguous() or frames.dim() != 5 or frames.shape[2] != frames.shape[3] or frames.shape[4] != 3:
+            raise RuntimeError('color_jitter_u8: frames must be a contiguous [n, T, S, S, 3] tensor')
+        n, T, S = frames.shape[:3]
+        if desc.numel() < n * C.sizeof(JitterDesc):
+            raise RuntimeError(f'color_jitter_u8: desc holds fewer than {n} descriptors')
+        p = ColorJitterParams()
+        p.frames, p.desc = frames.data_ptr(), _req(desc, torch.uint8, 'color_jitter.desc').data_ptr()
+        p.n, p.T, p.S = n, T, S
+        _check(lib.vt_color_jitter_u8(C.byref(p), _stream()), 'vt_color_jitter_u8')
+        return frames
 
     # -- HOG ------------------------------------------------------------------------------------
     def hog(self, frames, lut, want_bins=False):
