@@ -30,7 +30,7 @@ def rn(shape, seed, scale=1.0, dtype=torch.float32):
 
 
 # ---- LayerNorm, narrow rows ---------------------------------------------------------------------------
-@pytest.mark.parametrize('D', [96, 192, 32, 256])
+@pytest.mark.parametrize('D', [96, 192, 32, 256, 64, 160, 224])
 @pytest.mark.parametrize('rows', [1, 77, 4099])
 def test_layernorm_small(D, rows):
     x, g, b = rn((rows, D), 1), 1 + rn((D,), 2, 0.1), rn((D,), 3, 0.1)

@@ -1257,6 +1257,12 @@ extern "C" int vt_pool_bwd(const vt_pool_bwd_params* p, void* stream) {
   const long long Lo = (long long)p->To * p->Ho * p->Wo;
   const long long rows_out = (long long)p->B * p->H * (1 + Lo);
   VT_REQUIRE(rows_out < 0x7fffffffll, "vt_pool_bwd: too many rows");
+  // the d(input) kernels tabulate each axis in shared memory; checked before the first launch, so a refused call leaves
+  // every output untouched
+  VT_REQUIRE(p->T <= POOL_MAX_DIM && p->Hin <= POOL_MAX_DIM && p->Win <= POOL_MAX_DIM, "vt_pool_bwd: token grid %dx%dx%d exceeds %d per axis",
+             p->T, p->Hin, p->Win, POOL_MAX_DIM);
+  const long long tokens_in = (long long)p->B * (1 + (long long)p->T * p->Hin * p->Win);
+  VT_REQUIRE(tokens_in < 0x7fffffffll, "vt_pool_bwd: too many tokens");
   const int need = vt_pool_bwd_scratch((int)rows_out, p->hd);
   VT_REQUIRE(need > 0 && p->scratch_floats >= need, "vt_pool_bwd: scratch too small (%lld < %d floats)", (long long)p->scratch_floats, need);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1286,10 +1292,6 @@ extern "C" int vt_pool_bwd(const vt_pool_bwd_params* p, void* stream) {
     }
   }
   // 2. gradient w.r.t. the input tokens
-  VT_REQUIRE(p->T <= POOL_MAX_DIM && p->Hin <= POOL_MAX_DIM && p->Win <= POOL_MAX_DIM, "vt_pool_bwd: token grid %dx%dx%d exceeds %d per axis",
-             p->T, p->Hin, p->Win, POOL_MAX_DIM);
-  const long long tokens_in = (long long)p->B * (1 + (long long)p->T * p->Hin * p->Win);
-  VT_REQUIRE(tokens_in < 0x7fffffffll, "vt_pool_bwd: too many tokens");
   const bool v2 = pool_v2(p->in, p->in_bs, p->in_rs) && pool_v2(p->din, p->din_bs, p->din_rs);
   if (v2) {
     const int hw = p->Hin * p->Win;
