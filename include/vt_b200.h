@@ -204,7 +204,8 @@ int vt_gelu_bwd_colsum_bf16(const vt_gelu_bwd_colsum_params* p, void* stream);
  *   lse fp32 [Bp, H, N]   (saved for backward; NULL = not written, for every implementation);
  *   probs fp32 [Bp,H,N,N] optional (Attention returns it, :177)
  * Three kernels behind one entry point: a tensor-core flash kernel for the spatial pass (N = 197; mma.sync bf16 with
- * fp32 accumulators, K/V tiles in shared memory, vt_attention_mma.cu), a warp-per-problem kernel for the temporal pass
+ * fp32 accumulators, K/V tiles double-buffered in shared memory by cp.async, vt_attention_mma.cu), a warp-per-problem
+ * kernel for the temporal pass
  * (N = 8, 18 816 problems/layer), and a generic warp-per-query kernel for any other N <= 256 (ViViT N = 9, probs output).
  * VT_ATTN_TCGEN05 selects the tensor-core kernel (the name is kept for ABI compatibility).
  * ------------------------------------------------------------------------------------------- */
