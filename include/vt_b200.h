@@ -107,6 +107,27 @@ typedef struct {
 int vt_gemm(const vt_gemm_params* p, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * FP8 forward GEMM (inference forms of the block linears):  acc[M,N] = sum_k A[m,k] * B[n,k] with e4m3 operands, then
+ *   acc <- acc * (a_scale[m] * b_scale[n])   (per-token scale of A, per-output-channel scale of B)
+ * followed by the per-element code of VT_EPI_BF16 / VT_EPI_F32 / VT_EPI_GELU_H exactly as vt_gemm applies it (bias,
+ * bias2, row_scale, row maps, affine map, staged or register epilogue).  g.a / g.b point to e4m3 bytes (raw
+ * __nv_fp8_e4m3), lda / ldb in elements; both operands K-major (a_mn_major = b_mn_major = 0).  Each 128-wide k-block
+ * is accumulated by 4 x wgmma k32 into a fresh fp32 register tile and then added on the CUDA cores to the tile's fp32
+ * accumulator.  K % 16 == 0, lda % 16 == 0, ldb % 16 == 0, 16-byte aligned bases.  No split-K: workspace is ignored.
+ * VT_EPI_GELU / VT_EPI_DGELU are rejected.  sm_90 only.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct { vt_gemm_params g; const float* a_scale; const float* b_scale; } vt_gemm_e4m3_params;
+int vt_gemm_e4m3(const vt_gemm_e4m3_params* p, void* stream);
+
+/* Row quantiser of the fp8 forms: x bf16 (x_fp32 = 0) or fp32 [M, K] (leading dim ldx) -> q e4m3 [M, K] (leading dim
+ * ldq) and scale fp32 [M], one warp per row:
+ *   amax = max_k |x[m,k]|;  scale[m] = 2^ceil(log2(amax / 448)) clamped to [2^-126, 2^127], 1 for an all-zero row;
+ *   q[m,k] = e4m3_rn_satfinite(x[m,k] / scale[m])   (x / scale is exact: the cast is the only rounding).
+ * Serves activations (per token) and weights (per output channel).  K % 16 == 0; x and q rows 16-byte aligned. */
+typedef struct { const void* x; int32_t x_fp32; int64_t ldx; void* q; int64_t ldq; float* scale; int32_t M, K; } vt_quant_rows_params;
+int vt_quant_rows_e4m3(const vt_quant_rows_params* p, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * LayerNorm over the last dim (biased variance), fp32 statistics, one warp per row.
  * Replaces nn.LayerNorm at transformer.py:257 / :359 / :439 / :519 and video_transformer.py:251,
  * fused with the einops regroupings around it (transformer.py:250, :352-356): row m of the output

@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
-from typing import Optional
+from typing import NamedTuple, Optional
 
 import torch
 
@@ -32,6 +32,35 @@ class GemmParams(C.Structure):
                 ('map_period', c_i32), ('map_skip', c_i32), ('map_tcount', c_i32), ('force_tail', c_i32),
                 ('map_stride_t', c_i64), ('map_stride_p', c_i64), ('map_stride_b', c_i64), ('map_base', c_i64),
                 ('map_special_base', c_i64), ('map_special_stride', c_i64), ('bias2', c_vp), ('out_zeroed', c_i32)]
+
+
+class GemmE4m3Params(C.Structure):
+    _fields_ = [('g', GemmParams), ('a_scale', c_vp), ('b_scale', c_vp)]
+
+
+class QuantRowsParams(C.Structure):
+    _fields_ = [('x', c_vp), ('x_fp32', c_i32), ('ldx', c_i64), ('q', c_vp), ('ldq', c_i64), ('scale', c_vp),
+                ('M', c_i32), ('K', c_i32)]
+
+
+class E4M3(NamedTuple):
+    """An e4m3 GEMM operand: q float8_e4m3fn [rows, K] and its fp32 per-row scale [rows] (row r stands for
+    q[r].float() * scale[r]).  Weights carry one scale per output channel, activations one per token."""
+    q: torch.Tensor
+    scale: torch.Tensor
+
+    @property
+    def shape(self):
+        return self.q.shape
+
+
+def check_fp8_device(device) -> None:
+    """The e4m3 GEMM forms use sm_90 wgmma: any other CUDA device is refused."""
+    device = torch.device(device)
+    if device.type == 'cuda':
+        cap = torch.cuda.get_device_capability(device)
+        if cap[0] != 9:
+            raise RuntimeError(f'fp8 inference needs an sm_90 (Hopper) device; {device} is sm_{cap[0]}{cap[1]}')
 
 
 class LnFwdParams(C.Structure):
@@ -252,7 +281,7 @@ EXPORTS = ['vt_version', 'vt_last_error', 'vt_sm_count', 'vt_set_reserved_sms', 
            'vt_mse_fwd', 'vt_mse_bwd', 'vt_opt_norm2', 'vt_opt_sgd', 'vt_opt_adamw',
            'vt_linear_small_fwd', 'vt_linear_small_bwd', 'vt_softmax_ce', 'vt_scale_by_scalar', 'vt_attn_probs',
            'vt_im2col_u8_mix_bf16', 'vt_pos_resize_fwd', 'vt_pos_resize_bwd', 'vt_topk_hits',
-           'vt_resized_crop_u8', 'vt_color_jitter_u8']
+           'vt_resized_crop_u8', 'vt_color_jitter_u8', 'vt_gemm_e4m3', 'vt_quant_rows_e4m3']
 
 _dll = None
 
@@ -310,6 +339,8 @@ class CudaKernels:
     # the forward-only forms ops.run dispatches to: the 'gelu_h' GEMM epilogue and stats=False / want_lse=False /
     # want_idx=False (backward-only outputs not written)
     inference_forms = True
+    # the e4m3 GEMM and row quantiser of the fp8 inference forms (set_inference_precision('fp8'))
+    fp8_forms = True
 
     def __init__(self):
         self._ws = {}
@@ -331,9 +362,58 @@ class CudaKernels:
         """row_map: affine description of out_row / aux_row (ops.affine_row_maps) for the fp32 residual epilogue — lets the
         kernel move 32 x 32 boxes by TMA through a tensor map of the token stream instead of per-thread rows.  tag: role label of the launch
         ('qkv', 'proj', ...) for profilers that wrap this method (bench.py); ignored here."""
+        p, out, out2 = self._gemm_params(a, b, M, N, Kdim, torch.bfloat16, a_mn=a_mn, b_mn=b_mn, epi=epi, bias=bias, bias2=bias2,
+                                         out=out, out2=out2, aux=aux, out_row=out_row, aux_row=aux_row, row_scale=row_scale,
+                                         out_rows=out_rows, split_ok=split_ok, force_splits=force_splits, force_bn=force_bn,
+                                         force_cluster=force_cluster, debug=debug, row_map=row_map, force_tail=force_tail,
+                                         out_zeroed=out_zeroed)
+        _check(load_library().vt_gemm(C.byref(p), _stream()), 'vt_gemm')
+        return (out, out2) if epi == 'gelu' else out
+
+    def gemm_e4m3(self, a, b, M, N, Kdim, *, epi='bf16', bias=None, bias2=None, out=None, aux=None, out_row=None,
+                  aux_row=None, row_scale=None, out_rows=None, force_bn=0, row_map=None, tag=None):
+        """The fp8 forward form of gemm(): a, b are E4M3 operands ([M, K] and [N, K], K-major) and the product is
+        dequantised by a.scale[m] * b.scale[n] before the epilogue.  Epilogues 'bf16', 'f32' and 'gelu_h' only; the rest of
+        the arguments are gemm()'s."""
+        if not isinstance(a, E4M3) or not isinstance(b, E4M3):
+            raise RuntimeError('gemm_e4m3: both operands must be E4M3 (quantised rows + scales)')
+        if epi not in ('bf16', 'f32', 'gelu_h'):
+            raise RuntimeError(f'gemm_e4m3: epilogue {epi!r} has no fp8 form')
+        check_fp8_device(a.q.device)
+        for nm, op, rows in (('a', a, M), ('b', b, N)):
+            _req(op.scale, torch.float32, f'gemm_e4m3.{nm}.scale')
+            if op.scale.numel() != rows or not op.scale.is_contiguous():
+                raise RuntimeError(f'gemm_e4m3.{nm}.scale: expected {rows} contiguous entries, got {op.scale.numel()}')
+        p, out, _ = self._gemm_params(a.q, b.q, M, N, Kdim, torch.float8_e4m3fn, epi=epi, bias=bias, bias2=bias2, out=out,
+                                      aux=aux, out_row=out_row, aux_row=aux_row, row_scale=row_scale, out_rows=out_rows,
+                                      force_bn=force_bn, row_map=row_map)
+        q = GemmE4m3Params()
+        q.g, q.a_scale, q.b_scale = p, a.scale.data_ptr(), b.scale.data_ptr()
+        _check(load_library().vt_gemm_e4m3(C.byref(q), _stream()), 'vt_gemm_e4m3')
+        return out
+
+    def quant_rows_e4m3(self, x):
+        """bf16 or fp32 rows [M, K] -> E4M3 (q [M, K], power-of-two scale [M]); vt_quant_rows_e4m3."""
         lib = load_library()
-        _rows2d(_req(a, torch.bfloat16, 'gemm.a'), 'gemm.a')
-        _rows2d(_req(b, torch.bfloat16, 'gemm.b'), 'gemm.b')
+        if x.dtype not in (torch.bfloat16, torch.float32):
+            raise RuntimeError(f'quant_rows_e4m3: expected bf16 or fp32 rows, got {x.dtype}')
+        _rows2d(_req(x, x.dtype, 'quant_rows_e4m3.x'), 'quant_rows_e4m3.x')
+        check_fp8_device(x.device)
+        M, Kd = x.shape
+        q = torch.empty((M, Kd), dtype=torch.float8_e4m3fn, device=x.device)
+        scale = torch.empty(M, dtype=torch.float32, device=x.device)
+        p = QuantRowsParams()
+        p.x, p.x_fp32, p.ldx = x.data_ptr(), int(x.dtype == torch.float32), x.stride(0)
+        p.q, p.ldq, p.scale, p.M, p.K = q.data_ptr(), q.stride(0), scale.data_ptr(), M, Kd
+        _check(lib.vt_quant_rows_e4m3(C.byref(p), _stream()), 'vt_quant_rows_e4m3')
+        return E4M3(q, scale)
+
+    def _gemm_params(self, a, b, M, N, Kdim, op_dtype, *, a_mn=False, b_mn=False, epi='bf16', bias=None, bias2=None, out=None,
+                     out2=None, aux=None, out_row=None, aux_row=None, row_scale=None, out_rows=None, split_ok=False,
+                     force_splits=0, force_bn=0, force_cluster=0, debug=None, row_map=None, force_tail=0, out_zeroed=False):
+        """vt_gemm_params of one call (operands of dtype op_dtype), with the output allocated when not given."""
+        _rows2d(_req(a, op_dtype, 'gemm.a'), 'gemm.a')
+        _rows2d(_req(b, op_dtype, 'gemm.b'), 'gemm.b')
         exp_a = (Kdim, M) if a_mn else (M, Kdim)
         exp_b = (Kdim, N) if b_mn else (N, Kdim)
         if tuple(a.shape) != exp_a or tuple(b.shape) != exp_b:
@@ -386,8 +466,7 @@ class CudaKernels:
             p.map_stride_t, p.map_stride_p, p.map_stride_b = row_map['stride_t'], row_map['stride_p'], row_map['stride_b']
             p.map_base = row_map['base']
             p.map_special_base, p.map_special_stride = row_map.get('special_base', -1), row_map.get('special_stride', 0)
-        _check(lib.vt_gemm(C.byref(p), _stream()), 'vt_gemm')
-        return (out, out2) if epi == 'gelu' else out
+        return p, out, out2
 
     # -- LayerNorm ----------------------------------------------------------------------------
     def ln_fwd(self, x2d, gamma, beta, eps, in_row=None, rows=None, out_fp32=False, stats=True):

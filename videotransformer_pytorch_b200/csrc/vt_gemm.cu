@@ -8,6 +8,8 @@
 // producer runs ahead across tile boundaries, so the next tile's first k-blocks load while the consumers run the epilogue.
 // Both operands may be K-major or MN-major (wgmma transpose bits), so forward (X W^T), dgrad (dY W) and wgrad (dY^T X) all
 // run without transposed copies.
+// The same body also runs the fp8 inference form (gemm_e4m3_kernel, vt_gemm_e4m3): e4m3 K-major operands, BN = 128,
+// per-k-block promotion into the fp32 accumulator and a per-row x per-column dequantisation scale before the epilogue.
 #include <stdlib.h>
 #include <string.h>
 
@@ -41,6 +43,8 @@ struct GemmDev {
   long long map_stride_t, map_stride_p, map_stride_b, map_base;
   float* special_out;      // special rows go to special_out + outer * special_ld, or are dropped
   long long special_ld;
+  const float* a_scale;    // e4m3 forms only: per-row scale of A [M] and per-column scale of B [N]
+  const float* b_scale;
 };
 
 // Epilogue kinds (kernel template parameter SE): 0 = from registers; 1 = one staged bf16 output (VT_EPI_BF16, VT_EPI_GELU_H);
@@ -227,12 +231,18 @@ __device__ __forceinline__ Tile tile_at(const GemmDev& p, int t) {
 // boxes are rewritten, that thread waits until the previous store has read them.  For DGELU the producer TMA-loads the
 // tile's z (tmD) into the second staging tile after issuing the tile's last k-block, guarded by a z full / z empty
 // mbarrier pair.
-template <int BN, int TA, int TB, int SE>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmD, const GemmDev p) {
+// F8 = 1: e4m3 operands (vt_gemm_e4m3), BN = 128, both K-major.  A k-block is then 128 elements (the same 128 bytes per
+// row) and runs as 4 x wgmma k32 into a fresh register tile `part`, which the consumer adds to `acc` once the k-block's
+// MMAs have retired (promotion every 128 K: FP8 wgmma's internal accumulation is not documented to be full fp32).  Before
+// the epilogue acc is multiplied by a_scale[m] * b_scale[n].
+// The body of both kernels below; the tensor maps are the kernels' __grid_constant__ parameters.
+template <int BN, int TA, int TB, int SE, int F8>
+__device__ __forceinline__ void gemm_wgmma_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
+                                                const CUtensorMap& tmD, const GemmDev& p) {
   using Cfg = GemmCfg<BN, SE>;
+  static_assert(!F8 || (BN == 128 && !TA && !TB && SE < 2), "e4m3 forms: BN = 128, K-major operands, one output");
   constexpr int STAGES = Cfg::STAGES;
+  constexpr int KB_ELEMS = F8 ? 128 : BK;      // elements of one k-block (128 bytes per row either way)
   constexpr int HALF_BYTES = Cfg::EPI_TILE_BYTES / 2;   // one consumer warpgroup's 64 x BN part of a staged tile
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -273,13 +283,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           uint8_t* sB = sA + Cfg::A_BYTES;
           mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
           if (!TA) {
-            tma_load_2d(sA, &tmA, &full_bar[stage], kb * BK, c.m0);
+            tma_load_2d(sA, &tmA, &full_bar[stage], kb * KB_ELEMS, c.m0);
           } else {
 #pragma unroll
             for (int ch = 0; ch < BM / 64; ++ch) tma_load_2d(sA + ch * CHUNK_BYTES, &tmA, &full_bar[stage], c.m0 + ch * 64, kb * BK);
           }
           if (!TB) {
-            tma_load_2d(sB, &tmB, &full_bar[stage], kb * BK, c.n0);
+            tma_load_2d(sB, &tmB, &full_bar[stage], kb * KB_ELEMS, c.n0);
           } else {
 #pragma unroll
             for (int ch = 0; ch < BN / 64; ++ch) tma_load_2d(sB + ch * CHUNK_BYTES, &tmB, &full_bar[stage], c.n0 + ch * 64, kb * BK);
@@ -307,11 +317,44 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   uint8_t* stage = epi_smem + cw * HALF_BYTES;
   uint8_t* stage2 = stage + Cfg::EPI_TILE_BYTES;
   uint32_t it = 0, tj = 0;
+  float part[F8 ? BN / 2 : 1];
+#pragma unroll
+  for (int i = 0; i < (F8 ? BN / 2 : 1); ++i) part[i] = 0.f;
   for (int t = blockIdx.x; t < p.tiles; t += gridDim.x, ++tj) {
     const Tile c = tile_at<BN>(p, t);
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    if constexpr (F8) {
+      for (int kb = c.kb0; kb < c.kb1; ++kb, ++it) {
+        const int stage = (int)(it % STAGES);
+        mbar_wait(&full_bar[stage], (it / STAGES) & 1);
+        const uint32_t a_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES) + cw * 64 * 128;
+        const uint32_t b_addr = smem_u32(smem + stage * Cfg::STAGE_BYTES + Cfg::A_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma_m64n128k32_e4m3(part, sdesc_kmajor(a_addr + k * 32), sdesc_kmajor(b_addr + k * 32), k > 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(&empty_bar[stage]);
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+      }
+      // dequantise: acc * (a_scale[m] * b_scale[n]); rows >= M and columns >= N are never stored
+      const int rr = c.m0 + cw * 64 + warp * 16 + (lane >> 2);
+      const float sa0 = rr < p.M ? p.a_scale[rr] : 0.f, sa1 = rr + 8 < p.M ? p.a_scale[rr + 8] : 0.f;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int n = c.n0 + 8 * j + 2 * (lane & 3);
+        if (n >= p.N) break;
+        const float2 sb = __ldg(reinterpret_cast<const float2*>(p.b_scale + n));
+        acc[4 * j] *= sa0 * sb.x;
+        acc[4 * j + 1] *= sa0 * sb.y;
+        acc[4 * j + 2] *= sa1 * sb.x;
+        acc[4 * j + 3] *= sa1 * sb.y;
+      }
+    } else {
     int prev = -1;
     for (int kb = c.kb0; kb < c.kb1; ++kb, ++it) {
       const int stage = (int)(it % STAGES);
@@ -333,6 +376,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     }
     wgmma_wait<0>();
     if (lane == 0) mbar_arrive(&empty_bar[prev]);   // the producer is already filling the ring for the next tile
+    }
 
     if constexpr (SE > 0) {
       const int row0 = c.m0 + cw * 64;
@@ -372,6 +416,21 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   if (SE > 0 && leader) tma_store_wait_read_all();   // shared memory stays valid until the last store has read it
 }
 
+template <int BN, int TA, int TB, int SE>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                  const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmD, const GemmDev p) {
+  gemm_wgmma_body<BN, TA, TB, SE, 0>(tmA, tmB, tmC, tmD, p);
+}
+
+// vt_gemm_e4m3: 128-wide tiles, K-major e4m3 operands, SE = 0 or 1
+template <int SE>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_e4m3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                 const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmD, const GemmDev p) {
+  gemm_wgmma_body<128, 0, 0, SE, 1>(tmA, tmB, tmC, tmD, p);
+}
+
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
@@ -391,22 +450,30 @@ static EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
-// 2-D bf16 row-major [rows, cols] (leading dim ld), box {64 cols, box_rows}, 128B swizzle, OOB -> 0.
-int make_tmap_bf16_2d(CUtensorMap* map, const void* base, long long rows, long long cols, long long ld, int box_rows) {
+// 2-D row-major [rows, cols] (leading dim ld) of 2-byte (bf16) or 1-byte (e4m3) elements, box {128 bytes of columns,
+// box_rows}, 128B swizzle, OOB -> 0.
+static int make_tmap_2d(CUtensorMap* map, int esize, const void* base, long long rows, long long cols, long long ld,
+                        int box_rows) {
   EncodeTiledFn fn = get_encode_fn();
   VT_REQUIRE(fn != nullptr, "cuTensorMapEncodeTiled entry point unavailable");
   VT_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0, "TMA base pointer must be 16-byte aligned");
-  VT_REQUIRE((ld * 2) % 16 == 0, "TMA leading dimension must be a multiple of 8 elements (got %lld)", ld);
+  VT_REQUIRE((ld * esize) % 16 == 0, "TMA leading dimension must be a multiple of %d elements (got %lld)", 16 / esize, ld);
   cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t gstr[1] = {(cuuint64_t)(ld * 2)};
-  cuuint32_t box[2] = {64u, (cuuint32_t)box_rows};
+  cuuint64_t gstr[1] = {(cuuint64_t)(ld * esize)};
+  cuuint32_t box[2] = {(cuuint32_t)(128 / esize), (cuuint32_t)box_rows};
   cuuint32_t estr[2] = {1u, 1u};
-  CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstr, box, estr,
+  CUresult r = fn(map, esize == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base),
+                  gdim, gstr, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   VT_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed (%d) rows=%lld cols=%lld ld=%lld box_rows=%d", (int)r,
              rows, cols, ld, box_rows);
   return 0;
+}
+
+// 2-D bf16 row-major [rows, cols] (leading dim ld), box {64 cols, box_rows}, 128B swizzle, OOB -> 0.
+int make_tmap_bf16_2d(CUtensorMap* map, const void* base, long long rows, long long cols, long long ld, int box_rows) {
+  return make_tmap_2d(map, 2, base, rows, cols, ld, box_rows);
 }
 
 __global__ void reduce_rows_kernel(const float* __restrict__ in, float* __restrict__ out, long long stride, int S,
@@ -482,18 +549,21 @@ int launch_reduce_rows(const float* in, float* out, long long stride, int S, lon
 }
 
 // tm: A, B, and for the staged epilogue the output and GELU's out2 / DGELU's z
-template <int BN, int TA, int TB, int SE>
+template <int BN, int TA, int TB, int SE, int F8 = 0>
 static int launch_gemm_t(const CUtensorMap (&tm)[4], const GemmDev& d, cudaStream_t st) {
   using Cfg = GemmCfg<BN, SE>;
+  void (*kernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const GemmDev);
+  if constexpr (F8) kernel = gemm_e4m3_kernel<SE>;
+  else kernel = gemm_wgmma_kernel<BN, TA, TB, SE>;
   static bool attr_set = false;  // benign race: idempotent
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, TA, TB, SE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES);
     VT_REQUIRE(e == cudaSuccess, "cudaFuncSetAttribute(smem=%d) failed: %s", Cfg::SMEM_BYTES, cudaGetErrorString(e));
     attr_set = true;
   }
   const int grid = d.tiles < persistent_sm_count() ? d.tiles : persistent_sm_count();
-  gemm_wgmma_kernel<BN, TA, TB, SE><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(tm[0], tm[1], tm[2], tm[3], d);
-  return check_launch("gemm_wgmma_kernel");
+  kernel<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(tm[0], tm[1], tm[2], tm[3], d);
+  return check_launch(F8 ? "gemm_e4m3_kernel" : "gemm_wgmma_kernel");
 }
 
 template <int BN, int SE>
@@ -518,18 +588,23 @@ static int staged_kind(const vt_gemm_params* q) {
   return 2;
 }
 
-template <int BN>
+template <int BN, int F8 = 0>
 static int launch_gemm(const vt_gemm_params* q, GemmDev& d, cudaStream_t st) {
   CUtensorMap tm[4];
   memset(tm, 0, sizeof(tm));
   CUtensorMap &tmA = tm[0], &tmB = tm[1];
   int rc;
-  if (!q->a_mn_major) rc = make_tmap_bf16_2d(&tmA, q->a, q->M, q->K, q->lda, BM);
+  if (F8) {   // K-major e4m3 operands (checked by gemm_dispatch)
+    rc = make_tmap_2d(&tmA, 1, q->a, q->M, q->K, q->lda, BM);
+    if (!rc) rc = make_tmap_2d(&tmB, 1, q->b, q->N, q->K, q->ldb, BN);
+  } else if (!q->a_mn_major) rc = make_tmap_bf16_2d(&tmA, q->a, q->M, q->K, q->lda, BM);
   else rc = make_tmap_bf16_2d(&tmA, q->a, q->K, q->M, q->lda, BK);
   if (rc) return rc;
-  if (!q->b_mn_major) rc = make_tmap_bf16_2d(&tmB, q->b, q->N, q->K, q->ldb, BN);
-  else rc = make_tmap_bf16_2d(&tmB, q->b, q->K, q->N, q->ldb, BK);
-  if (rc) return rc;
+  if (!F8) {
+    if (!q->b_mn_major) rc = make_tmap_bf16_2d(&tmB, q->b, q->N, q->K, q->ldb, BN);
+    else rc = make_tmap_bf16_2d(&tmB, q->b, q->K, q->N, q->ldb, BK);
+    if (rc) return rc;
+  }
   d.num_m = (q->M + BM - 1) / BM;
   d.num_n = (q->N + BN - 1) / BN;
   const long long tiles = (long long)d.num_m * d.num_n * d.splits;
@@ -550,9 +625,13 @@ static int launch_gemm(const vt_gemm_params* q, GemmDev& d, cudaStream_t st) {
     if (!rc && q->epilogue == VT_EPI_DGELU) rc = make_tmap_bf16_2d(&tm[3], q->aux, q->M, q->N, q->ldaux, 64);
     if (rc) return rc;
   }
-  if (se == 1) rc = launch_layout<BN, 1>(q, tm, d, st);
-  else if (se == 2) rc = launch_layout<BN, 2>(q, tm, d, st);
-  else rc = launch_layout<BN, 0>(q, tm, d, st);
+  if constexpr (F8) {
+    rc = se == 1 ? launch_gemm_t<BN, 0, 0, 1, 1>(tm, d, st) : launch_gemm_t<BN, 0, 0, 0, 1>(tm, d, st);
+  } else {
+    if (se == 1) rc = launch_layout<BN, 1>(q, tm, d, st);
+    else if (se == 2) rc = launch_layout<BN, 2>(q, tm, d, st);
+    else rc = launch_layout<BN, 0>(q, tm, d, st);
+  }
   if (rc) return rc;
   if (d.splits > 1) {
     VT_REQUIRE(q->ldo == q->N, "vt_gemm: split-K requires ldo == N");
@@ -585,7 +664,7 @@ static int rows_split_point(const vt_gemm_params* q) {
   return q->M - r;
 }
 
-static int gemm_dispatch(const vt_gemm_params* q, void* stream);
+static int gemm_dispatch(const vt_gemm_params* q, const float* a_scale, const float* b_scale, void* stream);
 
 extern "C" int vt_gemm(const vt_gemm_params* q, void* stream) {
   using namespace vt;
@@ -594,16 +673,37 @@ extern "C" int vt_gemm(const vt_gemm_params* q, void* stream) {
   if (m0 > 0) {
     vt_gemm_params head = *q;
     head.M = m0;
-    const int rc = gemm_dispatch(&head, stream);
+    const int rc = gemm_dispatch(&head, nullptr, nullptr, stream);
     if (rc) return rc;
     return launch_gemm_rows(q, m0, stream);
   }
-  return gemm_dispatch(q, stream);
+  return gemm_dispatch(q, nullptr, nullptr, stream);
 }
 
-static int gemm_dispatch(const vt_gemm_params* q, void* stream) {
+extern "C" int vt_gemm_e4m3(const vt_gemm_e4m3_params* p, void* stream) {
+  using namespace vt;
+  VT_REQUIRE(p != nullptr, "vt_gemm_e4m3: null params");
+  const vt_gemm_params* q = &p->g;
+  VT_REQUIRE(p->a_scale && p->b_scale && (reinterpret_cast<uintptr_t>(p->b_scale) & 15) == 0,
+             "vt_gemm_e4m3: a_scale and b_scale are required (b_scale 16-byte aligned)");
+  VT_REQUIRE(!q->a_mn_major && !q->b_mn_major, "vt_gemm_e4m3: both operands must be K-major");
+  VT_REQUIRE(q->epilogue == VT_EPI_BF16 || q->epilogue == VT_EPI_F32 || q->epilogue == VT_EPI_GELU_H,
+             "vt_gemm_e4m3: epilogue %d not available (bf16, f32 and gelu_h only)", q->epilogue);
+  VT_REQUIRE(q->K > 0 && q->K % 16 == 0 && q->lda % 16 == 0 && q->ldb % 16 == 0,
+             "vt_gemm_e4m3: K, lda and ldb must be multiples of 16 (got K=%d lda=%lld ldb=%lld)", q->K, (long long)q->lda,
+             (long long)q->ldb);
+  VT_REQUIRE(q->force_bn == 0 || q->force_bn == 128, "vt_gemm_e4m3: the e4m3 forms run 128-wide tiles only");
+  int dev = 0, major = 0;
+  VT_REQUIRE(cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) == cudaSuccess &&
+                 major == 9, "vt_gemm_e4m3: needs an sm_90 device (compute capability %d.x found)", major);
+  return gemm_dispatch(q, p->a_scale, p->b_scale, stream);
+}
+
+// a_scale / b_scale non-null: the e4m3 forms (vt_gemm_e4m3, arguments checked there)
+static int gemm_dispatch(const vt_gemm_params* q, const float* a_scale, const float* b_scale, void* stream) {
   using namespace vt;
   VT_REQUIRE(q != nullptr, "vt_gemm: null params");
+  const bool f8 = a_scale != nullptr;
   VT_REQUIRE(q->M > 0 && q->N > 0 && q->K > 0, "vt_gemm: bad shape M=%d N=%d K=%d", q->M, q->N, q->K);
   VT_REQUIRE(q->N % 8 == 0, "vt_gemm: N must be a multiple of 8 (got %d)", q->N);
   VT_REQUIRE(q->a && q->b && q->out, "vt_gemm: null operand");
@@ -628,7 +728,8 @@ static int gemm_dispatch(const vt_gemm_params* q, void* stream) {
   d.out = q->out; d.out2 = q->out2; d.aux = q->aux;
   d.ldo = q->ldo; d.ldo2 = q->ldo2; d.ldaux = q->ldaux;
   d.out_row = q->out_row; d.aux_row = q->aux_row; d.row_scale = q->row_scale;
-  d.kblocks = (q->K + BK - 1) / BK;
+  d.kblocks = f8 ? (q->K + 127) / 128 : (q->K + BK - 1) / BK;
+  d.a_scale = a_scale; d.b_scale = b_scale;
   d.map_period = 0; d.map_skip = 0; d.map_tcount = 1;
   d.map_stride_t = d.map_stride_p = d.map_stride_b = d.map_base = 0;
   d.special_out = nullptr; d.special_ld = 0;
@@ -654,6 +755,10 @@ static int gemm_dispatch(const vt_gemm_params* q, void* stream) {
   // ones with the register epilogue, and the staged GELU / dGELU forms lose ring stages to their two staging tiles at
   // wider tiles.  The one-output staged form may also take the 192-wide tile (4 stages), which the model picks for qkv
   // (81 vs 92 us) and the projection's data gradient (29 vs 33 us).
+  if (f8) {   // two accumulator tiles per thread fit the register budget at BN = 128 only; no split-K
+    d.splits = 1;
+    return launch_gemm<128, 1>(q, d, static_cast<cudaStream_t>(stream));
+  }
   const bool short_k = d.kblocks <= 16;
   const bool one_staged = staged_kind(q) == 1;
   const int sms = persistent_sm_count();

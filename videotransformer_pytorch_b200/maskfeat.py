@@ -20,7 +20,7 @@ import torch.nn as nn
 
 from . import mvit_ops, ops
 from .ops import RowsNormFn
-from .transformer import ShadowWeights, _f32
+from .transformer import InferencePrecision, ShadowWeights, _f32
 
 HEAD_DIM = 96   # the kernels are specialised for MViT-B's head width (patch_embed_dim 96, heads double with dim)
 
@@ -118,6 +118,8 @@ class MultiScaleAttention(nn.Module):
 
 
 class MultiScaleBlock(nn.Module):
+    inference_precision = 'bf16'       # InferencePrecision.set_inference_precision
+
     def __init__(self, dim, dim_out, num_heads, hidden, stride_q, stride_kv, norm_eps=1e-6, qkv_bias=True):
         super().__init__()
         self.dim, self.dim_out = dim, dim_out
@@ -136,9 +138,20 @@ class MultiScaleBlock(nn.Module):
             return tuple(thw)
         return tuple((n + 2 - 3) // s + 1 for n, s in zip(thw, self.stride_q))
 
+    def _shadows(self, fp8):
+        """(qkv, proj, fc1, fc2, width-changing proj or None) weight shadows: bf16, or e4m3 for the fp8 forward-only form."""
+        a, sh, has_proj = self.attn, self._shadow, self.dim != self.dim_out
+        if fp8:
+            e = lambda name, *ps: sh.get_e4m3(name + ':e4m3', ps)
+            return (e('qkv', a.q.weight, a.k.weight, a.v.weight), e('proj', a.proj.weight), e('fc1', self.mlp.fc1.weight),
+                    e('fc2', self.mlp.fc2.weight), e('blkproj', self.proj.weight) if has_proj else None)
+        return (sh.get_cat('qkv', [a.q.weight, a.k.weight, a.v.weight]), sh.get('proj', a.proj.weight),
+                sh.get('fc1', self.mlp.fc1.weight), sh.get('fc2', self.mlp.fc2.weight),
+                sh.get('blkproj', self.proj.weight) if has_proj else None)
+
     def forward(self, x, thw):
-        a, sh = self.attn, self._shadow
-        qkv_wh = sh.get_cat('qkv', [a.q.weight, a.k.weight, a.v.weight])
+        a = self.attn
+        qkv_wh, proj_wh, fc1_wh, fc2_wh, blkproj_wh = self._shadows(ops.fp8_form(self, x))
         f = _f32
         pq = (f(a.pool_q.weight), f(a.norm_q.weight), f(a.norm_q.bias)) if self.stride_q is not None else (None, None, None)
         meta = (a.num_heads, tuple(thw), self.stride_q, self.stride_kv, self.norm1.eps, a.norm_k.eps)
@@ -146,14 +159,13 @@ class MultiScaleBlock(nn.Module):
             mvit_ops.PoolAttnFn, x, f(self.norm1.weight), f(self.norm1.bias), f(a.q.weight), f(a.q.bias), f(a.k.weight), f(a.k.bias),
             f(a.v.weight), f(a.v.bias), f(a.proj.weight), f(a.proj.bias), *pq,
             f(a.pool_k.weight), f(a.norm_k.weight), f(a.norm_k.bias), f(a.pool_v.weight), f(a.norm_v.weight), f(a.norm_v.bias),
-            qkv_wh, sh.get('proj', a.proj.weight), meta)
+            qkv_wh, proj_wh, meta)
         has_proj = self.dim != self.dim_out
         x = ops.run(
             mvit_ops.MlpFn, x, f(self.norm2.weight), f(self.norm2.bias), f(self.mlp.fc1.weight), f(self.mlp.fc1.bias),
             f(self.mlp.fc2.weight), f(self.mlp.fc2.bias),
             f(self.proj.weight) if has_proj else None, f(self.proj.bias) if has_proj else None,
-            sh.get('fc1', self.mlp.fc1.weight), sh.get('fc2', self.mlp.fc2.weight),
-            sh.get('blkproj', self.proj.weight) if has_proj else None, self.norm2.eps)
+            fc1_wh, fc2_wh, blkproj_wh, self.norm2.eps)
         return x, self.out_thw(thw)
 
 
@@ -195,7 +207,7 @@ def create_multiscale_vision_transformers(*, spatial_size, temporal_size, depth=
     return MultiscaleVisionTransformers(pos, blocks, nn.LayerNorm(plan[-1]['dim_out'], eps=1e-6))
 
 
-class MaskFeat(nn.Module):
+class MaskFeat(InferencePrecision, nn.Module):
     """forward(x[B,T,3,H,W], target_x[B,T,h,w,dc], mask[B,t,h,w], cube_marker) -> (pred[B,T,h,w,dc], loss);
     forward_features(x, mask=None) -> [B, 1+t*h*w, embed_dims]."""
 

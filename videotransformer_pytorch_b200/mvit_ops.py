@@ -11,7 +11,8 @@ q/k/v projection writes one bf16 [B*N, 3*dim] buffer; pooling and attention read
 through strides, and the backward kernels write the matching slices of the gradient buffer, so the reference's
 reshape/permute/contiguous copies (pytorchvideo _attention_pool) never materialise.
 
-Forward-only calls go through ops.run like the transformer blocks: ctx=None, no statistics, FC1 through 'gelu_h'.
+Forward-only calls go through ops.run like the transformer blocks: ctx=None, no statistics, FC1 through 'gelu_h', and
+with e4m3 weight shadows (fp8 inference precision) every block linear through ops._gemm.
 """
 from __future__ import annotations
 
@@ -19,7 +20,7 @@ import torch
 
 from . import _lib
 from . import ops as _ops
-from .ops import _cast_with_colsum, _dgrad, _lse, _stats, _wgrad
+from .ops import _act, _cast_with_colsum, _dgrad, _gemm, _lse, _stats, _wgrad
 
 
 def K():
@@ -104,7 +105,7 @@ class PoolAttnFn(torch.autograd.Function):
         save = ctx is not None
         st = _stats(save)
         xn, mean, rstd = k.ln_fwd(x2, n1w, n1b, eps_block, **st)
-        qkv = k.gemm(xn, qkv_wh, M, 3 * d, d, bias=torch.cat([qb, kb, vb]), epi='bf16')
+        qkv = _gemm(k, xn, qkv_wh, M, 3 * d, d, bias=torch.cat([qb, kb, vb]), epi='bf16')
         sq, sk, sv = _slots(qkv, B, N1, d)
         if stride_q is not None:
             q4, q_pooled, q_mean, q_rstd, q_thw = k.pool_fwd(sq, H, hd, thw, stride_q, pq_w.reshape(hd, 27), nq_w, nq_b, eps_pool,
@@ -122,7 +123,7 @@ class PoolAttnFn(torch.autograd.Function):
             x_res, idx, _ = k.maxpool_fwd(x, thw, kernel_skip, stride_q, **({} if save else {'want_idx': False}))
         else:
             x_res, idx = x, torch.empty(0, device=x.device)
-        y = k.gemm(o.view(Mq, d), proj_wh, Mq, d, d, bias=pb, epi='f32', aux=x_res.view(Mq, d))
+        y = _gemm(k, o.view(Mq, d), proj_wh, Mq, d, d, bias=pb, epi='f32', aux=x_res.view(Mq, d))
         if not save:
             return y.view(B, Nq, d)
         ctx.save_for_backward(x, n1w, mean, rstd, xn, qkv, o, lse, idx, q4 if stride_q is not None else torch.empty(0, device=x.device),
@@ -197,10 +198,11 @@ class MlpFn(torch.autograd.Function):
             z = k.gemm(xn, w1h, M, Dh, d, bias=b1, epi='bf16')
             h = k.gelu(z)
         else:
-            z, h = None, k.gemm(xn, w1h, M, Dh, d, bias=b1, epi='gelu_h')
+            xn = _act(k, xn, w1h)          # fp8: quantised once for FC1 and the width-changing proj
+            z, h = None, _gemm(k, xn, w1h, M, Dh, d, bias=b1, epi='gelu_h')
         has_proj = pjh is not None
-        r = k.gemm(xn, pjh, M, do, d, bias=pjb, epi='f32') if has_proj else x2
-        y = k.gemm(h, w2h, M, do, Dh, bias=b2, epi='f32', aux=r)
+        r = _gemm(k, xn, pjh, M, do, d, bias=pjb, epi='f32') if has_proj else x2
+        y = _gemm(k, h, w2h, M, do, Dh, bias=b2, epi='f32', aux=r)
         if not save:
             return y.view(B, N, do)
         ctx.save_for_backward(x, n2w, mean, rstd, xn, z, h, w1h, w2h, pjh if has_proj else torch.empty(0, device=x.device))

@@ -18,6 +18,10 @@ executes the same forward body with ctx=None instead of Function.apply.  The lau
 that write nothing the backward alone reads: FC1 writes h directly (epilogue 'gelu_h' instead of z + a GELU kernel),
 LayerNorm, attention, pooling and max-pool skip their statistics, and nothing is saved.
 
+FP8 inference (set_inference_precision('fp8') on the model, `fp8_form`): in the forward-only form the module hands the
+block e4m3 weight shadows (_lib.E4M3) instead of bf16 ones, and `_gemm` then quantises the activation rows
+(vt_quant_rows_e4m3) and runs the e4m3 GEMM with the same epilogue.  The block bodies are the same for both precisions.
+
 Data layout: the residual stream stays fp32 `[B, 1+P*T, D]` exactly as in the reference (token
 n = 1 + p*T + t).  The einops regroupings ('b (p t) d -> (b p) t d', '-> (b t) p d', cls replication /
 mean) never materialise: LayerNorm reads rows through an index map and the last GEMM of each
@@ -59,10 +63,37 @@ def run(fn, *args):
     """fn.apply(*args) when autograd records the call; otherwise fn.forward(None, *args), the forward-only form of the
     same launch sequence (module docstring).  Kernel tables without the forward-only forms (`inference_forms`) always
     take fn.apply."""
-    if not getattr(K(), 'inference_forms', False) or (
-            torch.is_grad_enabled() and any(isinstance(a, torch.Tensor) and a.requires_grad for a in args)):
+    if not _forward_only(args):
         return fn.apply(*args)
     return fn.forward(None, *args)
+
+
+def _forward_only(tensors):
+    return getattr(K(), 'inference_forms', False) and not (
+        torch.is_grad_enabled() and any(isinstance(a, torch.Tensor) and a.requires_grad for a in tensors))
+
+
+def fp8_form(module, x):
+    """True when run() takes the forward-only form for a call of `module` on x and the module's inference precision is
+    'fp8': the module then hands its block e4m3 weight shadows.  A kernel table without the e4m3 forms raises."""
+    if getattr(module, 'inference_precision', 'bf16') != 'fp8' or not _forward_only([x, *module.parameters()]):
+        return False
+    if not getattr(K(), 'fp8_forms', False):
+        raise RuntimeError(f'kernel table {getattr(K(), "name", type(K()).__name__)!r} has no fp8 forms (no fallback)')
+    return True
+
+
+def _act(k, a, w):
+    """The A operand for weight w: a itself for a bf16 weight shadow, its e4m3 rows (per-token scales) for an e4m3 one."""
+    return k.quant_rows_e4m3(a) if isinstance(w, _lib.E4M3) and not isinstance(a, _lib.E4M3) else a
+
+
+def _gemm(k, a, w, M, N, Kdim, **kw):
+    """a W^T through k.gemm for a bf16 weight shadow, or through k.gemm_e4m3 (a quantised per token unless it already is)
+    for an e4m3 one; same epilogue arguments either way."""
+    if isinstance(w, _lib.E4M3):
+        return k.gemm_e4m3(_act(k, a, w), w, M, N, Kdim, **kw)
+    return k.gemm(a, w, M, N, Kdim, **kw)
 
 
 def set_mask_arena(arena):
@@ -238,7 +269,7 @@ def _fc1_gelu(k, xn, w1h, b1, M, Dh, D, save):
     or 'bf16' GEMM + GELU kernel per FUSED_GELU_FWD.  Forward-only: the 'gelu_h' epilogue writes h alone (z is None), bit
     for bit the split form's h."""
     if not save:
-        return None, k.gemm(xn, w1h, M, Dh, D, bias=b1, epi='gelu_h')
+        return None, _gemm(k, xn, w1h, M, Dh, D, bias=b1, epi='gelu_h')
     if FUSED_GELU_EPILOGUE or FUSED_GELU_FWD:
         return k.gemm(xn, w1h, M, Dh, D, bias=b1, epi='gelu')
     z = k.gemm(xn, w1h, M, Dh, D, bias=b1, epi='bf16')
@@ -267,7 +298,7 @@ class TemporalAttnFn(torch.autograd.Function):
         Mt = B * P * T
         save = ctx is not None
         xn, mean, rstd = k.ln_fwd(x2, ln_w, ln_b, eps, in_row=maps['temporal'], rows=Mt, **_stats(save))
-        qkv = k.gemm(xn, qkv_wh, Mt, 3 * D, D, bias=qkv_b, epi='bf16', tag='qkv')
+        qkv = _gemm(k, xn, qkv_wh, Mt, 3 * D, D, bias=qkv_b, epi='bf16', tag='qkv')
         hd = D // H
         cx, lse, _ = k.attn_fwd(qkv, B * P, T, H, hd, hd ** -0.5, **_lse(save))
         y = torch.empty_like(x)
@@ -276,15 +307,16 @@ class TemporalAttnFn(torch.autograd.Function):
         if merged:
             # y = s (W_f (W_p c + b_p)) + b_f + x = s (W_c c + b_c) + b_f + x,  W_c = W_f W_p,  b_c = W_f b_p
             # (transformer.py:261-267: two nn.Linear with only DropPath's per-sample scale between them)
-            wc = k.gemm(fc_wh, proj_wh, D, D, D, b_mn=True, epi='bf16')
+            # fp8: fc_wh is already the e4m3 product weight (ShadowWeights.get_e4m3 of W_f W_p)
+            wc = fc_wh if isinstance(fc_wh, _lib.E4M3) else k.gemm(fc_wh, proj_wh, D, D, D, b_mn=True, epi='bf16')
             bc = torch.mv(fc_w.detach().float(), proj_b.detach().float())
-            k.gemm(cx, wc, Mt, D, D, bias=bc, bias2=fc_b, epi='f32', aux=x2, aux_row=maps['temporal'], out=y2,
-                   out_row=maps['temporal'], row_scale=dp, row_map=affine_row_maps(B, T, P, D)['temporal'], tag='proj')
+            _gemm(k, cx, wc, Mt, D, D, bias=bc, bias2=fc_b, epi='f32', aux=x2, aux_row=maps['temporal'], out=y2,
+                  out_row=maps['temporal'], row_scale=dp, row_map=affine_row_maps(B, T, P, D)['temporal'], tag='proj')
             a = wc
         else:
-            a = k.gemm(cx, proj_wh, Mt, D, D, bias=proj_b, epi='bf16', row_scale=dp, tag='proj')
-            k.gemm(a, fc_wh, Mt, D, D, bias=fc_b, epi='f32', aux=x2, aux_row=maps['temporal'], out=y2,
-                   out_row=maps['temporal'], row_map=affine_row_maps(B, T, P, D)['temporal'])
+            a = _gemm(k, cx, proj_wh, Mt, D, D, bias=proj_b, epi='bf16', row_scale=dp, tag='proj')
+            _gemm(k, a, fc_wh, Mt, D, D, bias=fc_b, epi='f32', aux=x2, aux_row=maps['temporal'], out=y2,
+                  out_row=maps['temporal'], row_map=affine_row_maps(B, T, P, D)['temporal'])
         k.cls_rows(y[:, 0], x[:, 0])
         if save:
             ctx.merged = merged
@@ -359,7 +391,7 @@ class SpatialAttnFn(torch.autograd.Function):
         hd = D // H
         save = ctx is not None
         xn, mean, rstd = k.ln_fwd(x2, ln_w, ln_b, eps, in_row=maps['sp_in'], rows=Ms, **_stats(save))
-        qkv = k.gemm(xn, qkv_wh, Ms, 3 * D, D, bias=qkv_b, epi='bf16', tag='qkv')
+        qkv = _gemm(k, xn, qkv_wh, Ms, 3 * D, D, bias=qkv_b, epi='bf16', tag='qkv')
         if P + 1 <= ATTN_SINGLE_PASS_MAX:
             cx, lse, _ = k.attn_fwd(qkv, B * T, P + 1, H, hd, hd ** -0.5, **_lse(save))
         else:
@@ -369,8 +401,8 @@ class SpatialAttnFn(torch.autograd.Function):
             cx, lse = k.xattn_fwd(q4, k4, v4, hd ** -0.5, **_lse(save))
             cx = cx.view(Ms, D)
         ybig = torch.empty((R + B * T, D), dtype=torch.float32, device=x.device)
-        k.gemm(cx, proj_wh, Ms, D, D, bias=proj_b, epi='f32', aux=x2, aux_row=maps['sp_aux'], out=ybig,
-               out_row=maps['sp_out'], row_scale=dp, row_map=affine_row_maps(B, T, P, D)['spatial'], tag='proj')
+        _gemm(k, cx, proj_wh, Ms, D, D, bias=proj_b, epi='f32', aux=x2, aux_row=maps['sp_aux'], out=ybig,
+              out_row=maps['sp_out'], row_scale=dp, row_map=affine_row_maps(B, T, P, D)['spatial'], tag='proj')
         y = ybig[:R].view(B, S, D)
         k.cls_rows(y[:, 0], x[:, 0], extra=ybig[R:].view(B, T, D), scale=1.0 / T)
         if save:
@@ -420,7 +452,7 @@ class JointAttnFn(torch.autograd.Function):
         hd = D // H
         save = ctx is not None
         xn, mean, rstd = k.ln_fwd(x2, ln_w, ln_b, eps, **_stats(save))
-        qkv = k.gemm(xn, qkv_wh, M, 3 * D, D, bias=qkv_b, epi='bf16', tag='qkv')
+        qkv = _gemm(k, xn, qkv_wh, M, 3 * D, D, bias=qkv_b, epi='bf16', tag='qkv')
         if N <= ATTN_SINGLE_PASS_MAX:
             cx, lse, _ = k.attn_fwd(qkv, Bp, N, H, hd, hd ** -0.5, **_lse(save))
         else:
@@ -430,7 +462,7 @@ class JointAttnFn(torch.autograd.Function):
             cx, lse = k.xattn_fwd(q4, k4, v4, hd ** -0.5, **_lse(save))
             cx = cx.view(M, D)
         y = torch.empty_like(x)
-        k.gemm(cx, proj_wh, M, D, D, bias=proj_b, epi='f32', aux=x2, out=y.view(M, D), row_scale=dp, tag='proj')
+        _gemm(k, cx, proj_wh, M, D, D, bias=proj_b, epi='f32', aux=x2, out=y.view(M, D), row_scale=dp, tag='proj')
         if save:
             ctx.save_for_backward(x, ln_w, mean, rstd, xn, qkv, cx, lse, qkv_wh, proj_wh, dp)
             ctx.geom = (Bp, N, D, H)
@@ -477,7 +509,7 @@ class FFNFn(torch.autograd.Function):
         xn, mean, rstd = k.ln_fwd(x2, ln_w, ln_b, eps, **_stats(save))
         z, h = _fc1_gelu(k, xn, w1h, b1, M, Dh, D, save)
         y = torch.empty_like(x)
-        k.gemm(h, w2h, M, D, Dh, bias=b2, epi='f32', aux=x2, out=y.view(M, D), row_scale=dp)
+        _gemm(k, h, w2h, M, D, Dh, bias=b2, epi='f32', aux=x2, out=y.view(M, D), row_scale=dp)
         if save:
             ctx.save_for_backward(x, ln_w, mean, rstd, xn, z, h, w1h, w2h, dp)
             ctx.wptrs = (w1.data_ptr(), w2.data_ptr())

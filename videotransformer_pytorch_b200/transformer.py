@@ -84,8 +84,50 @@ class ShadowWeights:
         return sh
 
 
+    def get_e4m3(self, name: str, params, derive=None) -> _lib.E4M3:
+        """e4m3 shadow with one power-of-two scale per output channel (vt_quant_rows_e4m3) of the fp32 weight rows of
+        `params` stacked along dim 0, or of the fp32 matrix derive() returns (a product of weights).  Re-quantised when
+        any of `params` changes and always while a CUDA graph is being captured, like the bf16 shadows."""
+        params = list(params)
+        key = tuple((p._version, p.data_ptr(), p.device) for p in params)
+        hit = self._cache.get(name)
+        capturing = params[0].is_cuda and torch.cuda.is_current_stream_capturing()
+        if hit is not None and hit[0] == key and not capturing:
+            return hit[1]
+        with torch.no_grad(), torch.inference_mode(False):
+            if derive is not None:
+                w = derive()
+            else:
+                w = torch.cat([_f32(p.detach()).reshape(p.shape[0], -1) for p in params], dim=0)
+            sh = _lib.K.quant_rows_e4m3(w.contiguous())
+        self._cache[name] = (key, sh)
+        return sh
+
+
 def _f32(p):
     return p if p.dtype == torch.float32 else p.float()
+
+
+INFERENCE_PRECISIONS = ('bf16', 'fp8')
+
+
+class InferencePrecision:
+    """set_inference_precision of the models (TimeSformer, ViViT, MaskFeat)."""
+
+    def set_inference_precision(self, precision: str):
+        """Operand precision of the block linears in forward-only calls (no_grad, inference_mode, nothing requiring
+        grad, GraphedForward): 'bf16' (default) or 'fp8' (e4m3 operands with per-token and per-output-channel scales,
+        sm_90 only).  Calls that autograd records, the patch embedding, the head, attention, LayerNorm and pooling are
+        not affected."""
+        if precision not in INFERENCE_PRECISIONS:
+            raise ValueError(f'inference precision must be one of {INFERENCE_PRECISIONS}, got {precision!r}')
+        if precision == 'fp8':
+            for dev in {p.device for p in self.parameters()}:
+                _lib.check_fp8_device(dev)
+        for m in self.modules():
+            if hasattr(type(m), 'inference_precision'):
+                m.inference_precision = precision
+        return self
 
 
 class DropPath(nn.Module):
@@ -213,6 +255,9 @@ class Attention(nn.Module):
     def shadows(self):
         return self._shadow.get('qkv', self.qkv.weight), self._shadow.get('proj', self.proj.weight)
 
+    def e4m3_shadows(self):
+        return self._shadow.get_e4m3('qkv:e4m3', [self.qkv.weight]), self._shadow.get_e4m3('proj:e4m3', [self.proj.weight])
+
     def qkv_bias_or_zeros(self):
         if self.qkv.bias is not None:
             return _f32(self.qkv.bias)
@@ -226,6 +271,8 @@ class Attention(nn.Module):
 
 
 class _DividedBase(nn.Module):
+    inference_precision = 'bf16'       # InferencePrecision.set_inference_precision
+
     def __init__(self, embed_dims, num_heads, num_frames, use_cls_token, attn_drop=0., proj_drop=0.,
                  layer_drop=None, norm_layer=nn.LayerNorm, **kwargs):
         super().__init__()
@@ -246,6 +293,17 @@ class _DividedBase(nn.Module):
 class DividedTemporalAttentionWithPreNorm(_DividedBase):
     """Temporal pass of divided space-time attention (attention over the T frames of each patch).
     Hot-path configuration: use_cls_token=False (cls bypasses the block, `temporal_fc` after DropPath)."""
+
+    def _e4m3_shadows(self, D):
+        """(qkv, proj, temporal_fc) e4m3 shadows; with the merged temporal_fc . proj GEMM (ops.MERGE_TEMPORAL_FC) the third
+        is the product W_f W_p, formed from the bf16 shadows in fp32 and quantised per output channel, and proj is unused."""
+        a, sh = self.attn, self.attn._shadow
+        qh = sh.get_e4m3('qkv:e4m3', [a.qkv.weight])
+        if not ops.MERGE_TEMPORAL_FC:
+            return qh, sh.get_e4m3('proj:e4m3', [a.proj.weight]), sh.get_e4m3('temporal_fc:e4m3', [self.temporal_fc.weight])
+        product = lambda: _lib.K.gemm(sh.get('temporal_fc', self.temporal_fc.weight), sh.get('proj', a.proj.weight), D, D, D,
+                                      b_mn=True, epi='f32')
+        return qh, None, sh.get_e4m3('wc:e4m3', [self.temporal_fc.weight, a.proj.weight], derive=product)
 
     def __init__(self, embed_dims, num_heads, num_frames, use_cls_token, attn_drop=0., proj_drop=0.,
                  layer_drop=None, norm_layer=nn.LayerNorm, **kwargs):
@@ -275,8 +333,11 @@ class DividedTemporalAttentionWithPreNorm(_DividedBase):
             xn = ops.run(ops.RowsNormFn, x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, maps['temporal'])
             return self.attn(xn.view(B * P, T, D))[1]
         dp = _dp_scale(self.layer_drop, B * P, T, x.device)
-        qh, ph = self.attn.shadows()
-        fh = self.attn._shadow.get('temporal_fc', self.temporal_fc.weight)
+        if ops.fp8_form(self, x):
+            qh, ph, fh = self._e4m3_shadows(D)
+        else:
+            qh, ph = self.attn.shadows()
+            fh = self.attn._shadow.get('temporal_fc', self.temporal_fc.weight)
         return ops.run(
             ops.TemporalAttnFn, x, _f32(self.norm.weight), _f32(self.norm.bias), _f32(self.attn.qkv.weight), _f32(self.attn.qkv.bias),
             _f32(self.attn.proj.weight), _f32(self.attn.proj.bias), _f32(self.temporal_fc.weight),
@@ -309,7 +370,7 @@ class DividedSpatialAttentionWithPreNorm(_DividedBase):
             xn = ops.run(ops.RowsNormFn, x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, maps['sp_in'])
             return self.attn(xn.view(B * T, P + 1, D))[1]
         dp = _dp_scale(self.layer_drop, B * T, P + 1, x.device)
-        qh, ph = self.attn.shadows()
+        qh, ph = self.attn.e4m3_shadows() if ops.fp8_form(self, x) else self.attn.shadows()
         return ops.run(
             ops.SpatialAttnFn, x, _f32(self.norm.weight), _f32(self.norm.bias), _f32(self.attn.qkv.weight), _f32(self.attn.qkv.bias),
             _f32(self.attn.proj.weight), _f32(self.attn.proj.bias), qh, ph, dp, T, self.num_heads, self.norm.eps)
@@ -317,6 +378,7 @@ class DividedSpatialAttentionWithPreNorm(_DividedBase):
 
 class MultiheadAttentionWithPreNorm(nn.Module):
     """Pre-norm joint self-attention with residual (ViViT encoders)."""
+    inference_precision = 'bf16'
 
     def __init__(self, embed_dims, num_heads, attn_drop=0., proj_drop=0., norm_layer=nn.LayerNorm,
                  layer_drop=None, batch_first=False, **kwargs):
@@ -340,7 +402,7 @@ class MultiheadAttentionWithPreNorm(nn.Module):
             xn = ops.run(ops.RowsNormFn, x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, None)
             return self.attn(xn.view(Bp, N, D))[1]
         dp = _dp_scale(self.layer_drop, Bp, N, x.device)
-        qh, ph = self.attn.shadows()
+        qh, ph = self.attn.e4m3_shadows() if ops.fp8_form(self, x) else self.attn.shadows()
         return ops.run(
             ops.JointAttnFn, x, _f32(self.norm.weight), _f32(self.norm.bias), _f32(self.attn.qkv.weight), _f32(self.attn.qkv.bias),
             _f32(self.attn.proj.weight), _f32(self.attn.proj.bias), qh, ph, dp, self.num_heads, self.norm.eps)
@@ -348,6 +410,7 @@ class MultiheadAttentionWithPreNorm(nn.Module):
 
 class FFNWithPreNorm(nn.Module):
     """Pre-norm 2-layer MLP with exact-erf GELU and residual."""
+    inference_precision = 'bf16'
 
     def __init__(self, embed_dims=256, hidden_channels=1024, num_layers=2, act_layer=nn.GELU,
                  norm_layer=nn.LayerNorm, dropout_p=0., layer_drop=None, **kwargs):
@@ -370,9 +433,12 @@ class FFNWithPreNorm(nn.Module):
         fc1, fc2 = self.layers[0][0], self.layers[1]
         n0 = x.shape[0]
         dp = _dp_scale(self.layer_drop, n0, x.numel() // (n0 * x.shape[-1]), x.device)
+        if ops.fp8_form(self, x):
+            w1h, w2h = self._shadow.get_e4m3('w1:e4m3', [fc1.weight]), self._shadow.get_e4m3('w2:e4m3', [fc2.weight])
+        else:
+            w1h, w2h = self._shadow.get('w1', fc1.weight), self._shadow.get('w2', fc2.weight)
         return ops.run(ops.FFNFn, x, _f32(self.norm.weight), _f32(self.norm.bias), _f32(fc1.weight), _f32(fc1.bias),
-                               _f32(fc2.weight), _f32(fc2.bias), self._shadow.get('w1', fc1.weight),
-                               self._shadow.get('w2', fc2.weight), dp, self.norm.eps)
+                               _f32(fc2.weight), _f32(fc2.bias), w1h, w2h, dp, self.norm.eps)
 
 
 class TransformerContainer(nn.Module):

@@ -17,7 +17,7 @@ import torch.nn as nn
 
 from . import ops
 from .mixup import MixedClip
-from .transformer import PatchEmbed, TransformerContainer, get_sine_cosine_pos_emb, _f32
+from .transformer import InferencePrecision, PatchEmbed, TransformerContainer, get_sine_cosine_pos_emb, _f32
 from .weight_init import init_from_kinetics_pretrain_, init_from_vit_pretrain_, trunc_normal_
 
 
@@ -64,7 +64,7 @@ class _ByteClipInput:
         return x, norm, plan
 
 
-class TimeSformer(_ByteClipInput, nn.Module):
+class TimeSformer(_ByteClipInput, InferencePrecision, nn.Module):
     """TimeSformer (divided space-time attention).  forward(x[B,T,3,H,W]) -> [B, embed_dims]."""
 
     supported_attention_types = ['divided_space_time', 'space_only', 'joint_space_time']
@@ -206,7 +206,7 @@ def get_vit_base_patch16_224(**kwargs):
                        return_cls_token=True)
 
 
-class ViViT(_ByteClipInput, nn.Module):
+class ViViT(_ByteClipInput, InferencePrecision, nn.Module):
     """ViViT factorised encoder (model 2): tubelet embed -> 12 spatial layers per frame ->
     frame tokens (+ the reference's `x[:b,0,:]` cls gather) -> 4 temporal layers."""
 
