@@ -512,6 +512,26 @@ int vt_pos_resize_bwd(const vt_pos_resize_params* p, void* stream);
  * 2 saturation), each _blend(x, y, r) = trunc(clamp(r * x + (1 - r) * y, 0, 255)) with the products and the sum rounded
  * separately in fp32; y is 0, the per-frame mean of the grayscale image (an exact integer sum, then one fp32 division),
  * or the grayscale image (0.2989 r + 0.587 g + 0.114 b, truncated).  one_minus[i] = fp32(1.0 - (double)factor[i]).
+ *
+ * vt_rand_augment_u8: torchvision RandAugment (NEAREST, fill None) on uint8, in place on frames [n, T, S, S, 3], one CTA
+ * per frame with the frame resident in shared memory (S <= 256).  Clip k applies desc[k].op[0 .. n_ops) in order, with
+ * torchvision's op index as the code: 0 Identity, 1 ShearX, 2 ShearY, 3 TranslateX, 4 TranslateY, 5 Rotate,
+ * 6 Brightness, 7 Color, 8 Contrast, 9 Sharpness, 10 Posterize, 11 Solarize, 12 AutoContrast, 13 Equalize.
+ *  - 1-5 sample the frame at nearest-rounded (half to even) source coordinates, zero outside: for the pixel centre
+ *    (x, y) = (col - S/2 + 0.5, row - S/2 + 0.5), g = (x * theta[0] + y * theta[1]) + theta[2] (and theta[3..5] for
+ *    the row), source = ((g + 1) * S - 1) / 2, every operation rounded separately in fp32.  theta is torchvision's
+ *    inverse affine matrix rounded to fp32 and divided in fp32 by S / 2 (what _gen_affine_grid multiplies by).
+ *  - 6-8 are ColorJitter's blends (above) with r = arg = fp32(1 + m), one_minus = fp32(1.0 - (1.0 + m)) in double.
+ *  - 9 blends with the rounded [1 1 1; 1 5 1; 1 1 1] / 13 blur over interior pixels (each border pixel blends with
+ *    itself); it is skipped when S <= 2.  The blur is computed exactly in integers: no blur of bytes lies within 1/26
+ *    of a half-integer, so fp32 convolution rounds to the same value.
+ *  - 10 keeps the bits of (int)arg, 11 inverts bytes >= arg (fp32 compare).
+ *  - 12 and 13 work per frame and channel: 12 maps c to trunc((c - min) * s) with s = fp32(1 / (max - min)) * 255
+ *    (torch's 255 / tensor is a reciprocal and a product), unless max == min;
+ *    13 maps through torchvision's equalize table ((cumsum + step / 2) / step shifted right by one bin, lut[0] = 0,
+ *    step = (pixels - count of the highest occupied bin) / 255) unless step == 0.
+ * n_ops outside [0, VT_RANDAUG_MAX_OPS] or an op code outside [0, 13] makes the clip all zeros and sets *err (if given).
+ * Launch: grid n * T, 512 threads, S * S * 3 bytes of dynamic shared memory.
  * ------------------------------------------------------------------------------------------- */
 #define VT_CROP_MAX_TAPS 32
 typedef struct {
@@ -539,6 +559,21 @@ typedef struct {
 } vt_jitter_desc;
 typedef struct { uint8_t* frames; const vt_jitter_desc* desc; int32_t n, T, S; } vt_color_jitter_params;
 int vt_color_jitter_u8(const vt_color_jitter_params* p, void* stream);
+
+#define VT_RANDAUG_MAX_OPS 4
+typedef struct {
+  int32_t n_ops, op[VT_RANDAUG_MAX_OPS];
+  float arg[VT_RANDAUG_MAX_OPS];           /* blend factor, posterize bit mask or solarize threshold */
+  float one_minus[VT_RANDAUG_MAX_OPS];     /* blend ops: fp32(1.0 - (1.0 + m)) */
+  float theta[VT_RANDAUG_MAX_OPS][6];      /* ops 1-5: the rescaled inverse affine matrix, row-major 2 x 3 */
+} vt_randaug_desc;
+typedef struct {
+  uint8_t* frames;
+  const vt_randaug_desc* desc;             /* device table, one per clip */
+  int32_t* err;                            /* optional device flag */
+  int32_t n, T, S;
+} vt_rand_augment_params;
+int vt_rand_augment_u8(const vt_rand_augment_params* p, void* stream);
 
 #ifdef __cplusplus
 }

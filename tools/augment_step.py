@@ -6,11 +6,14 @@ graphed TimeSformer-B train step with the transform inside it against the same s
 
 Prints one JSON line per measurement, after a line with the card's name and power limit read in the same run.
   * transform: CUDA events around `iters` back-to-back runs of the kernels on prepared arenas (batch 8, T = 8 and 16,
-    all clips 256x340 or all 320x427), three windows: median and range.
+    all clips 256x340 or all 320x427), three windows: median and range.  train_ra / mim_ra are the training forms with
+    auto_augment='rand_aug' (RandAugment in place of ColorJitter); their draws differ per prepare, the timed runs replay
+    the last one.
   * cpu_reference: torchvision's composition of the reference's pipelines (data_transform.py:495-615 and the test
     transform of data_trainer.py:110-115, ToTensor + Normalize included) on one thread, per 8-frame clip, three windows.
   * train_step: ms per step of GraphedTrainStep over TimeSformer-B + a 400-class head at batch 8, 8 x 224^2, host work
-    included (the transform's draws and its two uploads); the two arms alternate over three windows each.
+    included (the transform's draws and its two uploads), with the train transform (ColorJitter), with the RandAugment
+    train transform, and fed an already cropped clip; the three arms alternate over three windows each.
 """
 from __future__ import annotations
 
@@ -36,6 +39,10 @@ def forms(S=224):
     return {'train': lambda: A.create_video_transform(S, is_training=True, interpolation='bicubic', mean=MEAN, std=STD),
             'mim': lambda: A.create_video_transform(S, is_training=True, scale=(0.5, 1.0), color_jitter=None,
                                                     interpolation='bicubic', objective='mim', mean=MEAN, std=STD),
+            'train_ra': lambda: A.create_video_transform(S, is_training=True, auto_augment='rand_aug', interpolation='bicubic',
+                                                         mean=MEAN, std=STD),
+            'mim_ra': lambda: A.create_video_transform(S, is_training=True, scale=(0.5, 1.0), auto_augment='rand_aug',
+                                                       interpolation='bicubic', objective='mim', mean=MEAN, std=STD),
             'val': lambda: A.create_video_transform(S, is_training=False, interpolation='bicubic', mean=MEAN, std=STD),
             'test': lambda: A.ThreeCropTest(256, S, mean=MEAN, std=STD)}
 
@@ -74,7 +81,7 @@ def transform_times(iters):
                 host = (time.perf_counter() - host) / iters
                 yield dict(what='transform', form=name, batch=8, frames=T, decode=f'{h}x{w}', ms_per_batch=round(t[1], 4),
                            ms_range=[round(t[0], 4), round(t[2], 4)], prepare_ms=round(host * 1e3, 3),
-                           kernel_launches=1 + int(tf.jitter is not None))
+                           kernel_launches=1 + int(tf.jitter is not None or tf.rand_augment is not None))
 
 
 def cpu_reference(n_clips):
@@ -90,6 +97,10 @@ def cpu_reference(n_clips):
                                   TV.ColorJitter(0.4, 0.4, 0.4), to_tensor, norm]),
              'mim': TV.Compose([TV.RandomResizedCrop(224, scale=(0.5, 1.0), interpolation=I.BICUBIC),
                                 TV.RandomHorizontalFlip(0.5), to_tensor, norm]),
+             'train_ra': TV.Compose([TV.RandomResizedCrop(224, interpolation=I.BICUBIC), TV.RandomHorizontalFlip(0.5),
+                                     TV.RandAugment(), to_tensor, norm]),
+             'mim_ra': TV.Compose([TV.RandomResizedCrop(224, scale=(0.5, 1.0), interpolation=I.BICUBIC),
+                                   TV.RandomHorizontalFlip(0.5), TV.RandAugment(), to_tensor, norm]),
              'val': TV.Compose([TV.Resize(256, interpolation=I.BICUBIC), TV.CenterCrop(224), to_tensor, norm]),
              'test': TV.Compose([TV.Resize(256), lambda x: torch.stack([x[..., 16:240, :224], x[..., 16:240, -224:],
                                                                          x[..., 16:240, 58:282]]), to_tensor, norm])}
@@ -124,17 +135,23 @@ def train_steps(steps, warmup):
               for h, w in ((256, 340), (320, 427))]
     x = torch.randint(0, 256, (8, 8, 224, 224, 3), dtype=torch.uint8, generator=g).to(dev)
     plain = GraphedTrainStep(net, (x, y))
-    tf = forms()['train']()
-    tf.reserve(8 * 8 * 320 * 427 * 3, 8)
-    tf.prepare(packed[0])
-    inside = GraphedTrainStep(lambda lab: net(tf.run(), lab), [y], params=list(net.parameters()))
+    graphed = {}
+    for form in ('train', 'train_ra'):
+        tf = forms()[form]()
+        tf.reserve(8 * 8 * 320 * 427 * 3, 8)
+        tf.prepare(packed[0])
+        graphed[form] = (tf, GraphedTrainStep(lambda lab, tf=tf: net(tf.run(), lab), [y], params=list(net.parameters())))
     k = [0]
 
-    def with_tf():
+    def with_tf(form):
+        tf, step = graphed[form]
         k[0] ^= 1
         tf.prepare(packed[k[0]])
-        inside(y)
-    arms = {'cropped_uint8_input': lambda: plain(x, y), 'gpu_transform_inside': with_tf}
+        step(y)
+    arms = {'cropped_uint8_input': lambda: plain(x, y), 'gpu_transform_inside': lambda: with_tf('train'),
+            'gpu_transform_ra_inside': lambda: with_tf('train_ra')}
+    steps_of = {'cropped_uint8_input': plain, 'gpu_transform_inside': graphed['train'][1],
+                'gpu_transform_ra_inside': graphed['train_ra'][1]}
     times = {a: [] for a in arms}
     for fn in arms.values():
         for _ in range(warmup):
@@ -151,7 +168,7 @@ def train_steps(steps, warmup):
         ts.sort()
         yield dict(what='train_step', arm=a, batch=8, frames=8, ms_per_step=round(ts[1], 3),
                    ms_range=[round(ts[0], 3), round(ts[2], 3)],
-                   kernels_per_replay=(inside if a == 'gpu_transform_inside' else plain).kernels_per_replay)
+                   kernels_per_replay=steps_of[a].kernels_per_replay)
 
 
 def main():

@@ -272,6 +272,18 @@ class ColorJitterParams(C.Structure):
     _fields_ = [('frames', c_vp), ('desc', c_vp), ('n', c_i32), ('T', c_i32), ('S', c_i32)]
 
 
+RANDAUG_MAX_OPS = 4                     # VT_RANDAUG_MAX_OPS
+
+
+class RandAugDesc(C.Structure):
+    _fields_ = [('n_ops', c_i32), ('op', c_i32 * RANDAUG_MAX_OPS), ('arg', c_f32 * RANDAUG_MAX_OPS),
+                ('one_minus', c_f32 * RANDAUG_MAX_OPS), ('theta', (c_f32 * 6) * RANDAUG_MAX_OPS)]
+
+
+class RandAugmentParams(C.Structure):
+    _fields_ = [('frames', c_vp), ('desc', c_vp), ('err', c_vp), ('n', c_i32), ('T', c_i32), ('S', c_i32)]
+
+
 EXPORTS = ['vt_version', 'vt_last_error', 'vt_sm_count', 'vt_set_reserved_sms', 'vt_launch_count', 'vt_gemm', 'vt_layernorm_fwd', 'vt_ln_bwd_blocks',
            'vt_layernorm_bwd', 'vt_reduce_rows', 'vt_colsum_chunks', 'vt_colsum_bf16', 'vt_cast_f32_bf16',
            'vt_cls_rows', 'vt_gather_cast_colsum_blocks', 'vt_gather_cast_colsum_bf16', 'vt_gelu_bwd_colsum_blocks', 'vt_gelu_bwd_colsum_bf16',
@@ -281,7 +293,7 @@ EXPORTS = ['vt_version', 'vt_last_error', 'vt_sm_count', 'vt_set_reserved_sms', 
            'vt_mse_fwd', 'vt_mse_bwd', 'vt_opt_norm2', 'vt_opt_sgd', 'vt_opt_adamw',
            'vt_linear_small_fwd', 'vt_linear_small_bwd', 'vt_softmax_ce', 'vt_scale_by_scalar', 'vt_attn_probs',
            'vt_im2col_u8_mix_bf16', 'vt_pos_resize_fwd', 'vt_pos_resize_bwd', 'vt_topk_hits',
-           'vt_resized_crop_u8', 'vt_color_jitter_u8', 'vt_gemm_e4m3', 'vt_quant_rows_e4m3']
+           'vt_resized_crop_u8', 'vt_color_jitter_u8', 'vt_gemm_e4m3', 'vt_quant_rows_e4m3', 'vt_rand_augment_u8']
 
 _dll = None
 
@@ -915,6 +927,23 @@ class CudaKernels:
         p.frames, p.desc = frames.data_ptr(), _req(desc, torch.uint8, 'color_jitter.desc').data_ptr()
         p.n, p.T, p.S = n, T, S
         _check(lib.vt_color_jitter_u8(C.byref(p), _stream()), 'vt_color_jitter_u8')
+        return frames
+
+    def rand_augment_u8(self, frames, desc, err=None):
+        """RandAugment in place on uint8 [n, T, S, S, 3] with one RandAugDesc per clip (uint8 device bytes); err: optional
+        int32 [1] set to 1 by a descriptor with a bad op code or op count (its clip is zeroed)."""
+        lib = load_library()
+        _req(frames, torch.uint8, 'rand_augment.frames')
+        if not frames.is_contiguous() or frames.dim() != 5 or frames.shape[2] != frames.shape[3] or frames.shape[4] != 3:
+            raise RuntimeError('rand_augment_u8: frames must be a contiguous [n, T, S, S, 3] tensor')
+        n, T, S = frames.shape[:3]
+        if desc.numel() < n * C.sizeof(RandAugDesc):
+            raise RuntimeError(f'rand_augment_u8: desc holds fewer than {n} descriptors')
+        p = RandAugmentParams()
+        p.frames, p.desc = frames.data_ptr(), _req(desc, torch.uint8, 'rand_augment.desc').data_ptr()
+        p.err = _ptr(None if err is None else _req(err, torch.int32, 'rand_augment.err'))
+        p.n, p.T, p.S = n, T, S
+        _check(lib.vt_rand_augment_u8(C.byref(p), _stream()), 'vt_rand_augment_u8')
         return frames
 
     # -- HOG ------------------------------------------------------------------------------------

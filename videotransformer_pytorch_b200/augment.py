@@ -6,6 +6,7 @@ the DataLoader workers on each uint8 T C H W clip.  Here the workers only decode
 any sizes into one flat buffer) and the per-pixel work runs in two kernels (csrc/vt_augment.cu):
 
   train       RandomResizedCrop(S, scale, ratio) -> RandomHorizontalFlip(hflip) -> ColorJitter(cj, cj, cj)
+              or, with auto_augment, -> RandAugment() instead of ColorJitter (supervised and mim)
   train mim   RandomResizedCrop(S, scale=(0.5, 1)) -> RandomHorizontalFlip, no jitter
   val         Resize(floor(S / crop_pct)) (short side) -> CenterCrop(S)
   test        Resize(256) (short side, bilinear) -> ThreeCrop(S): views left, right, centre, clip-major
@@ -15,11 +16,13 @@ patch-operand kernel applies them.
 
 The random parameters are drawn on the host from torch's default CPU generator with the calls torchvision 0.26 makes, in
 the order Compose applies the transforms, once per clip (all frames of a clip share them): RandomResizedCrop.get_params,
-then torch.rand(1) < hflip, then ColorJitter.get_params (torch.randperm(4) and one uniform_ per factor; hue is never drawn).
-Under the same seed the crops, flips and jitter factors are the reference's.  The resize matches torchvision's uint8
+then torch.rand(1) < hflip, then ColorJitter.get_params (torch.randperm(4) and one uniform_ per factor; hue is never drawn)
+or RandAugment's draws (per op torch.randint(14), then torch.randint(2) for the sign of a signed op).  Under the same
+seed the crops, flips, jitter factors and RandAugment ops are the reference's.  The resize matches torchvision's uint8
 output up to the last bits of its fp32 pre-rounding value (a byte can differ by 1 where that value lies within
 1.75e-4 per filter tap, 2.8e-3 at 256x340 -> 224^2, of a half-integer); the jitter is bit for bit torchvision's on the
-same input.
+same input, and so is RandAugment except where a warped pixel's source coordinate lies within about 2e-4 of a
+half-integer (see rand_augment_params).
 
 The kernels read only two fixed device arenas (source bytes and descriptors), each refilled by one copy in `prepare`, and
 their launch configuration depends only on (clips, T, S).  So `run` can be captured in a CUDA graph (graph.GraphedTrainStep,
@@ -49,6 +52,10 @@ FILTERS = {'bicubic': 0, 'bilinear': 1}
 MAX_TAPS = 32                     # VT_CROP_MAX_TAPS
 BRIGHTNESS, CONTRAST, SATURATION = 0, 1, 2
 MAX_JITTER_SIDE = 256             # vt_color_jitter_u8: the frame in shared memory, its grayscale sum exact in fp32
+RANDAUG_OPS = ('Identity', 'ShearX', 'ShearY', 'TranslateX', 'TranslateY', 'Rotate', 'Brightness', 'Color', 'Contrast',
+               'Sharpness', 'Posterize', 'Solarize', 'AutoContrast', 'Equalize')      # torchvision's order = kernel op code
+RANDAUG_DEFAULTS = (2, 9, 31)     # RandAugment(): num_ops, magnitude, num_magnitude_bins
+MAX_RANDAUG_SIDE = 256            # vt_rand_augment_u8: the frame in shared memory
 
 
 # ---- parameter draws: torchvision 0.26's get_params, same torch calls in the same order --------------------------------
@@ -84,6 +91,71 @@ def color_jitter_params(brightness, contrast, saturation):
     for op, rng in ((BRIGHTNESS, brightness), (CONTRAST, contrast), (SATURATION, saturation)):
         f[op] = None if rng is None else float(torch.empty(1).uniform_(rng[0], rng[1]))
     return [(int(i), f[int(i)]) for i in fn_idx.tolist() if int(i) in f and f[int(i)] is not None]
+
+
+def _randaug_space(num_bins: int, S: int):
+    """RandAugment._augmentation_space(num_bins, (S, S)) as a list in op order: (magnitudes, signed)"""
+    return [(torch.tensor(0.0), False),
+            (torch.linspace(0.0, 0.3, num_bins), True),
+            (torch.linspace(0.0, 0.3, num_bins), True),
+            (torch.linspace(0.0, 150.0 / 331.0 * S, num_bins), True),
+            (torch.linspace(0.0, 150.0 / 331.0 * S, num_bins), True),
+            (torch.linspace(0.0, 30.0, num_bins), True),
+            (torch.linspace(0.0, 0.9, num_bins), True),
+            (torch.linspace(0.0, 0.9, num_bins), True),
+            (torch.linspace(0.0, 0.9, num_bins), True),
+            (torch.linspace(0.0, 0.9, num_bins), True),
+            (8 - (torch.arange(num_bins) / ((num_bins - 1) / 4)).round().int(), False),
+            (torch.linspace(255.0, 0.0, num_bins), False),
+            (torch.tensor(0.0), False),
+            (torch.tensor(0.0), False)]
+
+
+def rand_augment_params(S: int, num_ops: int = 2, magnitude: int = 9, num_magnitude_bins: int = 31):
+    """RandAugment.forward's draws on an S x S image -> [(op, signed magnitude), ...] with op the index in RANDAUG_OPS
+    and the magnitude torchvision hands to _apply_op: per op torch.randint(14), then torch.randint(2) for the sign of a
+    signed op (not drawn for the others)."""
+    space = _randaug_space(num_magnitude_bins, S)
+    out = []
+    for _ in range(num_ops):
+        op = int(torch.randint(len(space), (1,)).item())
+        mags, signed = space[op]
+        m = float(mags[magnitude].item()) if mags.ndim > 0 else 0.0
+        if signed and torch.randint(2, (1,)):
+            m *= -1.0
+        out.append((op, m))
+    return out
+
+
+def _inverse_affine(center, angle, translate, shear):
+    """torchvision's _get_inverse_affine_matrix at scale 1 (the same double operations in the same order)"""
+    rot, sx, sy = math.radians(angle), math.radians(shear[0]), math.radians(shear[1])
+    (cx, cy), (tx, ty) = center, translate
+    a = math.cos(rot - sy) / math.cos(sy)
+    b = -math.cos(rot - sy) * math.tan(sx) / math.cos(sy) - math.sin(rot)
+    c = math.sin(rot - sy) / math.cos(sy)
+    d = -math.sin(rot - sy) * math.tan(sx) / math.cos(sy) + math.cos(rot)
+    m = [d, -b, 0.0, -c, a, 0.0]
+    m[2] += m[0] * (-cx - tx) + m[1] * (-cy - ty)
+    m[5] += m[3] * (-cx - tx) + m[4] * (-cy - ty)
+    m[2] += cx
+    m[5] += cy
+    return m
+
+
+def randaug_theta(op: int, m: float, S: int):
+    """The grid matrix of a warp op as _gen_affine_grid uses it: the inverse affine matrix F.affine / F.rotate build
+    (shears about the top-left corner, translations by int(m), rotation by -m), rounded to fp32, divided in fp32 by S / 2."""
+    corner = [-S * 0.5, -S * 0.5]                     # center=[0, 0] in F.affine's centred coordinates
+    if op in (1, 2):
+        sh = math.degrees(math.atan(m))
+        mat = _inverse_affine(corner, 0.0, [0.0, 0.0], [sh, 0.0] if op == 1 else [0.0, sh])
+    elif op in (3, 4):
+        t = [1.0 * int(m), 0.0] if op == 3 else [0.0, 1.0 * int(m)]
+        mat = _inverse_affine([0.0, 0.0], 0.0, t, [0.0, 0.0])
+    else:
+        mat = _inverse_affine([0.0, 0.0], -m, [0.0, 0.0], [0.0, 0.0])
+    return np.float32(mat) / np.float32(0.5 * S)
 
 
 def _jitter_range(value):
@@ -174,7 +246,7 @@ class ClipTransform:
 
     def __init__(self, size: int, mode: str, *, scale=(0.08, 1.0), ratio=(3. / 4., 4. / 3.), hflip=0.5, color_jitter=None,
                  interpolation='bilinear', resize_to: Optional[int] = None, mean=IMAGENET_DEFAULT_MEAN,
-                 std=IMAGENET_DEFAULT_STD, device=None):
+                 std=IMAGENET_DEFAULT_STD, rand_augment=None, device=None):
         if mode not in ('train', 'center', 'three'):
             raise ValueError(f'unknown mode {mode!r}')
         if interpolation not in FILTERS:
@@ -195,10 +267,22 @@ class ClipTransform:
                 self.jitter = None
         if self.jitter is not None and self.size > MAX_JITTER_SIDE:
             raise ValueError(f'ColorJitter on the GPU needs S <= {MAX_JITTER_SIDE} (got {self.size})')
+        self.rand_augment = None
+        if rand_augment is not None:
+            num_ops, magnitude, bins = (int(v) for v in rand_augment)
+            if mode != 'train' or self.jitter is not None:
+                raise ValueError('rand_augment is a training transform and replaces color_jitter')
+            if not (0 <= num_ops <= _lib.RANDAUG_MAX_OPS and bins >= 2 and 0 <= magnitude < bins):
+                raise ValueError(f'rand_augment=(num_ops, magnitude, num_magnitude_bins) needs num_ops <= '
+                                 f'{_lib.RANDAUG_MAX_OPS} and 0 <= magnitude < num_magnitude_bins, got {tuple(rand_augment)}')
+            if self.size > MAX_RANDAUG_SIDE:
+                raise ValueError(f'RandAugment on the GPU needs S <= {MAX_RANDAUG_SIDE} (got {self.size})')
+            self.rand_augment = (num_ops, magnitude, bins)
         self.mean, self.std = tuple(mean), tuple(std)
         self.views = 3 if mode == 'three' else 1
         self.device = torch.device(device) if device is not None else None
-        self.src = None               # source arena (uint8), desc = descriptor arena: crop table then jitter table
+        self.src = None               # source arena (uint8), desc = descriptor arena: crop table, then the jitter or
+                                      # RandAugment table
         self.desc = None
         self.err = None
         self._shape = None            # (outputs, T) of the last prepare
@@ -208,14 +292,15 @@ class ClipTransform:
     # -- host ----------------------------------------------------------------------------------------------------------
     def draw(self, sizes):
         """sizes: [(H, W), ...] per clip -> descriptors, a list per clip of dicts (one per output view) with the crop box,
-        resized size, window, flip, filter and jitter ops, drawn in the reference's order."""
+        resized size, window, flip, filter, jitter ops and RandAugment ops ('ra'), drawn in the reference's order."""
         S, out = self.size, []
         for H, W in sizes:
             if self.mode == 'train':
                 i, j, h, w = random_resized_crop_params(H, W, self.scale, self.ratio)
                 flip = bool(torch.rand(1) < self.hflip) if self.hflip > 0 else False
                 ops = color_jitter_params(*self.jitter) if self.jitter is not None else []
-                out.append([dict(crop=(i, j, h, w), resized=(S, S), window=(0, 0), flip=flip, ops=ops)])
+                ra = rand_augment_params(S, *self.rand_augment) if self.rand_augment is not None else []
+                out.append([dict(crop=(i, j, h, w), resized=(S, S), window=(0, 0), flip=flip, ops=ops, ra=ra)])
                 continue
             RH, RW = resize_short_side(H, W, self.resize_to)
             if S > RH or S > RW:
@@ -231,6 +316,7 @@ class ClipTransform:
     def _pack(self, views, shapes, offsets):
         n = sum(len(v) for v in views)
         crops, jit = (_lib.CropDesc * n)(), (_lib.JitterDesc * n)()
+        ra = (_lib.RandAugDesc * n)() if self.rand_augment is not None else None
         k = 0
         for b, per_clip in enumerate(views):
             T, H, W = shapes[b]
@@ -250,8 +336,10 @@ class ClipTransform:
                     jd.op[s] = op
                     jd.factor[s] = f                                     # an fp32 value (from a float32 tensor)
                     jd.one_minus[s] = np.float32(1.0 - f)               # torchvision: (1.0 - ratio) in double, fp32 op
+                if ra is not None:
+                    _pack_randaug(ra[k], v['ra'], self.size)
                 k += 1
-        return bytes(crops) + bytes(jit), n
+        return bytes(crops) + (bytes(jit) if ra is None else bytes(ra)), n
 
     def _stage(self, payload: bytes, nbytes_cap: int, dev):
         cuda = dev.type == 'cuda'
@@ -288,7 +376,11 @@ class ClipTransform:
         """Size the arenas for batches of up to `clips` clips and `src_bytes` source bytes (before a graph capture)."""
         dev = self._device(torch.device(device) if device is not None else torch.device('cuda'))
         self._arena('src', src_bytes, dev)
-        self._arena('desc', clips * self.views * (C.sizeof(_lib.CropDesc) + C.sizeof(_lib.JitterDesc)), dev)
+        self._arena('desc', clips * self.views * (C.sizeof(_lib.CropDesc) + C.sizeof(self._second_desc())), dev)
+
+    def _second_desc(self):
+        """the descriptor type of the table after the crop table"""
+        return _lib.RandAugDesc if self.rand_augment is not None else _lib.JitterDesc
 
     def prepare(self, clips: Union[PackedClips, Sequence[torch.Tensor]]):
         """Draw this batch's parameters and upload sources and descriptors into the arenas."""
@@ -336,7 +428,8 @@ class ClipTransform:
 
     # -- device --------------------------------------------------------------------------------------------------------
     def run(self) -> torch.Tensor:
-        """Launch the transform on the arenas (one resize launch, one jitter launch in training with jitter)."""
+        """Launch the transform on the arenas (one resize launch, then one jitter or RandAugment launch in training with
+        either)."""
         if self._shape is None:
             raise RuntimeError('ClipTransform.run: nothing prepared')
         n, T = self._shape
@@ -348,6 +441,8 @@ class ClipTransform:
         _lib.K.resized_crop_u8(self.src, self.desc[:ncrop], out, self.err)
         if self.jitter is not None:
             _lib.K.color_jitter_u8(out, self.desc[ncrop:ncrop + n * C.sizeof(_lib.JitterDesc)])
+        if self.rand_augment is not None:
+            _lib.K.rand_augment_u8(out, self.desc[ncrop:ncrop + n * C.sizeof(_lib.RandAugDesc)], self.err)
         return out
 
     def __call__(self, clips):
@@ -356,7 +451,8 @@ class ClipTransform:
 
     def __repr__(self):
         return (f'{type(self).__name__}(size={self.size}, mode={self.mode!r}, scale={self.scale}, ratio={self.ratio}, '
-                f'hflip={self.hflip}, jitter={self.jitter}, filter={self.filter}, resize_to={self.resize_to})')
+                f'hflip={self.hflip}, jitter={self.jitter}, rand_augment={self.rand_augment}, filter={self.filter}, '
+                f'resize_to={self.resize_to})')
 
 
 def create_video_transform(input_size=224, is_training=False, scale=None, ratio=None, hflip=0.5, color_jitter=0.4,
@@ -364,19 +460,47 @@ def create_video_transform(input_size=224, is_training=False, scale=None, ratio=
                            std=IMAGENET_DEFAULT_STD, objective='supervised', crop_pct=None, device=None) -> ClipTransform:
     """data_transform.create_video_transform with the same arguments and defaults, on the GPU.  The `mim` objective
     returns one transform (the reference returns [crop + flip, ToTensor + Normalize]; here Normalize is the model's, via
-    set_input_normalization(tf.mean, tf.std)), and the HOG targets are computed from its output."""
+    set_input_normalization(tf.mean, tf.std)), and the HOG targets are computed from its output.
+
+    A truthy auto_augment selects torchvision's RandAugment() with its defaults in place of ColorJitter, as the
+    reference's transforms_train does for every truthy value.  timm policy strings ('rand-m9-mstd0.5-inc1', ...) raise
+    NotImplementedError: the reference would silently ignore their magnitude noise and severity fields."""
     img_size = input_size[-1] if isinstance(input_size, (tuple, list)) else input_size
     if isinstance(input_size, (tuple, list)) and input_size[-1] != input_size[-2]:
         raise ValueError('the GPU transforms produce square clips')
     if is_training:
+        rand_augment = None
         if auto_augment:
-            raise NotImplementedError('RandAugment (auto_augment) is not implemented on the GPU')
+            if isinstance(auto_augment, str) and auto_augment.startswith('rand-'):
+                raise NotImplementedError(
+                    f'auto_augment={auto_augment!r}: timm RandAugment policy strings are not implemented on the GPU.  The '
+                    f'reference builds torchvision\'s RandAugment() for any auto_augment and silently ignores the '
+                    f'string\'s magnitude noise and increasing-severity fields; pass auto_augment=\'rand_aug\' (or True) '
+                    f'for that transform.')
+            rand_augment, color_jitter = RANDAUG_DEFAULTS, None
         return ClipTransform(img_size, 'train', scale=tuple(scale or (0.08, 1.0)), ratio=tuple(ratio or (3. / 4., 4. / 3.)),
                              hflip=hflip, color_jitter=color_jitter, interpolation=interpolation, mean=mean, std=std,
-                             device=device)
+                             rand_augment=rand_augment, device=device)
     crop_pct = crop_pct or DEFAULT_CROP_PCT
     return ClipTransform(img_size, 'center', interpolation=interpolation, resize_to=int(math.floor(img_size / crop_pct)),
                          mean=mean, std=std, device=device)
+
+
+def _pack_randaug(d, ops, S: int):
+    """Fill one RandAugDesc from [(op, signed magnitude), ...] as _apply_op would apply them to an S x S frame."""
+    d.n_ops = len(ops)
+    for s, (op, m) in enumerate(ops):
+        d.op[s] = op
+        if 1 <= op <= 5:
+            for k, v in enumerate(randaug_theta(op, m, S)):
+                d.theta[s][k] = v
+        elif 6 <= op <= 9:                            # _blend(img, ., 1.0 + m): fp32 ratio and fp32 (1.0 - ratio)
+            d.arg[s] = np.float32(1.0 + m)
+            d.one_minus[s] = np.float32(1.0 - (1.0 + m))
+        elif op == 10:                                # posterize(img, int(m)): img & -2 ** (8 - bits)
+            d.arg[s] = float(-int(2 ** (8 - int(m))) & 0xFF)
+        elif op == 11:                                # solarize: an fp32 threshold
+            d.arg[s] = m
 
 
 def ThreeCropTest(short_side=256, size=224, mean=IMAGENET_DEFAULT_MEAN, std=IMAGENET_DEFAULT_STD, device=None):

@@ -20,6 +20,11 @@
 // ColorJitter.  One CTA per frame holds the S x S x 3 frame in shared memory and applies the clip's ops in order.  The
 // contrast mean is torch.mean over the fp32 grayscale frame: an integer sum (exact in fp32 up to 254 * 256 * 256 < 2^24)
 // divided by S * S.
+//
+// RandAugment.  The same one-CTA-per-frame layout, with torchvision's 14 ops applied in the drawn order.  Pointwise ops
+// and the per-frame statistics (grayscale sum, per-channel min / max and histograms: warp reductions, then shared
+// atomics) work on the frame in shared memory.  Ops that read other pixels (shears, translations, rotation, sharpness)
+// gather from shared memory into the frame's global output, which is reloaded only if another op follows.
 #include "vt_common.cuh"
 
 namespace vt {
@@ -199,6 +204,191 @@ color_jitter_u8_kernel(uint8_t* __restrict__ frames, const vt_jitter_desc* __res
   }
 }
 
+enum RandAugOp {
+  RA_IDENTITY, RA_SHEAR_X, RA_SHEAR_Y, RA_TRANSLATE_X, RA_TRANSLATE_Y, RA_ROTATE, RA_BRIGHTNESS, RA_COLOR, RA_CONTRAST,
+  RA_SHARPNESS, RA_POSTERIZE, RA_SOLARIZE, RA_AUTOCONTRAST, RA_EQUALIZE, RA_NUM_OPS
+};
+
+constexpr int RA_THREADS = 512;
+
+__device__ __forceinline__ void copy_frame(uint8_t* dst, const uint8_t* src, int nbytes, bool vec) {
+  if (vec) {
+    for (int k = threadIdx.x; k < nbytes / 16; k += blockDim.x) reinterpret_cast<uint4*>(dst)[k] = reinterpret_cast<const uint4*>(src)[k];
+  } else {
+    for (int k = threadIdx.x; k < nbytes; k += blockDim.x) dst[k] = src[k];
+  }
+}
+
+// source coordinate of output index i along an axis: ((g + 1) * S - 1) / 2, nearest (half to even); -1 when outside
+__device__ __forceinline__ int nearest_source(float g, int S) {
+  const float u = rintf(__fmul_rn(__fsub_rn(__fmul_rn(__fadd_rn(g, 1.f), (float)S), 1.f), 0.5f));
+  return u >= 0.f && u <= (float)(S - 1) ? (int)u : -1;
+}
+
+// Equalize table of channel `c` (one warp): lane l owns bins 8l .. 8l + 7 of hist and writes the same entries of lut.
+__device__ void equalize_lut(const unsigned int* hist, uint8_t* lut, int npx) {
+  const int lane = threadIdx.x & 31;
+  unsigned int h[8], local = 0;
+  int top = -1;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    h[k] = hist[8 * lane + k];
+    local += h[k];
+    if (h[k]) top = 8 * lane + k;
+  }
+  top = __reduce_max_sync(0xffffffffu, top + 1) - 1;      // the highest occupied bin (npx > 0, so one exists)
+  const unsigned int step = (unsigned int)(npx - (int)hist[top]) / 255u;
+  unsigned int incl = local;                               // inclusive scan of the lanes' totals
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned int v = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += v;
+  }
+  unsigned int before = incl - local;                      // pixels in bins below 8 * lane
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const int i = 8 * lane + k;
+    lut[i] = step == 0 ? (uint8_t)i : i == 0 ? 0 : (uint8_t)min((before + step / 2) / step, 255u);
+    before += h[k];
+  }
+}
+
+// The frame buffer is written by this CTA and read back by it after a gather op, so it is not read through the
+// read-only path (no const __restrict__ / __ldg).
+__global__ void __launch_bounds__(RA_THREADS)
+rand_augment_u8_kernel(uint8_t* frames, const vt_randaug_desc* __restrict__ descs, int32_t* err, int T, int S) {
+  extern __shared__ __align__(16) uint8_t px[];
+  __shared__ unsigned int stat[3 * 256];                   // histograms, or the grayscale sum / per-channel min, max
+  __shared__ uint8_t lut[3 * 256];
+  const vt_randaug_desc& d = descs[blockIdx.x / T];
+  const int npx = S * S;
+  const int nbytes = npx * 3;
+  uint8_t* g = frames + (int64_t)blockIdx.x * nbytes;
+  const int n_ops = d.n_ops;
+  bool ok = n_ops >= 0 && n_ops <= VT_RANDAUG_MAX_OPS;
+  for (int s = 0; ok && s < n_ops; ++s) ok = d.op[s] >= 0 && d.op[s] < RA_NUM_OPS;
+  if (!ok) {
+    if (threadIdx.x == 0 && err) *err = 1;
+    for (int k = threadIdx.x; k < nbytes; k += blockDim.x) g[k] = 0;
+    return;
+  }
+  const bool vec = (nbytes % 16) == 0 && (reinterpret_cast<uintptr_t>(g) % 16) == 0;
+  bool loaded = false, dirty = false;                      // px holds the frame / px is newer than g
+  const float off = __fsub_rn(0.5f, __fmul_rn(0.5f, (float)S));        // x of column 0: -S/2 + 0.5
+  for (int s = 0; s < n_ops; ++s) {
+    const int op = d.op[s];
+    if (op == RA_IDENTITY || (op == RA_SHARPNESS && S <= 2)) continue;
+    if (!loaded) {
+      copy_frame(px, g, nbytes, vec);
+      __syncthreads();
+      loaded = true;
+    }
+    const float r = d.arg[s], rc = d.one_minus[s];
+    if (op <= RA_ROTATE || op == RA_SHARPNESS) {           // gather from px into g, then reload px if an op follows
+      const float* th = d.theta[s];
+      for (int p = threadIdx.x; p < npx; p += blockDim.x) {
+        const int row = p / S, col = p % S;
+        const uint8_t* q = px + 3 * p;
+        uint8_t o0, o1, o2;
+        if (op == RA_SHARPNESS) {
+          const float c0 = q[0], c1 = q[1], c2 = q[2];
+          float y0 = c0, y1 = c1, y2 = c2;
+          if (row > 0 && row < S - 1 && col > 0 && col < S - 1) {
+            int n0 = 0, n1 = 0, n2 = 0;                    // 3 x 3 sum plus 4 x centre: 13 x the blur
+            for (int dy = -1; dy <= 1; ++dy)
+              for (int dx = -1; dx <= 1; ++dx) {
+                const uint8_t* e = q + 3 * (dy * S + dx);
+                n0 += e[0], n1 += e[1], n2 += e[2];
+              }
+            n0 += 4 * q[0], n1 += 4 * q[1], n2 += 4 * q[2];
+            y0 = (float)((2 * n0 + 13) / 26), y1 = (float)((2 * n1 + 13) / 26), y2 = (float)((2 * n2 + 13) / 26);
+          }
+          o0 = blend_u8(c0, y0, r, rc), o1 = blend_u8(c1, y1, r, rc), o2 = blend_u8(c2, y2, r, rc);
+        } else {
+          const float x = __fadd_rn((float)col, off), y = __fadd_rn((float)row, off);
+          const int sx = nearest_source(__fadd_rn(__fadd_rn(__fmul_rn(x, th[0]), __fmul_rn(y, th[1])), th[2]), S);
+          const int sy = nearest_source(__fadd_rn(__fadd_rn(__fmul_rn(x, th[3]), __fmul_rn(y, th[4])), th[5]), S);
+          if (sx >= 0 && sy >= 0) {
+            const uint8_t* e = px + 3 * (sy * S + sx);
+            o0 = e[0], o1 = e[1], o2 = e[2];
+          } else {
+            o0 = o1 = o2 = 0;
+          }
+        }
+        g[3 * p] = o0, g[3 * p + 1] = o1, g[3 * p + 2] = o2;
+      }
+      __syncthreads();
+      dirty = false;
+      loaded = false;
+      continue;
+    }
+    float mean = 0.f;
+    if (op == RA_CONTRAST || op == RA_AUTOCONTRAST || op == RA_EQUALIZE) {
+      for (int k = threadIdx.x; k < 3 * 256; k += blockDim.x) stat[k] = op == RA_AUTOCONTRAST && k < 3 ? 255u : 0u;
+      __syncthreads();
+      if (op == RA_CONTRAST) {
+        unsigned int part = 0;
+        for (int p = threadIdx.x; p < npx; p += blockDim.x) part += (unsigned int)gray_u8(px[3 * p], px[3 * p + 1], px[3 * p + 2]);
+        part = __reduce_add_sync(0xffffffffu, part);
+        if ((threadIdx.x & 31) == 0) atomicAdd(&stat[0], part);
+      } else if (op == RA_AUTOCONTRAST) {
+        unsigned int mn0 = 255, mn1 = 255, mn2 = 255, mx0 = 0, mx1 = 0, mx2 = 0;
+        for (int p = threadIdx.x; p < npx; p += blockDim.x) {
+          const unsigned int c0 = px[3 * p], c1 = px[3 * p + 1], c2 = px[3 * p + 2];
+          mn0 = min(mn0, c0), mn1 = min(mn1, c1), mn2 = min(mn2, c2);
+          mx0 = max(mx0, c0), mx1 = max(mx1, c1), mx2 = max(mx2, c2);
+        }
+        mn0 = __reduce_min_sync(0xffffffffu, mn0), mn1 = __reduce_min_sync(0xffffffffu, mn1);
+        mn2 = __reduce_min_sync(0xffffffffu, mn2), mx0 = __reduce_max_sync(0xffffffffu, mx0);
+        mx1 = __reduce_max_sync(0xffffffffu, mx1), mx2 = __reduce_max_sync(0xffffffffu, mx2);
+        if ((threadIdx.x & 31) == 0) {
+          atomicMin(&stat[0], mn0), atomicMin(&stat[1], mn1), atomicMin(&stat[2], mn2);
+          atomicMax(&stat[3], mx0), atomicMax(&stat[4], mx1), atomicMax(&stat[5], mx2);
+        }
+      } else {
+        for (int p = threadIdx.x; p < npx; p += blockDim.x) {
+          atomicAdd(&stat[px[3 * p]], 1u);
+          atomicAdd(&stat[256 + px[3 * p + 1]], 1u);
+          atomicAdd(&stat[512 + px[3 * p + 2]], 1u);
+        }
+      }
+      __syncthreads();
+      if (op == RA_CONTRAST) mean = __fdiv_rn((float)stat[0], (float)npx);
+      if (op == RA_EQUALIZE) {
+        if (threadIdx.x < 96) equalize_lut(stat + 256 * (threadIdx.x >> 5), lut + 256 * (threadIdx.x >> 5), npx);
+        __syncthreads();
+      }
+    }
+    const unsigned int mask = op == RA_POSTERIZE ? (unsigned int)r : 0u;
+    for (int p = threadIdx.x; p < npx; p += blockDim.x) {
+      uint8_t* q = px + 3 * p;
+      if (op == RA_POSTERIZE) {
+        q[0] &= mask, q[1] &= mask, q[2] &= mask;
+      } else if (op == RA_SOLARIZE) {
+        for (int c = 0; c < 3; ++c) q[c] = (float)q[c] >= r ? 255 - q[c] : q[c];
+      } else if (op == RA_AUTOCONTRAST) {
+        for (int c = 0; c < 3; ++c) {
+          const unsigned int mn = stat[c], mx = stat[3 + c];
+          if (mx != mn) {
+            // torch evaluates 255 / (max - min) as reciprocal(max - min) * 255
+            const float v = __fmul_rn((float)(q[c] - mn), __fmul_rn(__frcp_rn((float)(mx - mn)), 255.f));
+            q[c] = (uint8_t)__float2uint_rz(fminf(fmaxf(v, 0.f), 255.f));
+          }
+        }
+      } else if (op == RA_EQUALIZE) {
+        q[0] = lut[q[0]], q[1] = lut[256 + q[1]], q[2] = lut[512 + q[2]];
+      } else {                                             // brightness, color (saturation), contrast
+        const float c0 = q[0], c1 = q[1], c2 = q[2];
+        const float y = op == RA_BRIGHTNESS ? 0.f : op == RA_CONTRAST ? mean : gray_u8(c0, c1, c2);
+        q[0] = blend_u8(c0, y, r, rc), q[1] = blend_u8(c1, y, r, rc), q[2] = blend_u8(c2, y, r, rc);
+      }
+    }
+    __syncthreads();
+    dirty = true;
+  }
+  if (dirty) copy_frame(g, px, nbytes, vec);
+}
+
 }  // namespace vt
 
 extern "C" int vt_resized_crop_u8(const vt_resized_crop_params* p, void* stream) {
@@ -226,4 +416,18 @@ extern "C" int vt_color_jitter_u8(const vt_color_jitter_params* p, void* stream)
   color_jitter_u8_kernel<<<p->n * p->T, JITTER_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
       p->frames, p->desc, p->T, p->S);
   return check_launch("color_jitter_u8_kernel");
+}
+
+extern "C" int vt_rand_augment_u8(const vt_rand_augment_params* p, void* stream) {
+  using namespace vt;
+  VT_REQUIRE(p && p->frames && p->desc, "vt_rand_augment_u8: null pointer");
+  VT_REQUIRE(p->n > 0 && p->T > 0 && p->S > 0, "vt_rand_augment_u8: bad sizes n=%d T=%d S=%d", p->n, p->T, p->S);
+  VT_REQUIRE(p->S <= 256, "vt_rand_augment_u8: S=%d > 256 (the frame must fit in shared memory and its grayscale sum in "
+             "fp32's exact integers)", p->S);
+  VT_REQUIRE((int64_t)p->n * p->T < (1ll << 31), "vt_rand_augment_u8: too many frames");
+  const size_t smem = (size_t)p->S * p->S * 3;
+  cudaFuncSetAttribute(rand_augment_u8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+  rand_augment_u8_kernel<<<p->n * p->T, RA_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(
+      p->frames, p->desc, p->err, p->T, p->S);
+  return check_launch("rand_augment_u8_kernel");
 }
