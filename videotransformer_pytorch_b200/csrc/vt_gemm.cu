@@ -2,7 +2,10 @@
 //   TMA (cp.async.bulk.tensor, 128B swizzle) -> shared-memory ring (mbarrier full / empty pairs) -> wgmma.mma_async
 //   (fp32 accumulators in registers) -> epilogue fused with bias / GELU / dGELU / residual / row maps.  The bf16-output
 //   forms on plain rows stage the tile in shared memory and write it with TMA stores that run under the next tile's
-//   MMAs; the others write straight from the accumulator registers to global memory.
+//   MMAs.  The fp32 forms (residual adds through any row map, split-K partials) stage padded fp32 rows instead: two
+//   otherwise idle warps of the producer warpgroup load each tile's residual rows with 1-D bulk copies while its MMAs run
+//   and store the result rows the same way under the next tile's.  The bf16 forms with an output row map, and fp32 calls
+//   at BN = 256 or with rows that are not 16-byte aligned, write straight from the accumulator registers to global memory.
 // Persistent: one CTA per SM walks a static sequence of 128 x BN output tiles (x K split), BN in {128, 192, 256}.  384
 // threads: warpgroup 0 = TMA producer (one thread), warpgroups 1-2 = consumers, each owning 64 rows of every tile.  The
 // producer runs ahead across tile boundaries, so the next tile's first k-blocks load while the consumers run the epilogue.
@@ -48,8 +51,10 @@ struct GemmDev {
 };
 
 // Epilogue kinds (kernel template parameter SE): 0 = from registers; 1 = one staged bf16 output (VT_EPI_BF16, VT_EPI_GELU_H);
-// 2 = two staged bf16 tiles (VT_EPI_GELU: z and h; VT_EPI_DGELU: dz and the TMA-loaded z).
+// 2 = two staged bf16 tiles (VT_EPI_GELU: z and h; VT_EPI_DGELU: dz and the TMA-loaded z); 3 = staged fp32 rows
+// (VT_EPI_F32, BN = 128 / 192: residual rows loaded and result rows stored by 1-D bulk copies, see epi_f32_io).
 constexpr int EPI_BOX_BYTES = 64 * 64 * 2;   // one 64-row x 64-column bf16 box, 128B-swizzled as TMA reads / writes it
+constexpr int SE_F32 = 3;
 
 template <int BN, int SE>
 struct GemmCfg {
@@ -57,9 +62,13 @@ struct GemmCfg {
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int EPI_TILE_BYTES = BM * BN * 2;    // one staged 128 x BN bf16 tile (both consumer halves)
-  static constexpr int EPI_BYTES = SE * EPI_TILE_BYTES;
+  // fp32 staging rows are padded by 32 bytes: the 8-byte accumulator pairs of a half-warp (4 rows x 32 contiguous bytes)
+  // then fall in 4 different bank octets.  Unpadded, all 4 rows hit the same 8 banks.
+  static constexpr int F32_PITCH = BN + 8;              // floats per staged fp32 row
+  static constexpr int EPI_BYTES = SE == SE_F32 ? BM * F32_PITCH * 4 : SE * EPI_TILE_BYTES;
   static constexpr int SMEM_LIMIT = 232448, SMEM_EXTRA = 1024 /*align slack*/ + 256 /*barriers*/;
-  // the ring gives up stages to the staging tiles: 6 / 5 / 4 stages at BN = 128 / 192 / 256 without staging
+  // the ring gives up stages to the staging tiles: 6 / 5 / 4 stages at BN = 128 / 192 / 256 without staging, 4 / 3 at
+  // BN = 128 / 192 with the fp32 staging tile
   static constexpr int STAGES_FIT = (SMEM_LIMIT - SMEM_EXTRA - EPI_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = STAGES_FIT < 6 ? STAGES_FIT : 6;
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + EPI_BYTES + SMEM_EXTRA;
@@ -222,6 +231,84 @@ __device__ __forceinline__ Tile tile_at(const GemmDev& p, int t) {
   return c;
 }
 
+// Row mover of the staged fp32 epilogue: one warp of the producer warpgroup per consumer half; lane l owns rows l and
+// l + 32 of the half's 64 x F32_PITCH staging tile `stage`, and the same lane loads and stores them, so its own bulk-group
+// wait is what keeps a row from being refilled before its store has read it.  Per tile, under the tile's MMAs: each row
+// with an addend is loaded (min(BN, N - n0) floats, one 1-D bulk copy, completing on `full`), a stored row without one is
+// zero-filled; then, once the consumer half has written its results in place (`ready`), every row that has an output is
+// stored through the same row mapping as the register epilogue (epi_row: plain rows, split-K partials, index arrays, the
+// affine maps and their side rows).  Rows >= M, dropped rows and columns >= N are never written.
+template <int BN>
+__device__ __forceinline__ void epi_f32_io(const GemmDev& p, float* stage, uint64_t* full, uint64_t* ready, int half, int lane) {
+  constexpr int PITCH = GemmCfg<BN, SE_F32>::F32_PITCH;
+  uint32_t tj = 0;
+  for (int t = blockIdx.x; t < p.tiles; t += gridDim.x, ++tj) {
+    const Tile c = tile_at<BN>(p, t);
+    const int cols = p.N - c.n0 < BN ? p.N - c.n0 : BN;
+    const uint32_t bytes = (uint32_t)cols * 4;
+    const int row0 = c.m0 + half * 64 + lane;
+    const EpiRow e0 = epi_row(p, row0, c.split), e1 = epi_row(p, row0 + 32, c.split);
+    float* s0 = stage + lane * PITCH;
+    float* s1 = s0 + 32 * PITCH;
+    tma_store_wait_read_all();        // this lane's stores of the previous tile have read its rows
+    uint32_t tx = 0;
+    if (p.aux) {
+      if (e0.out && e0.aux) tx += bytes;
+      if (e1.out && e1.aux) tx += bytes;
+      for (int h = 0; h < 2; ++h) {
+        const EpiRow& e = h ? e1 : e0;
+        if (e.out && !e.aux)
+          for (int i = 0; i < cols; i += 4) st_shared_zero16(smem_u32((h ? s1 : s0) + i));
+      }
+    }
+    mbar_arrive_expect_tx(full, tx);  // also tells the consumers the rows are free when nothing is loaded
+    if (tx) {
+      if (e0.out && e0.aux) bulk_load_1d(s0, reinterpret_cast<const float*>(e0.aux) + c.n0, bytes, full);
+      if (e1.out && e1.aux) bulk_load_1d(s1, reinterpret_cast<const float*>(e1.aux) + c.n0, bytes, full);
+    }
+    mbar_wait(ready, tj & 1);
+    if (e0.out) bulk_store_1d(reinterpret_cast<float*>(e0.out) + c.n0, s0, bytes);
+    if (e1.out) bulk_store_1d(reinterpret_cast<float*>(e1.out) + c.n0, s1, bytes);
+    tma_store_commit();
+  }
+  tma_store_wait_read_all();          // shared memory stays valid until the last store has read it
+}
+
+// Consumer side of the staged fp32 epilogue: rows r, r + 8 of the half (r = 16 warp + lane / 4), column pairs
+// 8j + 2 (lane % 4).  The arithmetic and its order are epi_pair's: v + bias, then fmaf(s, v, addend + bias2), with an
+// addend of zero where the row has none (zero-filled, or no aux at all).
+template <int BN>
+__device__ __forceinline__ void epi_f32_stage(const GemmDev& p, const float (&acc)[BN / 2], const float* stage, int row0, int n0,
+                                              int warp, int lane) {
+  constexpr int PITCH = GemmCfg<BN, SE_F32>::F32_PITCH;
+  const int r = warp * 16 + (lane >> 2);
+  float s[2] = {1.0f, 1.0f};
+  if (p.row_scale) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      if (row0 + r + 8 * h < p.M) s[h] = p.row_scale[row0 + r + 8 * h];
+  }
+  const uint32_t a0 = smem_u32(stage + r * PITCH + 2 * (lane & 3));
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int n = n0 + 8 * j + 2 * (lane & 3);
+    if (n >= p.N) break;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t o = a0 + (h * 8 * PITCH + 8 * j) * 4;
+      float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+      add_bias(p, n, v0, v1);
+      float2 a = make_float2(0.f, 0.f);
+      if (p.aux) a = ld_shared_f32x2(o);
+      if (p.bias2) {
+        const float2 b2 = __ldg(reinterpret_cast<const float2*>(p.bias2 + n));
+        a.x += b2.x; a.y += b2.y;
+      }
+      st_shared_f32x2(o, fmaf(s[h], v0, a.x), fmaf(s[h], v1, a.y));
+    }
+  }
+}
+
 // min(tiles, SMs) CTAs; CTA b runs tiles b, b + gridDim.x, ...  The producer thread streams every tile's k-blocks
 // through one shared-memory ring whose stage / phase count runs on across tiles, so barrier set-up, register hand-over and
 // the tensor-map prefetch happen once per CTA and the ring refills during each epilogue.  The walk is static: a tile's
@@ -240,7 +327,8 @@ template <int BN, int TA, int TB, int SE, int F8>
 __device__ __forceinline__ void gemm_wgmma_body(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC,
                                                 const CUtensorMap& tmD, const GemmDev& p) {
   using Cfg = GemmCfg<BN, SE>;
-  static_assert(!F8 || (BN == 128 && !TA && !TB && SE < 2), "e4m3 forms: BN = 128, K-major operands, one output");
+  static_assert(!F8 || (BN == 128 && !TA && !TB && SE != 2), "e4m3 forms: BN = 128, K-major operands, one output");
+  static_assert(SE != SE_F32 || BN != 256, "the fp32 staging tile leaves too few ring stages at BN = 256");
   constexpr int STAGES = Cfg::STAGES;
   constexpr int KB_ELEMS = F8 ? 128 : BK;      // elements of one k-block (128 bytes per row either way)
   constexpr int HALF_BYTES = Cfg::EPI_TILE_BYTES / 2;   // one consumer warpgroup's 64 x BN part of a staged tile
@@ -251,13 +339,15 @@ __device__ __forceinline__ void gemm_wgmma_body(const CUtensorMap& tmA, const CU
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* zfull_bar = empty_bar + STAGES;
   uint64_t* zempty_bar = zfull_bar + 1;
+  uint64_t* rows_full_bar = zempty_bar + 1;    // SE_F32, per consumer half: residual rows loaded / staging rows free
+  uint64_t* rows_ready_bar = rows_full_bar + 2;   // SE_F32, per consumer half: results written, rows may be stored
   const bool load_z = SE == 2 && p.epi == VT_EPI_DGELU;
 
   const int wg = threadIdx.x >> 7;
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    if (SE > 0) tma_prefetch_desc(&tmC);
+    if (SE == 1 || SE == 2) tma_prefetch_desc(&tmC);
     if (SE == 2) tma_prefetch_desc(&tmD);
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
@@ -265,12 +355,23 @@ __device__ __forceinline__ void gemm_wgmma_body(const CUtensorMap& tmA, const CU
     }
     mbar_init(zfull_bar, 1);
     mbar_init(zempty_bar, 2);        // one arrive per consumer warpgroup
+    for (int h = 0; h < 2; ++h) {
+      mbar_init(&rows_full_bar[h], 32);    // one arrive per lane of the row-moving warp
+      mbar_init(&rows_ready_bar[h], 128);  // one arrive per consumer thread
+    }
     fence_barrier_init();
   }
   __syncthreads();
 
   if (wg == 0) {
     setmaxnreg_dec<40>();
+    const int pw = threadIdx.x >> 5;
+    if constexpr (SE == SE_F32) {   // warps 1 and 2 move the fp32 rows of consumer halves 0 and 1
+      if (pw == 1 || pw == 2) {
+        float* rows = reinterpret_cast<float*>(epi_smem) + (pw - 1) * 64 * Cfg::F32_PITCH;
+        epi_f32_io<BN>(p, rows, &rows_full_bar[pw - 1], &rows_ready_bar[pw - 1], pw - 1, threadIdx.x & 31);
+      }
+    }
     if (threadIdx.x == 0) {
       uint32_t it = 0;   // ring position: k-blocks loaded so far by this CTA
       uint32_t tj = 0;   // tiles of this CTA so far
@@ -378,7 +479,13 @@ __device__ __forceinline__ void gemm_wgmma_body(const CUtensorMap& tmA, const CU
     if (lane == 0) mbar_arrive(&empty_bar[prev]);   // the producer is already filling the ring for the next tile
     }
 
-    if constexpr (SE > 0) {
+    if constexpr (SE == SE_F32) {
+      const float* rows = reinterpret_cast<const float*>(epi_smem) + cw * 64 * Cfg::F32_PITCH;
+      mbar_wait(&rows_full_bar[cw], tj & 1);
+      epi_f32_stage<BN>(p, acc, rows, c.m0 + cw * 64, c.n0, warp, lane);
+      fence_proxy_async_smem();
+      mbar_arrive(&rows_ready_bar[cw]);
+    } else if constexpr (SE > 0) {
       const int row0 = c.m0 + cw * 64;
       if (load_z) mbar_wait(zfull_bar, tj & 1);
       if (leader) tma_store_wait_read_all();       // the previous tile's store has read the staging boxes
@@ -413,7 +520,7 @@ __device__ __forceinline__ void gemm_wgmma_body(const CUtensorMap& tmA, const CU
       }
     }
   }
-  if (SE > 0 && leader) tma_store_wait_read_all();   // shared memory stays valid until the last store has read it
+  if ((SE == 1 || SE == 2) && leader) tma_store_wait_read_all();   // shared memory stays valid until the last store has read it
 }
 
 template <int BN, int TA, int TB, int SE>
@@ -423,7 +530,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   gemm_wgmma_body<BN, TA, TB, SE, 0>(tmA, tmB, tmC, tmD, p);
 }
 
-// vt_gemm_e4m3: 128-wide tiles, K-major e4m3 operands, SE = 0 or 1
+// VT_EPI_F32 with the staged rows (SE_F32), BN = 128 or 192
+template <int BN, int TA, int TB>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_f32_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmD, const GemmDev p) {
+  gemm_wgmma_body<BN, TA, TB, SE_F32, 0>(tmA, tmB, tmC, tmD, p);
+}
+
+// vt_gemm_e4m3: 128-wide tiles, K-major e4m3 operands, SE = 0, 1 or SE_F32
 template <int SE>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_e4m3_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -554,6 +669,7 @@ static int launch_gemm_t(const CUtensorMap (&tm)[4], const GemmDev& d, cudaStrea
   using Cfg = GemmCfg<BN, SE>;
   void (*kernel)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const CUtensorMap, const GemmDev);
   if constexpr (F8) kernel = gemm_e4m3_kernel<SE>;
+  else if constexpr (SE == SE_F32) kernel = gemm_f32_kernel<BN, TA, TB>;
   else kernel = gemm_wgmma_kernel<BN, TA, TB, SE>;
   static bool attr_set = false;  // benign race: idempotent
   if (!attr_set) {
@@ -563,7 +679,7 @@ static int launch_gemm_t(const CUtensorMap (&tm)[4], const GemmDev& d, cudaStrea
   }
   const int grid = d.tiles < persistent_sm_count() ? d.tiles : persistent_sm_count();
   kernel<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(tm[0], tm[1], tm[2], tm[3], d);
-  return check_launch(F8 ? "gemm_e4m3_kernel" : "gemm_wgmma_kernel");
+  return check_launch(F8 ? "gemm_e4m3_kernel" : SE == SE_F32 ? "gemm_f32_kernel" : "gemm_wgmma_kernel");
 }
 
 template <int BN, int SE>
@@ -578,10 +694,21 @@ static int launch_layout(const vt_gemm_params* q, const CUtensorMap (&tm)[4], co
 #define VT_DEFAULT_STAGED_EPI true
 #endif
 // Staged epilogue kind for this call (see GemmCfg): the bf16-output forms on plain rows, whose outputs (and DGELU's z)
-// TMA can address as [M, N] tensors.  VT_GEMM_STAGED_EPI=0 keeps every form on the register epilogue.
+// TMA can address as [M, N] tensors, and the fp32 forms with any row mapping, whose rows move as 1-D bulk copies of
+// 16-byte aligned segments.  gemm_dispatch checks out / aux and their pitches for that; the affine map only has to be
+// even there, so a map with an offset or stride that is not a multiple of 4 elements stays on the register epilogue,
+// as do BN = 256 and split-K partials at BN = 192 (launch_gemm).  VT_GEMM_STAGED_EPI=0 keeps every form on the register
+// epilogue.
 static int staged_kind(const vt_gemm_params* q) {
-  if (q->epilogue == VT_EPI_F32 || q->out_row) return 0;
   if (!feature_on("VT_GEMM_STAGED_EPI", VT_DEFAULT_STAGED_EPI)) return 0;
+  if (q->epilogue == VT_EPI_F32) {
+    if (q->map_period > 0 &&
+        (q->map_base % 4 || q->map_stride_t % 4 || q->map_stride_p % 4 || q->map_stride_b % 4 ||
+         (q->map_special_base >= 0 && (q->map_special_base % 4 || q->map_special_stride % 4))))
+      return 0;
+    return SE_F32;
+  }
+  if (q->out_row) return 0;
   if (q->epilogue == VT_EPI_BF16 || q->epilogue == VT_EPI_GELU_H) return 1;
   // GELU's out2 is not checked by the register path's alignment rule; TMA needs it 16-byte aligned
   if (q->epilogue == VT_EPI_GELU && ((reinterpret_cast<uintptr_t>(q->out2) & 15) || (q->ldo2 * 2) % 16)) return 0;
@@ -618,19 +745,29 @@ static int launch_gemm(const vt_gemm_params* q, GemmDev& d, cudaStream_t st) {
     d.ldo = q->N;
     d.split_stride = tile_out;
   }
-  const int se = d.splits > 1 ? 0 : staged_kind(q);
-  if (se > 0) {
+  // split-K partials take the staged rows at BN = 128 only: at 192 the 3 ring stages left cost more over the ~200
+  // k-blocks of a weight gradient than the epilogue saves
+  int se = staged_kind(q);
+  if (se == SE_F32 && (BN == 256 || (d.splits > 1 && (BN != 128 || (reinterpret_cast<uintptr_t>(q->workspace) & 15))))) se = 0;
+  if (se == 1 || se == 2) {
     rc = make_tmap_bf16_2d(&tm[2], q->out, q->M, q->N, q->ldo, 64);
     if (!rc && q->epilogue == VT_EPI_GELU) rc = make_tmap_bf16_2d(&tm[3], q->out2, q->M, q->N, q->ldo2, 64);
     if (!rc && q->epilogue == VT_EPI_DGELU) rc = make_tmap_bf16_2d(&tm[3], q->aux, q->M, q->N, q->ldaux, 64);
     if (rc) return rc;
   }
   if constexpr (F8) {
-    rc = se == 1 ? launch_gemm_t<BN, 0, 0, 1, 1>(tm, d, st) : launch_gemm_t<BN, 0, 0, 0, 1>(tm, d, st);
+    if (se == 1) rc = launch_gemm_t<BN, 0, 0, 1, 1>(tm, d, st);
+    else if (se == SE_F32) rc = launch_gemm_t<BN, 0, 0, SE_F32, 1>(tm, d, st);
+    else rc = launch_gemm_t<BN, 0, 0, 0, 1>(tm, d, st);
   } else {
     if (se == 1) rc = launch_layout<BN, 1>(q, tm, d, st);
     else if (se == 2) rc = launch_layout<BN, 2>(q, tm, d, st);
-    else rc = launch_layout<BN, 0>(q, tm, d, st);
+    else if constexpr (BN != 256) {
+      if (se == SE_F32) rc = launch_layout<BN, SE_F32>(q, tm, d, st);
+      else rc = launch_layout<BN, 0>(q, tm, d, st);
+    } else {
+      rc = launch_layout<BN, 0>(q, tm, d, st);
+    }
   }
   if (rc) return rc;
   if (d.splits > 1) {
@@ -754,7 +891,8 @@ static int gemm_dispatch(const vt_gemm_params* q, const float* a_scale, const fl
   // the model undervalues: measured on an H100 at B = 8 it is 20-35 % faster than the 256-wide tile on the wide-output
   // ones with the register epilogue, and the staged GELU / dGELU forms lose ring stages to their two staging tiles at
   // wider tiles.  The one-output staged form may also take the 192-wide tile (4 stages), which the model picks for qkv
-  // (81 vs 92 us) and the projection's data gradient (29 vs 33 us).
+  // (81 vs 92 us) and the projection's data gradient (29 vs 33 us); so may the staged fp32 form (3 stages), which the model
+  // picks for the projections' forward with the residual add (56 vs 63 us, H100 at 700 W).
   if (f8) {   // two accumulator tiles per thread fit the register budget at BN = 128 only; no split-K
     d.splits = 1;
     return launch_gemm<128, 1>(q, d, static_cast<cudaStream_t>(stream));
@@ -765,13 +903,17 @@ static int gemm_dispatch(const vt_gemm_params* q, const float* a_scale, const fl
   const int num_m = (q->M + BM - 1) / BM;
   const bool can_split = q->epilogue == VT_EPI_F32 && q->workspace && !q->out_row && !q->aux && !q->row_scale && !q->bias &&
                          q->map_period == 0;
+  // the staged fp32 rows exist at BN = 128 / 192 only; split-K calls keep the plan they had (a different split count
+  // would change the sums) and take the register epilogue where it is 192 or 256 wide (launch_gemm)
+  const bool f32_staged = staged_kind(q) == SE_F32 && !can_split;
   const int cand[3] = {256, 192, 128};
   const double penalty[3] = {1.0, 1.04, 1.10};
   double best = 1e30;
   int bn = 128, splits = 1;
   for (int i = 0; i < 3; ++i) {
     if (q->force_bn && cand[i] != q->force_bn) continue;
-    if (!q->force_bn && !can_split && short_k && cand[i] != 128 && !(one_staged && cand[i] == 192)) continue;
+    if (!q->force_bn && !can_split && short_k && cand[i] != 128 && !((one_staged || f32_staged) && cand[i] == 192)) continue;
+    if (!q->force_bn && f32_staged && cand[i] == 256) continue;
     const int num_n = (q->N + cand[i] - 1) / cand[i];
     const int smax = can_split ? 16 : 1;
     for (int sp = 1; sp <= smax; ++sp) {
