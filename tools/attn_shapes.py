@@ -1,7 +1,7 @@
 """Time every distinct attention-core call of the benched workloads stand-alone on the GPU.
 
     python tools/attn_shapes.py [--reps 30] [--warmup 5] [--rounds 3] [--workloads timesformer,vivit,mvit,maskfeat]
-                                [--baseline-lib PATH] [--profile] [--json OUT]
+                                [--baseline-lib PATH] [--tiled] [--profile] [--json OUT]
 
 The shapes are recorded, not listed: one eager fwd + bwd step of each workload (bench.py's models and batches) runs with
 K.attn_fwd / attn_bwd / xattn_fwd / xattn_bwd wrapped, and the first call of each distinct shape keeps its real operands
@@ -13,8 +13,12 @@ Per row: microseconds, the bytes the call must move at least once and its algori
 --baseline-lib PATH loads a second libvt_b200.so (another build of the same C ABI) and alternates the two libraries row by
 row, `--rounds` times each, in this one process: the columns give the median of each and its spread (max - min).
 
---profile instead runs every backward shape a few times under torch.profiler and prints the time of each kernel the
-backward launches (the dQ and dK/dV kernels of the tensor-core path); run it on its own, the profiler slows the host.
+--tiled adds this library once more with VT_ATTN_WHOLE=0 (the 64-row tiled tensor-core kernels instead of the
+whole-problem ones on the packed-qkv path), alternated with the others in the same way.
+
+--profile instead runs every forward and backward shape a few times under torch.profiler and prints the time of each
+kernel it launches (the whole-problem kernels, or with --tiled also the tiled forward, dQ and dK/dV kernels); run it on its
+own, the profiler slows the host.
 
 The card's name, power limit and SM clocks are read with read-only nvidia-smi queries and printed with the numbers.
 Needs a CUDA device; there is no CPU path.
@@ -38,8 +42,16 @@ WRAPPED = ('attn_fwd', 'attn_bwd', 'xattn_fwd', 'xattn_bwd')
 
 
 def packed_kernel(N):
-    """which vt_attn_* kernel the automatic choice takes (vt_attention.cu pick_impl)"""
-    return 'warp8' if N == 8 else 'mma' if 32 < N <= 256 else 'generic'
+    """which vt_attn_* kernel the automatic choice takes (vt_attention.cu pick_impl, use_whole)"""
+    return 'warp8' if N == 8 else 'whole' if 32 < N <= 256 else 'generic'
+
+
+def set_whole(env):
+    """VT_ATTN_WHOLE for the following calls (read by the library at every call); None: the library's default"""
+    if env is None:
+        os.environ.pop('VT_ATTN_WHOLE', None)
+    else:
+        os.environ['VT_ATTN_WHOLE'] = env
 
 
 def record(workloads, dev):
@@ -122,30 +134,32 @@ def open_lib(path):
 
 
 def timings(rows, args, libs):
-    """{(row index, side, lib name): [us per round]}, libraries alternated inside each round"""
+    """{(row index, side, lib name): [us per round]}, libraries (and VT_ATTN_WHOLE settings) alternated inside each round"""
     from videotransformer_pytorch_b200 import _lib
     res = {}
     own = _lib._dll
     try:
         for i, row in enumerate(rows):
             for _ in range(args.rounds):
-                for lname, lib in libs:
+                for lname, lib, env in libs:
                     _lib._dll = lib
+                    set_whole(env)
                     for side in ('fwd', 'bwd'):
                         us = 1e3 * events_ms(lambda: call(row, side), args.reps, args.warmup)
                         res.setdefault((i, side, lname), []).append(us)
     finally:
         _lib._dll = own
+        set_whole(None)
     return res
 
 
 def report(rows, res, libs, out):
-    names = [n for n, _ in libs]
+    names = [n for n, _, _ in libs]
     hdr = f'{"shape":28s} {"kernel":7s} {"pass":4s} {"MB":>7s} {"GFLOP":>7s} {"floor us":>8s}'
     for n in names:
         hdr += f' {"us " + n:>10s} {"+-":>6s} {"x floor":>7s}'
-    if len(names) == 2:
-        hdr += f' {names[1] + "/" + names[0]:>10s}'
+    for n in names[1:]:
+        hdr += f' {n + "/" + names[0]:>10s}'
     print(hdr)
     for i, row in enumerate(rows):
         label, kern, fwd, bwd = describe(row)
@@ -159,34 +173,41 @@ def report(rows, res, libs, out):
                 med = statistics.median(ts)
                 r[n] = dict(us=med, spread=max(ts) - min(ts), over_floor=med / floor, rounds=ts)
                 line += f' {med:10.1f} {max(ts) - min(ts):6.1f} {med / floor:7.2f}'
-            if len(names) == 2:
-                r['ratio'] = r[names[1]]['us'] / r[names[0]]['us']
-                line += f' {r["ratio"]:10.3f}'
+            for n in names[1:]:
+                r['ratio_' + n] = r[n]['us'] / r[names[0]]['us']
+                line += f' {r["ratio_" + n]:10.3f}'
             out.append(r)
             print(line + f'   [{",".join(row["workloads"])}]')
 
 
-def profile(rows, args):
-    """per-kernel split of every backward shape, from torch.profiler (CUDA activity)"""
+def profile(rows, args, envs):
+    """per-kernel split of every forward and backward shape, from torch.profiler (CUDA activity), for each
+    VT_ATTN_WHOLE setting in `envs`"""
     from torch.profiler import ProfilerActivity
     from torch.profiler import profile as prof
     out = []
-    for row in rows:
-        label = describe(row)[0]
-        for _ in range(args.warmup):
-            call(row, 'bwd')
-        torch.cuda.synchronize()
-        with prof(activities=[ProfilerActivity.CUDA]) as p:
-            for _ in range(args.reps):
-                call(row, 'bwd')
-            torch.cuda.synchronize()
-        per = {}
-        for ev in p.events():
-            if ev.device_type == torch.autograd.DeviceType.CUDA:
-                per[ev.name] = per.get(ev.name, 0.0) + ev.device_time / args.reps
-        for name, us in sorted(per.items(), key=lambda kv: -kv[1]):
-            out.append(dict(shape=label, kernel=name, us=us))
-            print(f'{label:28s} {us:9.1f} us  {name[:110]}')
+    try:
+        for row in rows:
+            label = describe(row)[0]
+            for env in envs:
+                set_whole(env)
+                for side in ('fwd', 'bwd'):
+                    for _ in range(args.warmup):
+                        call(row, side)
+                    torch.cuda.synchronize()
+                    with prof(activities=[ProfilerActivity.CUDA]) as p:
+                        for _ in range(args.reps):
+                            call(row, side)
+                        torch.cuda.synchronize()
+                    per = {}
+                    for ev in p.events():
+                        if ev.device_type == torch.autograd.DeviceType.CUDA:
+                            per[ev.name] = per.get(ev.name, 0.0) + ev.device_time / args.reps
+                    for name, us in sorted(per.items(), key=lambda kv: -kv[1]):
+                        out.append(dict(shape=label, side=side, whole=env, kernel=name, us=us))
+                        print(f'{label:28s} {side} {us:9.1f} us  {name[:110]}')
+    finally:
+        set_whole(None)
     return out
 
 
@@ -197,7 +218,8 @@ def main():
     ap.add_argument('--rounds', type=int, default=3, help='timings per row and library, alternating')
     ap.add_argument('--workloads', default='timesformer,vivit,mvit,maskfeat')
     ap.add_argument('--baseline-lib', default=None, help='a second libvt_b200.so, timed against this tree\'s')
-    ap.add_argument('--profile', action='store_true', help='only the torch.profiler split of the backward kernels')
+    ap.add_argument('--tiled', action='store_true', help='also time / profile this library with VT_ATTN_WHOLE=0')
+    ap.add_argument('--profile', action='store_true', help='only the torch.profiler split of the attention kernels')
     ap.add_argument('--json', default=None, help='also write the rows as JSON to this file')
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -207,13 +229,15 @@ def main():
     info = card()
     print(json.dumps({'card': info}))
     lib = _lib.load_library()
-    libs = [('this', lib)]
+    libs = [('this', lib, '1' if args.tiled else None)]
+    if args.tiled:
+        libs.append(('tiled', lib, '0'))
     if args.baseline_lib:
-        libs.append(('base', open_lib(args.baseline_lib)))
+        libs.append(('base', open_lib(args.baseline_lib), None))
     rows = record([w for w in args.workloads.split(',') if w], dev)
     print(f'{len(rows)} distinct attention shapes')
     if args.profile:
-        out = profile(rows, args)
+        out = profile(rows, args, ['1', '0'] if args.tiled else [None])
     else:
         out = []
         report(rows, timings(rows, args, libs), libs, out)

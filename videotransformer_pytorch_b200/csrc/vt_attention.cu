@@ -248,6 +248,9 @@ static MmaAttn packed_operands(const void* qkv, const void* ctx, const float* ls
   return a;
 }
 
+// the tensor-core kernels that own a whole problem per CTA where they cover N; VT_ATTN_WHOLE=0 keeps the 64-row tiles
+static bool use_whole(const MmaAttn& a) { return feature_on("VT_ATTN_WHOLE", true) && attn_whole_ok(a, HD); }
+
 }  // namespace vt
 
 using namespace vt;
@@ -263,6 +266,7 @@ extern "C" int vt_attn_fwd(const vt_attn_fwd_params* p, void* stream) {
     VT_REQUIRE((((uintptr_t)p->qkv | (uintptr_t)p->ctx) & 15) == 0, "vt_attn_fwd: qkv / ctx must be 16-byte aligned");
     MmaAttn a = packed_operands(p->qkv, p->ctx, p->lse, p->Bp, p->N, p->H, p->scale);
     a.o_out = static_cast<__nv_bfloat16*>(p->ctx);
+    if (use_whole(a)) return attn_whole_fwd(a, p->Bp, static_cast<cudaStream_t>(stream));
     return attn_mma_fwd(a, p->Bp, HD, static_cast<cudaStream_t>(stream));
   }
   if (impl == VT_ATTN_WARP8) {
@@ -298,6 +302,7 @@ extern "C" int vt_attn_bwd(const vt_attn_bwd_params* p, void* stream) {
     a.dq_bs = a.dk_bs = a.dv_bs = a.q_bs;
     a.dq_hs = a.dk_hs = a.dv_hs = HD;
     a.dq_rs = a.dk_rs = a.dv_rs = a.q_rs;
+    if (use_whole(a)) return attn_whole_bwd(a, p->Bp, static_cast<cudaStream_t>(stream));
     return attn_mma_bwd(a, p->Bp, HD, static_cast<cudaStream_t>(stream));
   }
   if (impl == VT_ATTN_WARP8) {

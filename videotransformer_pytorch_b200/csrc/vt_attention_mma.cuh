@@ -32,5 +32,10 @@ struct MmaAttn {
 bool mma_layout_ok(const void* ptr, long long bs, long long hs, long long rs, int hd);
 int attn_mma_fwd(const MmaAttn& a, int B, int hd, cudaStream_t st);
 int attn_mma_bwd(const MmaAttn& a, int B, int hd, cudaStream_t st);
+// One CTA per (b, h) problem with its operands resident in shared memory: Nq == Nk <= 256 at head dim 64, bf16 dK / dV
+// and no delta output.  Same bits as attn_mma_fwd / attn_mma_bwd.
+bool attn_whole_ok(const MmaAttn& a, int hd);
+int attn_whole_fwd(const MmaAttn& a, int B, cudaStream_t st);
+int attn_whole_bwd(const MmaAttn& a, int B, cudaStream_t st);
 
 }  // namespace vt
