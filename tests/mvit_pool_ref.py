@@ -7,8 +7,8 @@ bound covers only the arithmetic of one stage.  With u = 2^-24 and gamma_n = n u
 is within gamma_n of the sum of the absolute values of its terms, in any order of summation:
 
   pooled   gamma_n sum|w x| over the n <= 27 taps in range; the cls row is an exact copy
-  mean     gamma_97 mean|pooled|: 95 additions, the rounded 1/96 and the product
-  rstd     gamma_101 on mean((x - mean_k)^2) + eps (squares, sum, scale, eps), the kernel's own mean error delta entering as
+  mean     gamma_97 mean|pooled|: 95 additions, the rounded 1/96 and the product (gamma_{D+1} at width D)
+  rstd     gamma_101 (gamma_{D+5}) on mean((x - mean_k)^2) + eps (squares, sum, scale, eps), the kernel's own mean error delta entering as
            (1 + delta^2 / (var + eps)), and the 2 ulp of rsqrtf
   out      gamma_4 |xhat gamma| + u |beta|, then half a bf16 ulp
   dpooled  first-order LayerNorm backward with absolute sums (see ln_backward_bound)
@@ -178,7 +178,9 @@ def pool_forward(xh, w, thw, stride, gam=None, bet=None):
 
 
 def ln_plan(rows, sm_count):
-    """(CTAs, rows per warp) of ln_small_bwd_kernel over `rows` rows (vt_ln_bwd_blocks)"""
+    """(CTAs, rows per warp) of every LayerNorm kernel over `rows` rows: 8 warps per CTA, one row per warp and step, at
+    most 4 CTAs per SM (vt_ln_bwd_blocks; ln_blocks of the D % 128 == 0 kernels, row_blocks(rows, 4) of the narrow
+    forward)"""
     blocks = max(1, min((rows + ROW_WARPS - 1) // ROW_WARPS, 4 * sm_count))
     return blocks, -(-rows // (ROW_WARPS * blocks))
 
@@ -227,21 +229,31 @@ def check_forward(xh, w, gam, bet, thw, stride, got, report):
     absum = torch.cat([torch.zeros_like(xh[:, :, :1]), conv(xh[:, :, 1:].abs(), w.abs(), thw, stride)], 2)
     taps = torch.cat([torch.zeros(1, dtype=torch.float64), taps_in_range(thw, stride)])
     check('pooled', got['pooled'], pooled_ref, gamma(taps)[:, None] * absum, report)
-    p = got['pooled'].double()
-    mu, rs = got['mean'].double(), got['rstd'].double()
+    check_ln_forward(got['pooled'].double(), got['mean'], got['rstd'], gam, bet, EPS, got['out'], report)
+
+
+def check_ln_forward(p, mu, rs, gam, bet, eps, out, report, names=('mean', 'rstd', 'out')):
+    """LayerNorm forward over the last dim (any width D) of the fp32 rows p (fp64 tensor [..., D]): the kernel's mean and
+    rstd against fp64, and its output (bf16, or fp32) against fp64 computed from the kernel's own mean and rstd.  The
+    kernels sum D terms, scale by the rounded 1/D (mean: gamma_{D+1}), and for rstd square D rounded differences, sum, scale
+    and add eps (gamma_{D+5}); out is (x - mean) * rstd * gamma + beta (gamma_4, u |beta|)."""
+    D = p.shape[-1]
+    mu, rs = mu.double(), rs.double()
     mean = p.mean(-1)
-    check('mean', mu, mean, gamma(HD + 1) * p.abs().mean(-1), report)
+    check(names[0], mu, mean, gamma(D + 1) * p.abs().mean(-1), report)
     var = (p - mean[..., None]).square().mean(-1)
-    a = var + EPS32
+    a = var + float(torch.tensor(eps, dtype=torch.float32))
     q = 1 + (mu - mean).square() / a
-    g = gamma(HD + 5)
+    g = gamma(D + 5)
     rstd = a.rsqrt()
     rel = torch.maximum((q * (1 - g)).rsqrt() * (1 + RSQRT_REL) - 1, 1 - (q * (1 + g)).rsqrt() * (1 - RSQRT_REL))
-    check('rstd', rs, rstd, rstd * rel, report)
+    check(names[1], rs, rstd, rstd * rel, report)
     xg = (p - mu[..., None]) * rs[..., None] * gam.double()
-    out = xg + bet.double()
+    ref = xg + bet.double()
     e32 = gamma(4) * xg.abs() + U * bet.double().abs()
-    check('out', got['out'], out, e32 + half_ulp_bf16(out.abs() + e32), report)
+    if out.dtype == torch.bfloat16:
+        e32 = e32 + half_ulp_bf16(ref.abs() + e32)
+    check(names[2], out, ref, e32, report)
 
 
 def ln_backward(p, mu, rs, gam, dout):
@@ -254,10 +266,11 @@ def ln_backward(p, mu, rs, gam, dout):
 
 
 def ln_backward_bound(rs, xhat, gy, m1, m2):
-    """first order: gy rounded (u), m1 from 96 rounded terms (gamma_98), m2 from terms with xhat's two roundings
-    (gamma_101), xhat itself (gamma_2), the product and two subtractions and the final scaling (gamma_4)"""
-    return rs[..., None] * (U * gy.abs() + gamma(HD + 2) * gy.abs().mean(-1, keepdim=True)
-                            + gamma(HD + 5) * xhat.abs() * (gy * xhat).abs().mean(-1, keepdim=True)
+    """first order, rows of width D: gy rounded (u), m1 from D rounded terms (gamma_{D+2}), m2 from terms with xhat's two
+    roundings (gamma_{D+5}), xhat itself (gamma_2), the product and two subtractions and the final scaling (gamma_4)"""
+    D = gy.shape[-1]
+    return rs[..., None] * (U * gy.abs() + gamma(D + 2) * gy.abs().mean(-1, keepdim=True)
+                            + gamma(D + 5) * xhat.abs() * (gy * xhat).abs().mean(-1, keepdim=True)
                             + gamma(2) * m2.abs() * xhat.abs()
                             + gamma(4) * (gy.abs() + m1.abs() + (xhat * m2).abs())) * SECOND_ORDER
 
@@ -286,8 +299,15 @@ def check_backward(xh, w, gam, thw, stride, fwd, dout, got, gen, sm_count, repor
         check('dw', got['dw'], conv_wgrad(xh[:, :, 1:], dp[:, :, 1:], thw, stride),
               gamma(n) * conv_wgrad(xh[:, :, 1:].abs(), dp[:, :, 1:].abs(), thw, stride), report)
     if 'dgb' in parts:
-        blocks, per_warp = ln_plan(B * H * p.shape[2], sm_count)
-        n = per_warp + ROW_WARPS + blocks
-        dims = (0, 1, 2)
-        check('dgamma', got['dgamma'], (d * xhat).sum(dims), gamma(n + 2) * (d * xhat).abs().sum(dims), report)
-        check('dbeta', got['dbeta'], d.sum(dims), gamma(n) * d.abs().sum(dims), report)
+        check_dgamma_dbeta(d, xhat, got['dgamma'], got['dbeta'], sm_count, report)
+
+
+def check_dgamma_dbeta(d, xhat, dgamma, dbeta, sm_count, report):
+    """d, xhat fp64 [..., D] over every row the backward walked; a warp adds its rows' d * xhat and d per column, the 8
+    warps of a CTA are summed, then the CTAs' partial rows: n = rows per warp + 8 warps + CTAs (ln_plan), +2 for xhat's
+    own roundings"""
+    d, xhat = d.reshape(-1, d.shape[-1]), xhat.reshape(-1, d.shape[-1])
+    blocks, per_warp = ln_plan(d.shape[0], sm_count)
+    n = per_warp + ROW_WARPS + blocks
+    check('dgamma', dgamma, (d * xhat).sum(0), gamma(n + 2) * (d * xhat).abs().sum(0), report)
+    check('dbeta', dbeta, d.sum(0), gamma(n) * d.abs().sum(0), report)

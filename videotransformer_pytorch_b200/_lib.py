@@ -502,10 +502,17 @@ class CudaKernels:
     def ln_bwd(self, dy, x2d, mean, rstd, gamma, in_row=None, out_row=None, dres=None, dx=None, n_aux=0):
         """-> (dx [x2d.shape] or given, dx_aux [n_aux, D] or None, dgamma, dbeta)"""
         lib = load_library()
+        # the kernel reads dy with pitch D and dres with dx's pitch
+        if dy.dtype not in (torch.float32, torch.bfloat16):
+            raise RuntimeError(f'ln_bwd.dy: expected dtype torch.float32 or torch.bfloat16, got {dy.dtype}')
+        if not dy.is_cuda or dy.dim() != 2 or not dy.is_contiguous():
+            raise RuntimeError(f'ln_bwd.dy: expected a contiguous 2-D CUDA tensor, got shape {tuple(dy.shape)} stride {dy.stride()}')
         rows, D = dy.shape
         dev = dy.device
         if dx is None:
             dx = torch.empty((x2d.shape[0], D), dtype=torch.float32, device=dev)
+        if dres is not None and (dres.dim() != 2 or dres.stride() != dx.stride()):
+            raise RuntimeError(f'ln_bwd.dres: expected the row pitch of dx {dx.stride()}, got stride {dres.stride()}')
         dx_aux = torch.empty((n_aux, D), dtype=torch.float32, device=dev) if n_aux else None
         blocks = lib.vt_ln_bwd_blocks(rows)
         partials = torch.empty((blocks, 2, D), dtype=torch.float32, device=dev)

@@ -299,6 +299,9 @@ ln_bwd2_kernel(const void* __restrict__ dy, int dy_fp32, const float* __restrict
   }
 }
 
+// the entry points refuse pointers the kernels' 16-byte vector accesses cannot take (NULL passes: optional operands)
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
 static int ln_blocks(int rows) {
   int blocks = (rows + LN_WARPS - 1) / LN_WARPS;
   const int cap = sm_count() * 4;
@@ -755,6 +758,8 @@ extern "C" int vt_layernorm_fwd(const vt_ln_fwd_params* p, void* stream) {
   if (p->D % 128 != 0) return layernorm_fwd_small(p, stream);
   VT_REQUIRE(p->D % 128 == 0 && p->D >= 128 && p->D <= 1024, "vt_layernorm_fwd: D=%d unsupported (multiple of 128, <=1024)", p->D);
   VT_REQUIRE(p->ldx % 4 == 0, "vt_layernorm_fwd: ldx must be a multiple of 4");
+  VT_REQUIRE(aligned16(p->x) && aligned16(p->gamma) && aligned16(p->beta) && aligned16(p->y),
+             "vt_layernorm_fwd: x, gamma, beta and y must be 16-byte aligned (D=%d)", p->D);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int blocks = ln_blocks(p->rows);
 #define VT_LN_FWD(V)                                                                                                    \
@@ -776,6 +781,11 @@ extern "C" int vt_layernorm_bwd(const vt_ln_bwd_params* p, void* stream) {
   VT_REQUIRE(p->rows > 0, "vt_layernorm_bwd: rows=%d", p->rows);
   if (p->D % 128 != 0) return layernorm_bwd_small(p, stream);
   VT_REQUIRE(p->D % 128 == 0 && p->D >= 128 && p->D <= 1024, "vt_layernorm_bwd: D=%d unsupported", p->D);
+  VT_REQUIRE(p->ldx % 4 == 0 && p->lddx % 4 == 0, "vt_layernorm_bwd: ldx and lddx must be multiples of 4");
+  // dy is read as uint2 (bf16) or float4 (fp32) vectors, everything else as float4
+  VT_REQUIRE((reinterpret_cast<uintptr_t>(p->dy) & (p->dy_fp32 ? 15 : 7)) == 0 && aligned16(p->x) && aligned16(p->gamma) &&
+                 aligned16(p->dx) && aligned16(p->dres) && aligned16(p->dx_aux) && aligned16(p->partials),
+             "vt_layernorm_bwd: dy, x, gamma, dx, dres, dx_aux and partials must be 16-byte aligned (bf16 dy: 8-byte)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int blocks = ln_blocks(p->rows);
   const bool v2 = feature_on("VT_LN_BWD_V2", false);
@@ -799,6 +809,7 @@ extern "C" int vt_layernorm_bwd(const vt_ln_bwd_params* p, void* stream) {
 
 extern "C" int vt_cast_f32_bf16(const vt_cast_params* p, void* stream) {
   VT_REQUIRE(p && p->src && p->dst && p->n > 0, "vt_cast_f32_bf16: bad params");
+  VT_REQUIRE(p->n < 8 || (aligned16(p->src) && aligned16(p->dst)), "vt_cast_f32_bf16: src and dst must be 16-byte aligned");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long n8 = p->n / 8;
   if (n8 > 0) cast_kernel<<<grid_for(n8, 256), 256, 0, st>>>(p->src, static_cast<__nv_bfloat16*>(p->dst), n8);
@@ -809,6 +820,7 @@ extern "C" int vt_cast_f32_bf16(const vt_cast_params* p, void* stream) {
 extern "C" int vt_gather_cast_bf16(const vt_gather_cast_params* p, void* stream) {
   VT_REQUIRE(p && p->src && p->dst && p->rows > 0, "vt_gather_cast_bf16: bad params");
   VT_REQUIRE(p->D % 8 == 0 && p->lds % 4 == 0, "vt_gather_cast_bf16: D %% 8 and lds %% 4 required");
+  VT_REQUIRE(aligned16(p->src) && aligned16(p->dst), "vt_gather_cast_bf16: src and dst must be 16-byte aligned");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int blocks = grid_for((long long)p->rows * 32, 256);
   gather_cast_kernel<<<blocks, 256, 0, st>>>(p->src, p->lds, p->in_row, p->row_scale, static_cast<__nv_bfloat16*>(p->dst),
@@ -902,6 +914,7 @@ extern "C" int vt_gelu_bwd_colsum_blocks(int32_t M) { return fused_colsum_blocks
 extern "C" int vt_gather_cast_colsum_bf16(const vt_gather_cast_colsum_params* p, void* stream) {
   VT_REQUIRE(p && p->src && p->dst && p->colsum && p->workspace && p->rows > 0, "vt_gather_cast_colsum_bf16: bad params");
   VT_REQUIRE(p->D % 8 == 0 && p->lds % 4 == 0 && p->D <= GCC_CH * 256, "vt_gather_cast_colsum_bf16: D %% 8, lds %% 4 and D <= %d required", GCC_CH * 256);
+  VT_REQUIRE(aligned16(p->src) && aligned16(p->dst), "vt_gather_cast_colsum_bf16: src and dst must be 16-byte aligned");
   const int blocks = vt_gather_cast_colsum_blocks(p->rows);
   VT_REQUIRE(p->workspace_rows >= blocks, "vt_gather_cast_colsum_bf16: workspace holds %d partial rows, %d needed", p->workspace_rows, blocks);
   const int W = p->unscaled_sums ? 2 * p->D : p->D;     // colsum then holds [scaled sums | sums before the row scale]
