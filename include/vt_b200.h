@@ -223,18 +223,20 @@ int vt_gelu_bwd_colsum_bf16(const vt_gelu_bwd_colsum_params* p, void* stream);
  *   qkv bf16 [Bp, N, 3, H, hd] (the layout produced by transformer.py:167's reshape), hd = 64
  *   ctx bf16 [Bp, N, H*hd] = softmax(q k^T * scale) v      (transformer.py:170-174)
  *   lse fp32 [Bp, H, N]   (saved for backward; NULL = not written, for every implementation);
- *   probs fp32 [Bp,H,N,N] optional (Attention returns it, :177)
- * Three kernels behind one entry point: a tensor-core flash kernel for the spatial pass (N = 197; mma.sync bf16 with
- * fp32 accumulators, K/V tiles double-buffered in shared memory by cp.async, vt_attention_mma.cu), a warp-per-problem
- * kernel for the temporal pass
- * (N = 8, 18 816 problems/layer), and a generic warp-per-query kernel for any other N <= 256 (ViViT N = 9, probs output).
+ *   probs fp32 [Bp,H,N,N] optional (Attention returns it, :177; get_last_selfattention, video_transformer.py:258-261)
+ * Three kernels behind one entry point: tensor-core flash kernels for any N > 32 (the spatial pass N = 197, the joint
+ * space-time pass N = 1569; mma.sync bf16 with fp32 accumulators, K/V tiles double-buffered in shared memory by cp.async,
+ * vt_attention_mma.cu), a warp-per-problem kernel for the temporal pass (N = 8, 18 816 problems/layer), and a generic
+ * warp-per-query kernel for N <= 256 (ViViT N = 9, probs output).  With the tensor-core kernels the probs output comes
+ * from a row-tile softmax kernel that fits 8 rows of scores in shared memory (N <= ~6000).
  * VT_ATTN_TCGEN05 selects the tensor-core kernel (the name is kept for ABI compatibility).
  * ------------------------------------------------------------------------------------------- */
 enum { VT_ATTN_AUTO = 0, VT_ATTN_GENERIC = 1, VT_ATTN_TCGEN05 = 2, VT_ATTN_WARP8 = 3 };
 typedef struct {
   const void* qkv; void* ctx; float* lse; float* probs;
   int32_t Bp, N, H, hd; float scale;
-  int32_t impl;   /* VT_ATTN_AUTO picks: N == 8 -> warp-per-problem kernel; 32 < N <= 256 -> tensor-core kernel; else generic */
+  int32_t impl;   /* VT_ATTN_AUTO picks: N > 256 -> tensor-core kernel (probs included); else probs -> generic;
+                     N == 8 -> warp-per-problem kernel; N > 32 -> tensor-core kernel; else generic */
 } vt_attn_fwd_params;
 int vt_attn_fwd(const vt_attn_fwd_params* p, void* stream);
 typedef struct {
@@ -458,12 +460,6 @@ typedef struct {
   int32_t n_k; int32_t k[4];
 } vt_topk_hits_params;
 int vt_topk_hits(const vt_topk_hits_params* p, void* stream);
-
-/* probs[bp,h,i,j] = softmax_j(q_i . k_j * scale) for any N that fits 8 rows of scores in shared memory (N <= ~6000),
- * q/k read in place from the packed projection bf16 [Bp, N, 3, H, 64].  Serves get_last_selfattention
- * (video_transformer.py:258-261, transformer.py:560-561) for the 1569-token joint space-time variants. */
-typedef struct { const void* qkv; float* probs; int32_t Bp, N, H, hd; float scale; } vt_attn_probs_params;
-int vt_attn_probs(const vt_attn_probs_params* p, void* stream);
 
 /* vt_im2col_u8_bf16 with the batch-level Mixup / CutMix of mixup.py:102-114 folded in: sample b is blended with (mode 1,
  * lam*x + (1-lam)*x.flip(0)) or patched from (mode 2, box rows [yl,yh) x cols [xl,xh)) sample B-1-b after normalisation.

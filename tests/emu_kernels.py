@@ -184,6 +184,7 @@ class EmuKernels:
         return self._h(self._up(dh) * (cdf + zz * pdf))
 
     def attn_fwd(self, qkv, Bp, N, H, hd, scale, want_probs=False, impl=0):
+        self.calls.append(('attn', 'fwd', N))
         q = self._up(qkv).reshape(Bp, N, 3, H, hd).permute(2, 0, 3, 1, 4)
         s = (q[0] @ q[1].transpose(-1, -2)) * scale
         lse = torch.logsumexp(s, dim=-1)
@@ -192,6 +193,7 @@ class EmuKernels:
         return self._h(o), lse.to(self.f), (p.to(self.f) if want_probs else None)
 
     def attn_bwd(self, qkv, ctx, dctx, lse, Bp, N, H, hd, scale, impl=0):
+        self.calls.append(('attn', 'bwd', N))
         q = self._up(qkv).reshape(Bp, N, 3, H, hd).permute(2, 0, 3, 1, 4)
         Q, Kk, V = q[0], q[1], q[2]
         O = self._up(ctx).reshape(Bp, N, H, hd).transpose(1, 2)
@@ -227,11 +229,6 @@ class EmuKernels:
             xf = xf.clone()
             xf[..., yl:yh, xl:xh] = xf.flip(0)[..., yl:yh, xl:xh]
         return self.im2col(xf, tube, ph, pw)
-
-    def attn_probs(self, qkv, Bp, N, H, hd, scale):
-        q5 = self._up(qkv).reshape(Bp, N, 3, H, hd)
-        q, k = q5[:, :, 0].permute(0, 2, 1, 3), q5[:, :, 1].permute(0, 2, 1, 3)
-        return ((q @ k.transpose(-1, -2)) * scale).softmax(dim=-1).to(torch.float32)
 
     def linear_small_fwd(self, x, w, b):
         y = self._up(x) @ self._up(w).t()

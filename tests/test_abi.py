@@ -42,7 +42,7 @@ def test_missing_library_fails_loudly(monkeypatch):
         _lib.load_library()
 
 
-def test_ctypes_structs_match_the_header(tmp_path):
+def test_ctypes_param_structs_match_the_header(tmp_path):
     """Every ctypes Structure in _lib.py has the size and field offsets of its C twin in include/vt_b200.h."""
     import shutil
     import subprocess
@@ -62,7 +62,7 @@ def test_ctypes_structs_match_the_header(tmp_path):
              'vt_mse_bwd_params': _lib.MseBwdParams, 'vt_opt_params': _lib.OptParams,
              'vt_linear_small_params': _lib.LinearSmallParams, 'vt_linear_small_bwd_params': _lib.LinearSmallBwdParams,
              'vt_softmax_ce_params': _lib.SoftmaxCeParams, 'vt_scale_params': _lib.ScaleParams,
-             'vt_attn_probs_params': _lib.AttnProbsParams, 'vt_im2col_u8_mix_params': _lib.Im2colU8MixParams,
+             'vt_im2col_u8_mix_params': _lib.Im2colU8MixParams,
              'vt_cls_rows_params': _lib.ClsRowsParams, 'vt_gather_cast_colsum_params': _lib.GatherCastColsumParams, 'vt_gelu_bwd_colsum_params': _lib.GeluBwdColsumParams}
     lines = ['#include <stdio.h>', '#include <stddef.h>', f'#include "{os.path.join(ROOT, "include", "vt_b200.h")}"',
              'int main(void) {']

@@ -284,11 +284,11 @@ def test_xattn_delta_is_rowsum_of_do_times_o():
 
 
 # ---- packed-qkv attention (vt_attn_*): every implementation, dispatch thresholds ----------------------------------------
-ATTN_N = [8, 9, 32, 33, 63, 64, 65, 128, 129, 197, 255, 256]
+ATTN_N = [8, 9, 32, 33, 63, 64, 65, 128, 129, 197, 255, 256, 257, 289]
 
 
 def picked(N):
-    return WARP8 if N == 8 else (TC if 32 < N <= 256 else SIMT)
+    return WARP8 if N == 8 else (TC if N > 32 else SIMT)
 
 
 @pytest.mark.parametrize('impl', [SIMT, TC, WARP8])
@@ -296,6 +296,8 @@ def picked(N):
 def test_attn_packed_each_implementation(N, impl):
     if impl == WARP8 and N != 8:
         pytest.skip('the warp-per-problem kernel takes N = 8 only (refusal checked below)')
+    if impl == SIMT and N > 256:
+        pytest.skip('the generic kernel takes N <= 256 only (refusal checked below)')
     scale = 0.125
     q, k, v, do = inputs(2, 3, N, N, 64, scale, seed=N + impl)
     got = run_attn(q, k, v, do, scale, impl)
@@ -304,22 +306,22 @@ def test_attn_packed_each_implementation(N, impl):
 
 @pytest.mark.parametrize('N', ATTN_N)
 def test_attn_packed_auto_dispatch(N):
-    """impl 0 picks warp8 at N = 8, the tensor-core kernel for 32 < N <= 256 and the generic kernel otherwise: bitwise the
-    same results as the implementation asked for by name."""
+    """impl 0 picks warp8 at N = 8, the tensor-core kernel for N > 32 and the generic kernel otherwise: bitwise the same
+    results as the implementation asked for by name."""
     q, k, v, do = inputs(2, 3, N, N, 64, 0.125, seed=N)
     a, b = run_attn(q, k, v, do, 0.125, AUTO), run_attn(q, k, v, do, 0.125, picked(N))
     for n in a:
         assert torch.equal(a[n], b[n]), (N, n)
 
 
-def test_attn_packed_refusals():
+def test_attn_packed_refusals_at_kernel_limits():
     q, k, v, do = inputs(1, 1, 257, 257, 64, 0.125)
-    for impl in (AUTO, SIMT, TC, WARP8):
-        with pytest.raises(RuntimeError, match='N=257 unsupported'):
-            run_attn(q, k, v, do, 0.125, impl)
-    q, k, v, do = inputs(1, 1, 9, 9, 64, 0.125)
-    with pytest.raises(RuntimeError, match='warp8 kernel needs N == 8'):
-        run_attn(q, k, v, do, 0.125, WARP8)
+    with pytest.raises(RuntimeError, match='N=257 unsupported'):
+        run_attn(q, k, v, do, 0.125, SIMT)
+    for n in (9, 257):
+        q, k, v, do = inputs(1, 1, n, n, 64, 0.125)
+        with pytest.raises(RuntimeError, match='warp8 kernel needs N == 8'):
+            run_attn(q, k, v, do, 0.125, WARP8)
 
 
 @pytest.mark.parametrize('scale', [1.0, 0.05])

@@ -80,14 +80,15 @@ def test_head_module_and_fused_loss_autograd():
 
 
 @pytest.mark.parametrize('Bp,H,N', [(1, 12, 1569), (2, 2, 289), (1, 1, 77), (1, 3, 2049)])
-def test_attention_probabilities_long_sequences(Bp, H, N):
+def test_attn_fwd_probabilities_long_sequences(Bp, H, N):
     hd = 64
     g = torch.Generator().manual_seed(N)
     qkv = (torch.randn(Bp * N, 3 * H * hd, generator=g)).bfloat16()
     q5 = qkv.float().view(Bp, N, 3, H, hd)
     q, k = q5[:, :, 0].permute(0, 2, 1, 3), q5[:, :, 1].permute(0, 2, 1, 3)
     ref = ((q.double() @ k.double().transpose(-1, -2)) * hd ** -0.5).softmax(dim=-1)
-    got = K().attn_probs(qkv.cuda(), Bp, N, H, hd, hd ** -0.5)
+    # impl 2, the tensor-core path: the row-tile probability kernel at every N, as the automatic choice takes it past 256
+    _, _, got = K().attn_fwd(qkv.cuda(), Bp, N, H, hd, hd ** -0.5, want_probs=True, impl=2)
     assert got.shape == (Bp, H, N, N)
     assert rel_err(got.cpu(), ref) < 1e-5
     assert float((got.sum(-1) - 1).abs().max()) < 1e-5
@@ -117,8 +118,8 @@ def test_get_last_selfattention_joint_space_time_1569_tokens():
 
 
 def test_attention_module_long_sequence_forward_backward():
-    """Stand-alone Attention.forward (transformer.py:165-177) past 256 tokens: context from the streaming tensor-core kernels,
-    probabilities from the row-tile kernel, gradients through the streaming backward."""
+    """Stand-alone Attention.forward (transformer.py:165-177) past 256 tokens: context from the tiled tensor-core kernels,
+    probabilities from the row-tile kernel, gradients through the tiled backward."""
     from videotransformer_pytorch_b200 import Attention
     torch.manual_seed(1)
     a = Attention(128, num_heads=2, qkv_bias=True)

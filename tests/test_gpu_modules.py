@@ -182,7 +182,7 @@ def test_space_only_small_vs_oracle():
 
 
 def test_joint_space_time_vs_golden(golden):
-    """joint_space_time with 289 tokens per clip (past the single-pass kernels): streaming tensor-core attention, head dim 64."""
+    """joint_space_time with 289 tokens per clip (past the single-pass kernels): tiled tensor-core attention, head dim 64."""
     from videotransformer_pytorch_b200 import TimeSformer
     g = golden('timesformer_joint_n289')
     c = g.cfg
@@ -237,7 +237,7 @@ def test_vivit_joint_and_divided_variants_vs_golden(golden, name, attention_type
 
 
 def test_vivit_b_joint_space_time_1569_tokens_vs_oracle():
-    """ViViT-B model 1 at 16x224 (1 + 196*8 = 1569 tokens per clip, streaming tensor-core attention), one layer, B=1."""
+    """ViViT-B model 1 at 16x224 (1 + 196*8 = 1569 tokens per clip, tiled tensor-core attention), one layer, B=1."""
     from oracle import vt_oracle as O
     from videotransformer_pytorch_b200 import ViViT
     torch.manual_seed(8)

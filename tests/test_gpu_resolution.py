@@ -122,7 +122,7 @@ def _timesformer_b(T, seed):
 
 @pytest.mark.parametrize('T,side', [(16, 448), (8, 320)])
 def test_timesformer_b_larger_inputs_vs_oracle(T, side, monkeypatch):
-    """img_size 224, one layer, B = 1: 448^2 gives spatial N = 785 (streaming kernels), 320^2 gives N = 401.  The fp64
+    """img_size 224, one layer, B = 1: 448^2 gives spatial N = 785 (tiled tensor-core kernels), 320^2 gives N = 401.  The fp64
     oracle runs on the GPU for speed, except its pos_embed resize, which runs on the CPU like the reference's."""
     from oracle import resize_oracle as O
     cpu_resize = O.interpolate_pos_encoding

@@ -125,9 +125,9 @@ def test_timesformer_space_only(golden, emu):
 
 
 @pytest.mark.parametrize('name', ['timesformer_joint_tiny', 'timesformer_joint_n289'])
-def test_timesformer_joint_space_time(golden, emu, name):
-    """joint_space_time (video_transformer.py:104-116): 17 tokens go through the single-pass attention kernel, 289 tokens
-    through the streaming one (ops.ATTN_SINGLE_PASS_MAX)."""
+def test_timesformer_joint_space_time_through_vt_attn(golden, emu, name):
+    """joint_space_time (video_transformer.py:104-116): the packed-qkv attention vt_attn_* takes every sequence length,
+    17 tokens and 289 tokens (past the 256 of the single-pass kernels) alike; the pooling attention vt_xattn_* never runs."""
     from videotransformer_pytorch_b200 import TimeSformer
     g = golden(name)
     c = g.cfg
@@ -145,8 +145,10 @@ def test_timesformer_joint_space_time(golden, emu, name):
     assert rel_err(y, g.out['y_train']) < 2e-5
     (y.double() * g.out['loss_w']).sum().backward()
     check_grads({n: p.grad for n, p in m.named_parameters()}, g, 2e-4)
-    used = {c_[0] for c_ in emu.calls if isinstance(c_, tuple)}
-    assert ('xattn' in used) == (name == 'timesformer_joint_n289')
+    n = 1 + c['num_frames'] * (c['img_size'] // c['patch_size']) ** 2
+    assert n == (289 if name == 'timesformer_joint_n289' else 17)
+    assert ('attn', 'fwd', n) in emu.calls and ('attn', 'bwd', n) in emu.calls
+    assert not any(c_[0] == 'xattn' for c_ in emu.calls)
 
 
 def test_timesformer_accepts_uint8_clip(golden, emu):

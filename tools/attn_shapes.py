@@ -43,7 +43,7 @@ WRAPPED = ('attn_fwd', 'attn_bwd', 'xattn_fwd', 'xattn_bwd')
 
 def packed_kernel(N):
     """which vt_attn_* kernel the automatic choice takes (vt_attention.cu pick_impl, use_whole)"""
-    return 'warp8' if N == 8 else 'whole' if 32 < N <= 256 else 'generic'
+    return 'warp8' if N == 8 else 'generic' if N <= 32 else 'whole' if N <= 256 else 'tiled'
 
 
 def set_whole(env):

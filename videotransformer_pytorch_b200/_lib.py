@@ -234,10 +234,6 @@ class ScaleParams(C.Structure):
     _fields_ = [('inp', c_vp), ('scalar', c_vp), ('out', c_vp), ('n', c_i64)]
 
 
-class AttnProbsParams(C.Structure):
-    _fields_ = [('qkv', c_vp), ('probs', c_vp), ('Bp', c_i32), ('N', c_i32), ('H', c_i32), ('hd', c_i32), ('scale', c_f32)]
-
-
 class TopkHitsParams(C.Structure):
     _fields_ = [('logits', c_vp), ('labels', c_vp), ('probs', c_vp), ('hits', c_vp), ('samples', c_vp),
                 ('B', c_i32), ('V', c_i32), ('C', c_i32), ('n_k', c_i32), ('k', c_i32 * 4)]
@@ -291,7 +287,7 @@ EXPORTS = ['vt_version', 'vt_last_error', 'vt_sm_count', 'vt_set_reserved_sms', 
            'vt_pool_fwd', 'vt_pool_bwd_scratch', 'vt_pool_bwd', 'vt_xattn_fwd', 'vt_xattn_bwd', 'vt_maxpool_fwd',
            'vt_maxpool_bwd', 'vt_im2col3d_bf16', 'vt_mvit_tokens_fwd', 'vt_mvit_tokens_bwd', 'vt_mse_blocks',
            'vt_mse_fwd', 'vt_mse_bwd', 'vt_opt_norm2', 'vt_opt_sgd', 'vt_opt_adamw',
-           'vt_linear_small_fwd', 'vt_linear_small_bwd', 'vt_softmax_ce', 'vt_scale_by_scalar', 'vt_attn_probs',
+           'vt_linear_small_fwd', 'vt_linear_small_bwd', 'vt_softmax_ce', 'vt_scale_by_scalar',
            'vt_im2col_u8_mix_bf16', 'vt_pos_resize_fwd', 'vt_pos_resize_bwd', 'vt_topk_hits',
            'vt_resized_crop_u8', 'vt_color_jitter_u8', 'vt_gemm_e4m3', 'vt_quant_rows_e4m3', 'vt_rand_augment_u8']
 
@@ -691,19 +687,6 @@ class CudaKernels:
         p.Bp, p.N, p.H, p.hd, p.scale, p.impl = Bp, N, H, hd, scale, impl
         _check(lib.vt_attn_bwd(C.byref(p), _stream()), 'vt_attn_bwd')
         return dqkv
-
-    def attn_probs(self, qkv, Bp, N, H, hd, scale):
-        """softmax(q k^T * scale) of a packed projection [Bp, N, 3, H, hd] -> fp32 [Bp, H, N, N] (any N; head dim 64)"""
-        lib = load_library()
-        _req(qkv, torch.bfloat16, 'attn_probs.qkv')
-        if not qkv.is_contiguous() or qkv.numel() != Bp * N * 3 * H * hd:
-            raise RuntimeError('attn_probs: qkv must be contiguous [Bp, N, 3, H, hd]')
-        probs = torch.empty((Bp, H, N, N), dtype=torch.float32, device=qkv.device)
-        p = AttnProbsParams()
-        p.qkv, p.probs = qkv.data_ptr(), probs.data_ptr()
-        p.Bp, p.N, p.H, p.hd, p.scale = Bp, N, H, hd, scale
-        _check(lib.vt_attn_probs(C.byref(p), _stream()), 'vt_attn_probs')
-        return probs
 
     # -- classification head + loss -----------------------------------------------------------
     def linear_small_fwd(self, x, w, b):

@@ -1,8 +1,8 @@
 // Softmax attention core on packed qkv (bf16 [Bp, N, 3, H, 64]) — generic warp-primitive kernels.
 // One CTA per (batch', head); Q/K/V/dO rows live in shared memory with a 33-word row pitch so that both
 // "lane = key/query index" and "lane = feature pair" access patterns are bank-conflict free.
-// Used for the temporal pass of ViViT (N = 9), the probability output and as the general-N path; the 197-token spatial
-// pass runs on the tensor-core kernels (vt_attention_mma.cu), N = 8 on the warp-per-problem kernel (vt_attention_small.cu).
+// Used for the temporal pass of ViViT (N = 9), the probability output at N <= 256 and the other N <= 32; N > 32 runs on
+// the tensor-core kernels (vt_attention_mma.cu), N = 8 on the warp-per-problem kernel (vt_attention_small.cu).
 #include "vt_attention_mma.cuh"
 
 namespace vt {
@@ -222,12 +222,16 @@ attn_bwd_kernel(const __nv_bfloat16* __restrict__ qkv, const __nv_bfloat16* __re
 
 int attn8_fwd_launch(const vt_attn_fwd_params* p, cudaStream_t st);
 int attn8_bwd_launch(const vt_attn_bwd_params* p, cudaStream_t st);
+int attn_probs_launch(const void* qkv, float* probs, int Bp, int N, int H, float scale, cudaStream_t st);
 
+// past the generic kernel's N the tensor-core kernels take every call, probabilities included (the 64-row tiles: the
+// whole-problem kernels stop at N = 256)
 static int pick_impl(int impl, int N, bool probs) {
   if (impl != VT_ATTN_AUTO) return impl;
+  if (N > MAX_N) return VT_ATTN_TCGEN05;
   if (probs) return VT_ATTN_GENERIC;
   if (N == 8) return VT_ATTN_WARP8;
-  if (N > 32 && N <= 256) return VT_ATTN_TCGEN05;
+  if (N > 32) return VT_ATTN_TCGEN05;
   return VT_ATTN_GENERIC;
 }
 
@@ -258,12 +262,15 @@ using namespace vt;
 extern "C" int vt_attn_fwd(const vt_attn_fwd_params* p, void* stream) {
   VT_REQUIRE(p && p->qkv && p->ctx, "vt_attn_fwd: null pointer");   // lse may be NULL (not written)
   VT_REQUIRE(p->hd == HD, "vt_attn_fwd: head dim %d unsupported (64 only)", p->hd);
-  VT_REQUIRE(p->N >= 1 && p->N <= MAX_N, "vt_attn_fwd: N=%d unsupported (1..%d)", p->N, MAX_N);
+  VT_REQUIRE(p->N >= 1, "vt_attn_fwd: N=%d unsupported", p->N);
   VT_REQUIRE(p->Bp > 0 && p->H > 0, "vt_attn_fwd: bad Bp/H");
   const int impl = pick_impl(p->impl, p->N, p->probs != nullptr);
   if (impl == VT_ATTN_TCGEN05) {
-    VT_REQUIRE(p->probs == nullptr, "vt_attn_fwd: the tensor-core kernel has no probs output");
     VT_REQUIRE((((uintptr_t)p->qkv | (uintptr_t)p->ctx) & 15) == 0, "vt_attn_fwd: qkv / ctx must be 16-byte aligned");
+    if (p->probs) {   // the tensor-core kernels write no probabilities: the row-tile softmax kernel does
+      const int rc = attn_probs_launch(p->qkv, p->probs, p->Bp, p->N, p->H, p->scale, static_cast<cudaStream_t>(stream));
+      if (rc) return rc;
+    }
     MmaAttn a = packed_operands(p->qkv, p->ctx, p->lse, p->Bp, p->N, p->H, p->scale);
     a.o_out = static_cast<__nv_bfloat16*>(p->ctx);
     if (use_whole(a)) return attn_whole_fwd(a, p->Bp, static_cast<cudaStream_t>(stream));
@@ -273,6 +280,7 @@ extern "C" int vt_attn_fwd(const vt_attn_fwd_params* p, void* stream) {
     VT_REQUIRE(p->probs == nullptr && p->N == 8, "vt_attn_fwd: warp8 kernel needs N == 8 and no probs output");
     return attn8_fwd_launch(p, static_cast<cudaStream_t>(stream));
   }
+  VT_REQUIRE(p->N <= MAX_N, "vt_attn_fwd: N=%d unsupported by the generic kernel (1..%d)", p->N, MAX_N);
   const int npad = (p->N + 31) & ~31;
   const int smem = (2 * p->N * PITCH + AT_WARPS * npad) * 4;
   static int max_set = 0;
@@ -289,7 +297,7 @@ extern "C" int vt_attn_fwd(const vt_attn_fwd_params* p, void* stream) {
 extern "C" int vt_attn_bwd(const vt_attn_bwd_params* p, void* stream) {
   VT_REQUIRE(p && p->qkv && p->ctx && p->dctx && p->lse && p->dqkv, "vt_attn_bwd: null pointer");
   VT_REQUIRE(p->hd == HD, "vt_attn_bwd: head dim %d unsupported (64 only)", p->hd);
-  VT_REQUIRE(p->N >= 1 && p->N <= MAX_N, "vt_attn_bwd: N=%d unsupported (1..%d)", p->N, MAX_N);
+  VT_REQUIRE(p->N >= 1, "vt_attn_bwd: N=%d unsupported", p->N);
   const int impl = pick_impl(p->impl, p->N, false);
   if (impl == VT_ATTN_TCGEN05) {
     VT_REQUIRE((((uintptr_t)p->qkv | (uintptr_t)p->ctx | (uintptr_t)p->dctx | (uintptr_t)p->dqkv) & 15) == 0,
@@ -309,6 +317,7 @@ extern "C" int vt_attn_bwd(const vt_attn_bwd_params* p, void* stream) {
     VT_REQUIRE(p->N == 8, "vt_attn_bwd: warp8 kernel needs N == 8");
     return attn8_bwd_launch(p, static_cast<cudaStream_t>(stream));
   }
+  VT_REQUIRE(p->N <= MAX_N, "vt_attn_bwd: N=%d unsupported by the generic kernel (1..%d)", p->N, MAX_N);
   const int npad = (p->N + 31) & ~31;
   const int smem = (4 * p->N * PITCH + 2 * npad + 2 * AT_WARPS * npad) * 4;
   static int max_set = 0;

@@ -1,7 +1,8 @@
 // Small fp32 kernels around the transformer body:
 //   * skinny linear layer (classification head: 8 x 768 -> 400) forward / backward — warp-per-output GEMV, fp32 throughout
 //   * softmax cross-entropy (hard labels or soft targets) forward + gradient in one launch
-//   * attention probabilities softmax(q k^T * scale) for long sequences (get_last_selfattention of the joint variants)
+//   * attention probabilities softmax(q k^T * scale) for long sequences (vt_attn_fwd's probs output past 256 tokens:
+//     get_last_selfattention of the joint variants)
 //   * uint8 clip -> normalised bf16 patch operand with Mixup / CutMix of the flipped batch folded in
 //   * top-k hit counters of an evaluation step (view mean, optional softmax, rank of the label)
 // All are latency / bandwidth bound warp-primitive kernels (no tensor cores: M <= 64 rows or one-off visualisation work).
@@ -283,6 +284,21 @@ __global__ void im2col_u8_mix_kernel(const uint8_t* __restrict__ x, const float*
   }
 }
 
+// the probs output of vt_attn_fwd on the tensor-core path (vt_attention.cu); qkv is the packed projection at head dim 64
+int attn_probs_launch(const void* qkv, float* probs, int Bp, int N, int H, float scale, cudaStream_t st) {
+  const size_t smem = ((size_t)PR_ROWS * N + PR_ROWS * 64 + PR_KT * 65) * sizeof(float);
+  VT_REQUIRE(smem <= 200 * 1024, "vt_attn_fwd: N=%d too long for the probs output (%zu bytes of shared memory)", N, smem);
+  static size_t max_set = 48 * 1024;
+  if (smem > max_set) {
+    cudaError_t e = cudaFuncSetAttribute(attn_probs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    VT_REQUIRE(e == cudaSuccess, "vt_attn_fwd: probs smem attribute: %s", cudaGetErrorString(e));
+    max_set = 200 * 1024;
+  }
+  dim3 grid((N + PR_ROWS - 1) / PR_ROWS, Bp * H);
+  attn_probs_kernel<<<grid, 256, smem, st>>>(static_cast<const __nv_bfloat16*>(qkv), probs, N, H, scale);
+  return check_launch("attn_probs_kernel");
+}
+
 static int grid_1d(long long n, int threads) {
   long long b = (n + threads - 1) / threads;
   const long long cap = (long long)sm_count() * 16;
@@ -335,24 +351,6 @@ extern "C" int vt_scale_by_scalar(const vt_scale_params* p, void* stream) {
   VT_REQUIRE(p && p->in && p->scalar && p->out && p->n > 0, "vt_scale_by_scalar: bad params");
   scale_by_scalar_kernel<<<grid_1d(p->n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(p->in, p->scalar, p->out, p->n);
   return check_launch("scale_by_scalar_kernel");
-}
-
-extern "C" int vt_attn_probs(const vt_attn_probs_params* p, void* stream) {
-  VT_REQUIRE(p && p->qkv && p->probs, "vt_attn_probs: null pointer");
-  VT_REQUIRE(p->hd == 64, "vt_attn_probs: head dim %d unsupported (64 only)", p->hd);
-  VT_REQUIRE(p->Bp > 0 && p->H > 0 && p->N > 0, "vt_attn_probs: bad shape");
-  const size_t smem = ((size_t)PR_ROWS * p->N + PR_ROWS * 64 + PR_KT * 65) * sizeof(float);
-  VT_REQUIRE(smem <= 200 * 1024, "vt_attn_probs: N=%d too long (%zu bytes of shared memory)", p->N, smem);
-  static size_t max_set = 48 * 1024;
-  if (smem > max_set) {
-    cudaError_t e = cudaFuncSetAttribute(attn_probs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-    VT_REQUIRE(e == cudaSuccess, "vt_attn_probs: smem attribute: %s", cudaGetErrorString(e));
-    max_set = 200 * 1024;
-  }
-  dim3 grid((p->N + PR_ROWS - 1) / PR_ROWS, p->Bp * p->H);
-  attn_probs_kernel<<<grid, 256, smem, static_cast<cudaStream_t>(stream)>>>(static_cast<const __nv_bfloat16*>(p->qkv), p->probs,
-                                                                             p->N, p->H, p->scale);
-  return check_launch("attn_probs_kernel");
 }
 
 extern "C" int vt_im2col_u8_mix_bf16(const vt_im2col_u8_mix_params* p, void* stream) {

@@ -226,27 +226,6 @@ def _dgrad(dout, w, m_tok, k_in, n_out, **kw):
     return K().gemm(dout, w, m_tok, k_in, n_out, b_mn=True, **kw)
 
 
-ATTN_SINGLE_PASS_MAX = 256      # vt_attn_*: single-pass kernels; longer sequences go to the streaming vt_xattn_* kernels
-
-
-def _packed_heads(qkv, Bp, N, H, hd):
-    """q, k, v of a packed [Bp*N, 3*H*hd] projection as [Bp, H, N, hd] views (token-major, no copy)."""
-    v5 = qkv.view(Bp, N, 3, H, hd)
-    return tuple(v5[:, :, s].permute(0, 2, 1, 3) for s in range(3))
-
-
-def _streaming_attn_bwd(k, qkv, cx, dcx, lse, Bp, N, H, hd):
-    """dqkv of a long-sequence attention through the streaming tensor-core kernels (q/k/v and dq in place in the packed layout)."""
-    q4, k4, v4 = _packed_heads(qkv, Bp, N, H, hd)
-    dqkv = torch.empty_like(qkv)
-    dq4, dk4, dv4 = _packed_heads(dqkv, Bp, N, H, hd)
-    D = H * hd
-    dk, dv = k.xattn_bwd(q4, k4, v4, cx.view(Bp, N, D), dcx.view(Bp, N, D), lse, hd ** -0.5, dq4)
-    dk4.copy_(dk)           # fp32 [Bp,H,N,hd] accumulators -> their bf16 slots of the packed gradient
-    dv4.copy_(dv)
-    return dqkv
-
-
 def _cast_with_colsum(k, src2d, in_row=None, row_scale=None, rows=None):
     """dY in bf16 (gathered / scaled rows of the fp32 gradient stream) and its column sums = the bias gradient."""
     if FUSED_COLSUM:
@@ -392,14 +371,7 @@ class SpatialAttnFn(torch.autograd.Function):
         save = ctx is not None
         xn, mean, rstd = k.ln_fwd(x2, ln_w, ln_b, eps, in_row=maps['sp_in'], rows=Ms, **_stats(save))
         qkv = _gemm(k, xn, qkv_wh, Ms, 3 * D, D, bias=qkv_b, epi='bf16', tag='qkv')
-        if P + 1 <= ATTN_SINGLE_PASS_MAX:
-            cx, lse, _ = k.attn_fwd(qkv, B * T, P + 1, H, hd, hd ** -0.5, **_lse(save))
-        else:
-            # frames of 256 patches or more (inputs larger than 256 x 256 at patch 16): streaming tensor-core kernel,
-            # q/k/v read in place from the packed projection
-            q4, k4, v4 = _packed_heads(qkv, B * T, P + 1, H, hd)
-            cx, lse = k.xattn_fwd(q4, k4, v4, hd ** -0.5, **_lse(save))
-            cx = cx.view(Ms, D)
+        cx, lse, _ = k.attn_fwd(qkv, B * T, P + 1, H, hd, hd ** -0.5, **_lse(save))
         ybig = torch.empty((R + B * T, D), dtype=torch.float32, device=x.device)
         _gemm(k, cx, proj_wh, Ms, D, D, bias=proj_b, epi='f32', aux=x2, aux_row=maps['sp_aux'], out=ybig,
               out_row=maps['sp_out'], row_scale=dp, row_map=affine_row_maps(B, T, P, D)['spatial'], tag='proj')
@@ -425,10 +397,7 @@ class SpatialAttnFn(torch.autograd.Function):
         g, d_proj_b = _cast_with_colsum(k, dy2, in_row=maps['sp_in'], row_scale=_mul_opt(dp, maps['sp_cls_scale']), rows=Ms)
         d_proj_w = _wgrad(g, cx, D, D, Ms, tag='proj', wptr=ctx.wptrs[1])
         dcx = _dgrad(g, proj_wh, Ms, D, D, epi='bf16', tag='proj')
-        if P + 1 <= ATTN_SINGLE_PASS_MAX:
-            dqkv = k.attn_bwd(qkv, cx, dcx, lse, B * T, P + 1, H, hd, hd ** -0.5)
-        else:
-            dqkv = _streaming_attn_bwd(k, qkv, cx, dcx, lse, B * T, P + 1, H, hd)
+        dqkv = k.attn_bwd(qkv, cx, dcx, lse, B * T, P + 1, H, hd, hd ** -0.5)
         d_qkv_w = _wgrad(dqkv, xn, 3 * D, D, Ms, tag='qkv', wptr=ctx.wptrs[0])
         d_qkv_b = k.colsum(dqkv)
         dxn = _dgrad(dqkv, qkv_wh, Ms, D, 3 * D, epi='bf16', tag='qkv')
@@ -453,14 +422,7 @@ class JointAttnFn(torch.autograd.Function):
         save = ctx is not None
         xn, mean, rstd = k.ln_fwd(x2, ln_w, ln_b, eps, **_stats(save))
         qkv = _gemm(k, xn, qkv_wh, M, 3 * D, D, bias=qkv_b, epi='bf16', tag='qkv')
-        if N <= ATTN_SINGLE_PASS_MAX:
-            cx, lse, _ = k.attn_fwd(qkv, Bp, N, H, hd, hd ** -0.5, **_lse(save))
-        else:
-            # long sequences (joint space-time attention: 1 + P*T = 1569 tokens): streaming tensor-core kernel, q/k/v read in
-            # place from the packed projection
-            q4, k4, v4 = _packed_heads(qkv, Bp, N, H, hd)
-            cx, lse = k.xattn_fwd(q4, k4, v4, hd ** -0.5, **_lse(save))
-            cx = cx.view(M, D)
+        cx, lse, _ = k.attn_fwd(qkv, Bp, N, H, hd, hd ** -0.5, **_lse(save))
         y = torch.empty_like(x)
         _gemm(k, cx, proj_wh, M, D, D, bias=proj_b, epi='f32', aux=x2, out=y.view(M, D), row_scale=dp, tag='proj')
         if save:
@@ -482,10 +444,7 @@ class JointAttnFn(torch.autograd.Function):
         g, d_proj_b = _cast_with_colsum(k, dy2, row_scale=dp)
         d_proj_w = _wgrad(g, cx, D, D, M, tag='proj', wptr=ctx.wptrs[1])
         dcx = _dgrad(g, proj_wh, M, D, D, epi='bf16', tag='proj')
-        if N <= ATTN_SINGLE_PASS_MAX:
-            dqkv = k.attn_bwd(qkv, cx, dcx, lse, Bp, N, H, hd, hd ** -0.5)
-        else:
-            dqkv = _streaming_attn_bwd(k, qkv, cx, dcx, lse, Bp, N, H, hd)
+        dqkv = k.attn_bwd(qkv, cx, dcx, lse, Bp, N, H, hd, hd ** -0.5)
         d_qkv_w = _wgrad(dqkv, xn, 3 * D, D, M, tag='qkv', wptr=ctx.wptrs[0])
         d_qkv_b = k.colsum(dqkv)
         dxn = _dgrad(dqkv, qkv_wh, M, D, 3 * D, epi='bf16', tag='qkv')
@@ -713,15 +672,7 @@ class AttentionCoreFn(torch.autograd.Function):
         hd = C // H
         xh = k.gather_cast(x.reshape(M, C).float().contiguous())
         qkv = k.gemm(xh, qkv_wh, M, 3 * C, C, bias=qkv_b, epi='bf16')
-        if N <= ATTN_SINGLE_PASS_MAX:
-            cx, lse, probs = k.attn_fwd(qkv, Bp, N, H, hd, hd ** -0.5, want_probs=want_probs)
-        else:
-            # long sequences (joint space-time: 1569 tokens): context by the streaming tensor-core kernel; the probability
-            # maps the reference returns (transformer.py:171-177) by a row-tile softmax kernel, 8 query rows per CTA
-            q4, k4, v4 = _packed_heads(qkv, Bp, N, H, hd)
-            cx, lse = k.xattn_fwd(q4, k4, v4, hd ** -0.5)
-            cx = cx.view(M, C)
-            probs = k.attn_probs(qkv, Bp, N, H, hd, hd ** -0.5) if want_probs else None
+        cx, lse, probs = k.attn_fwd(qkv, Bp, N, H, hd, hd ** -0.5, want_probs=want_probs)
         out = k.gemm(cx, proj_wh, M, C, C, bias=proj_b, epi='f32').view(Bp, N, C)
         ctx.save_for_backward(xh, qkv, cx, lse, qkv_wh, proj_wh)
         ctx.geom = (Bp, N, C, H)
@@ -741,10 +692,7 @@ class AttentionCoreFn(torch.autograd.Function):
         d_proj_w = _wgrad(g, cx, C, C, M)
         d_proj_b = k.colsum(g)
         dcx = _dgrad(g, proj_wh, M, C, C, epi='bf16')
-        if N <= ATTN_SINGLE_PASS_MAX:
-            dqkv = k.attn_bwd(qkv, cx, dcx, lse, Bp, N, H, hd, hd ** -0.5)
-        else:
-            dqkv = _streaming_attn_bwd(k, qkv, cx, dcx, lse, Bp, N, H, hd)
+        dqkv = k.attn_bwd(qkv, cx, dcx, lse, Bp, N, H, hd, hd ** -0.5)
         d_qkv_w = _wgrad(dqkv, xh, 3 * C, C, M)
         d_qkv_b = k.colsum(dqkv)
         dx = _dgrad(dqkv, qkv_wh, M, C, 3 * C, epi='f32').view(Bp, N, C)

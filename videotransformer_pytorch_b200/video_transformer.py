@@ -3,7 +3,7 @@ and state-dict keys (reference video_transformer.py:20-268 and :270-557), forwar
 sm_90a kernels.
 
 Covered configurations (SURVEY.md §8a, §8f rank 4): TimeSformer `divided_space_time`, `space_only` (197-token joint
-attention per frame) and `joint_space_time` (one 1569-token attention per clip, streaming tensor-core kernel); ViViT
+attention per frame) and `joint_space_time` (one 1569-token attention per clip, tiled tensor-core kernels); ViViT
 `fact_encoder` (model 2), `joint_space_time` (model 1) and `divided_space_time` (model 3).  TimeSformer also takes clips
 whose patch grid differs from img_size's (interpolate_pos_encoding, reference :171-191).  Nothing falls back to eager
 PyTorch.
