@@ -37,7 +37,7 @@ class EmuKernels:
 
     def gemm(self, a, b, M, N, Kdim, *, a_mn=False, b_mn=False, epi='bf16', bias=None, bias2=None, out=None, out2=None,
              aux=None, out_row=None, aux_row=None, row_scale=None, out_rows=None, split_ok=False,
-             force_splits=0, force_bn=0, force_cluster=0, debug=None, row_map=None, force_tail=0, tag=None, out_zeroed=False):
+             force_splits=0, force_bn=0, row_map=None, tag=None):
         self.calls.append(('gemm', M, N, Kdim, a_mn, b_mn, epi))
         if row_map is not None:
             # the affine description handed to the TMA residual epilogue must be the out_row / aux_row arrays in closed form

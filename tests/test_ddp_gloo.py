@@ -285,7 +285,9 @@ def _captured_body_worker(rank, world, port, q):
             direct.append((M, N))
         return real_gemm(a, b, M, N, Kd, **kw)
     _lib.K.gemm = spy
-    red.zero_grad()
+    with torch.no_grad():                      # no gradient may depend on zeroed buckets
+        for p in params:
+            p.grad.fill_(float('nan'))
     grads = red.backward_into_buckets(net(x).square().mean(), params)
     assert ops.GRAD_DEST is None
     aliased = sum(1 for p, gr in zip(params, grads) if gr.data_ptr() == p.grad.data_ptr())

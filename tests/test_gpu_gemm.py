@@ -1,8 +1,4 @@
-"""wgmma GEMM (vt_gemm) vs torch fp32 matmul on the same bf16-rounded operands.  -m gpu
-
-force_cluster, force_tail and the VT_TMA_* / VT_SPLITK_WORKSPACE switches are still accepted by the ABI but select nothing
-on sm_90a (one kernel, register epilogue, split-K through the workspace); the tests that flip them check that both sides
-still match torch."""
+"""wgmma GEMM (vt_gemm) vs torch fp32 matmul on the same bf16-rounded operands.  -m gpu"""
 
 import pytest
 import torch
@@ -96,24 +92,24 @@ def test_gemm_gelu_and_dgelu():
     assert rel(out, ref_mm(g, b, False, False) * zz.grad) < 4e-3
 
 
-@pytest.mark.parametrize('path', ['tma-reduce-add', 'workspace'])
-@pytest.mark.parametrize('cluster', [1, 3], ids=['single-cta', 'cta-pair'])
+@pytest.mark.parametrize('bn,staged', [(0, '1'), (128, '0'), (192, '1'), (256, '1')],
+                         ids=['auto', 'bn128-register', 'bn192', 'bn256'])
 @pytest.mark.parametrize('splits', [2, 5, 16])
-def test_gemm_splitk_wgrad(splits, cluster, path, monkeypatch):
-    """split-K partial tiles: reduce-added into the zeroed output by TMA (default) or summed from an fp32 workspace."""
-    if path == 'workspace':
-        monkeypatch.setenv('VT_SPLITK_WORKSPACE', '1')
+def test_gemm_splitk_wgrad(splits, bn, staged, monkeypatch):
+    """split-K partial tiles summed from the fp32 workspace into the output: with the planner's tile, and at each forced
+    width (the partials take the staged fp32 rows at BN = 128 only, so BN = 128 is also run on the register epilogue)."""
+    monkeypatch.setenv('VT_GEMM_STAGED_EPI', staged)
     Mtok, Nout, Kin = 2048 + 64, 384, 256
     dy, x = mk((Mtok, Nout), 16).bfloat16(), mk((Mtok, Kin), 17).bfloat16()
     out = torch.full((Nout, Kin), 7.0, device='cuda')            # stale contents must not leak into the result
-    K().gemm(dy, x, Nout, Kin, Mtok, a_mn=True, b_mn=True, epi='f32', split_ok=True, force_splits=splits,
-             force_cluster=cluster, out=out)
+    K().gemm(dy, x, Nout, Kin, Mtok, a_mn=True, b_mn=True, epi='f32', split_ok=True, force_splits=splits, force_bn=bn,
+             out=out)
     r = dy.float().t() @ x.float()
     assert rel(out, r) < 1e-5
 
 
 def test_gemm_splitk_odd_tile_edges():
-    """in-place split-K on a shape whose tiles hang over both output edges (TMA clips the reduce-add box)."""
+    """split-K on a shape whose tiles hang over both output edges."""
     Mtok, Nout, Kin = 1000, 200, 136
     dy, x = mk((Mtok, Nout), 26).bfloat16(), mk((Mtok, Kin), 27).bfloat16()
     out = K().gemm(dy, x, Nout, Kin, Mtok, a_mn=True, b_mn=True, epi='f32', split_ok=True, force_splits=4)
@@ -159,83 +155,80 @@ def test_gelu_kernels(shape):
     assert rel(K().dgelu(dh, z), zf.grad) < 3e-3
 
 
-@pytest.mark.parametrize('cluster', [1, 2, 3])
-@pytest.mark.parametrize('M,N,Kd,a_mn,b_mn,bn', [(128, 256, 128, False, False, 256), (100, 128, 64, False, False, 128),
-                                                  (1000, 768, 768, False, False, 0), (12544, 768, 768, False, True, 0),
-                                                  (12552, 3072, 768, False, False, 256), (12608, 768, 768, False, True, 192),
-                                                  (2304, 768, 12544, True, True, 0), (640, 576, 320, True, True, 192),
-                                                  (640, 384, 320, True, False, 128)])
-def test_gemm_cluster_multicast(M, N, Kd, a_mn, b_mn, bn, cluster):
-    if cluster == 3 and bn == 192:
-        bn = 256          # the CTA-pair kernel has BN 128 / 256
+@pytest.mark.parametrize('bn', [0, 128, 192, 256])
+@pytest.mark.parametrize('M,N,Kd,a_mn,b_mn', [(128, 256, 128, False, False), (100, 128, 64, False, False),
+                                              (1000, 768, 768, False, False), (12544, 768, 768, False, True),
+                                              (12552, 3072, 768, False, False), (12608, 768, 768, False, True),
+                                              (2304, 768, 12544, True, True), (640, 576, 320, True, True),
+                                              (640, 384, 320, True, False)])
+def test_gemm_forced_tile_widths(M, N, Kd, a_mn, b_mn, bn):
+    """every operand layout at the planner's tile width (bn = 0) and at each forced one"""
     a = mk((Kd, M) if a_mn else (M, Kd), 31, 0.3).bfloat16()
     b = mk((Kd, N) if b_mn else (N, Kd), 32, 0.3).bfloat16()
-    out = K().gemm(a, b, M, N, Kd, a_mn=a_mn, b_mn=b_mn, epi='f32', force_bn=bn, force_cluster=cluster,
-                   split_ok=a_mn and b_mn)
+    out = K().gemm(a, b, M, N, Kd, a_mn=a_mn, b_mn=b_mn, epi='f32', force_bn=bn, split_ok=a_mn and b_mn)
     torch.cuda.synchronize()
     assert rel(out, ref_mm(a, b, a_mn, b_mn)) < 1e-5
 
 
 @pytest.mark.parametrize('epi', ['bf16', 'f32res', 'gelu', 'dgelu'])
-def test_gemm_pair_kernel_epilogues(epi):
+def test_gemm_epilogues_partial_last_tile(epi):
+    """every epilogue with M = 1000: the last row of tiles holds 104 valid rows"""
     M, N, Kd = 1000, 512, 256
     a, b = mk((M, Kd), 41, 0.3).bfloat16(), mk((N, Kd), 42, 0.3).bfloat16()
     bias = mk((N,), 43)
     r = ref_mm(a, b, False, False)
     if epi == 'bf16':
-        out = K().gemm(a, b, M, N, Kd, epi='bf16', bias=bias, force_cluster=3)
+        out = K().gemm(a, b, M, N, Kd, epi='bf16', bias=bias)
         assert rel(out, r + bias) < 4e-3
     elif epi == 'f32res':
         aux = mk((M, N), 44)
         perm = torch.randperm(M).to(torch.int32).cuda()
         out = torch.zeros(M, N, device='cuda')
-        K().gemm(a, b, M, N, Kd, epi='f32', bias=bias, aux=aux, aux_row=perm, out_row=perm, out=out, force_cluster=3)
+        K().gemm(a, b, M, N, Kd, epi='f32', bias=bias, aux=aux, aux_row=perm, out_row=perm, out=out)
         exp = torch.zeros(M, N, device='cuda')
         exp[perm.long()] = r + bias + aux[perm.long()]
         assert rel(out, exp) < 1e-5
     elif epi == 'gelu':
-        z, h = K().gemm(a, b, M, N, Kd, epi='gelu', bias=bias, force_cluster=3)
+        z, h = K().gemm(a, b, M, N, Kd, epi='gelu', bias=bias)
         assert rel(z, r + bias) < 4e-3 and rel(h, torch.nn.functional.gelu(r + bias)) < 4e-3
     else:
         z = mk((M, N), 45).bfloat16()
-        out = K().gemm(a, b, M, N, Kd, epi='dgelu', aux=z, force_cluster=3)
+        out = K().gemm(a, b, M, N, Kd, epi='dgelu', aux=z)
         zz = z.float().requires_grad_(True)
         torch.nn.functional.gelu(zz).sum().backward()
         assert rel(out, r * zz.grad) < 4e-3
 
 
-# ---- round 2: fp32 residual epilogue on TMA (affine row maps through a tensor map of the token stream), narrow tail units ---
+# ---- fp32 residual epilogue with plain rows and affine row maps, short last row tiles, GELU / dGELU epilogues ----------
 def _ops():
     from videotransformer_pytorch_b200 import ops
     return ops
 
 
-@pytest.mark.parametrize('cluster', [1, 3], ids=['single-cta', 'cta-pair'])
 @pytest.mark.parametrize('bn', [0, 128, 192, 256])
-@pytest.mark.parametrize('M,N,Kd', [(1000, 768, 256), (12552, 768, 768), (130, 96, 192), (4096, 256, 64)])
-def test_residual_epilogue_tma_plain_rows(M, N, Kd, bn, cluster, monkeypatch):
-    """y = s(m) (A B^T + bias) + aux without row maps (FC2, joint proj): TMA residual path == generic per-thread path."""
-    if cluster == 3 and bn == 192:
-        pytest.skip('the pair kernel has no 192-wide tile')
+@pytest.mark.parametrize('M,N,Kd', [(1000, 768, 256), (12552, 768, 768), (130, 96, 192), (4096, 256, 64),
+                                    (12544, 768, 3072), (1568, 384, 128), (200, 136, 72)])
+def test_residual_epilogue_plain_rows_deterministic(M, N, Kd, bn):
+    """y = s(m) (A B^T + bias) + aux without row maps (FC2, joint proj) against torch, with full and partial row and column
+    tiles; a second call into a fresh output gives the same bits."""
     a, b = mk((M, Kd), 30).bfloat16(), mk((N, Kd), 31).bfloat16()
     bias, rs, aux = mk((N,), 32), mk((M,), 33), mk((M, N), 34)
     out = torch.full((M, N), 55.0, device='cuda')
-    monkeypatch.setenv('VT_TMA_RES', '1')
-    K().gemm(a, b, M, N, Kd, epi='f32', bias=bias, row_scale=rs, aux=aux, out=out, force_bn=bn, force_cluster=cluster)
+    K().gemm(a, b, M, N, Kd, epi='f32', bias=bias, row_scale=rs, aux=aux, out=out, force_bn=bn)
     r = (ref_mm(a, b, False, False) + bias) * rs[:, None] + aux
     assert rel(out, r) < 1e-5
-    monkeypatch.setenv('VT_TMA_RES', '0')
-    old = torch.empty_like(out)
-    K().gemm(a, b, M, N, Kd, epi='f32', bias=bias, row_scale=rs, aux=aux, out=old, force_bn=bn, force_cluster=cluster)
-    assert rel(out, old) < 1e-6
+    again = torch.empty_like(out)
+    K().gemm(a, b, M, N, Kd, epi='f32', bias=bias, row_scale=rs, aux=aux, out=again, force_bn=bn)
+    assert torch.equal(out, again)
 
 
-@pytest.mark.parametrize('cluster', [1, 3], ids=['single-cta', 'cta-pair'])
+@pytest.mark.parametrize('staged', ['0', '1'], ids=['register', 'staged'])
 @pytest.mark.parametrize('B,T,P,D', [(2, 8, 196, 768), (3, 4, 9, 128), (1, 2, 50, 256), (2, 8, 196, 96)])
-def test_residual_epilogue_tma_temporal_and_spatial_maps(B, T, P, D, cluster, monkeypatch):
-    """The divided space-time scatters as TMA boxes (temporal '(b p) t', spatial '(b t) (1+p)' with the per-frame cls
-    replicas going to side rows; 32-row groups that straddle a period go row by row) against the same GEMM driven by the
-    out_row / aux_row arrays alone (generic epilogue)."""
+def test_residual_epilogue_affine_maps_match_index_arrays(B, T, P, D, staged, monkeypatch):
+    """The divided space-time scatters given as affine row maps (temporal '(b p) t', spatial '(b t) (1+p)' with the
+    per-frame cls replicas going to side rows) against the same GEMM driven by the out_row / aux_row arrays alone, on the
+    register and on the staged fp32 epilogue."""
+    monkeypatch.setenv('VT_GEMM_STAGED_EPI', staged)
     ops = _ops()
     maps = ops.token_maps(B, T, P, 'cuda:0')
     aff = ops.affine_row_maps(B, T, P, D)
@@ -249,14 +242,10 @@ def test_residual_epilogue_tma_temporal_and_spatial_maps(B, T, P, D, cluster, mo
         a = mk((Mrows, Kd), 43).bfloat16()
         rs = mk((Mrows,), 44)
         got = torch.full((out_rows, D), -7.0, device='cuda')
-        monkeypatch.setenv('VT_TMA_RES', '1')
-        monkeypatch.setenv('VT_TMA_RES_SPATIAL', '1')
         K().gemm(a, w, Mrows, D, Kd, epi='f32', bias=bias, row_scale=rs, aux=x2, aux_row=aux_row, out=got, out_row=out_row,
-                 row_map=aff[name], force_cluster=cluster)
-        monkeypatch.setenv('VT_TMA_RES', '0')
+                 row_map=aff[name])
         exp = torch.full((out_rows, D), -7.0, device='cuda')
-        K().gemm(a, w, Mrows, D, Kd, epi='f32', bias=bias, row_scale=rs, aux=x2, aux_row=aux_row, out=exp, out_row=out_row,
-                 force_cluster=cluster)
+        K().gemm(a, w, Mrows, D, Kd, epi='f32', bias=bias, row_scale=rs, aux=x2, aux_row=aux_row, out=exp, out_row=out_row)
         assert rel(got, exp) < 1e-6, name
         # rows the map never names (the cls row of every sample) keep their old contents
         assert bool((got[torch.arange(B, device='cuda') * S] == -7.0).all()), name
@@ -267,12 +256,12 @@ def test_residual_epilogue_tma_temporal_and_spatial_maps(B, T, P, D, cluster, mo
         assert rel(got, full) < 1e-5, name
 
 
-@pytest.mark.parametrize('cluster', [0, 1, 3], ids=['auto', 'single-cta', 'cta-pair'])
 @pytest.mark.parametrize('M,N,Kd', [(12552, 768, 768), (12608, 2304, 256), (12552, 3072, 128), (136, 512, 192), (264, 256, 64)])
 @pytest.mark.parametrize('form', ['fwd_bf16', 'dgrad_bf16', 'fwd_f32_residual'])
-def test_narrow_tail_units(M, N, Kd, form, cluster, monkeypatch):
-    """A last row of tiles with <= 64 valid rows runs as narrow units (M = 12552 / 12608 of the FFN / spatial pass): same
-    results as with the feature off, and against fp32 torch."""
+@pytest.mark.parametrize('bn', [0, 128, 192, 256])
+def test_short_last_row_tile_deterministic(bn, M, N, Kd, form):
+    """A last row of tiles with <= 64 valid rows (M = 12552 / 12608 of the FFN / spatial pass), at the planner's tile width
+    (bn = 0) and at each forced one: against fp32 torch, and a second call gives the same bits."""
     a = mk((M, Kd), 50).bfloat16()
     bias, rs = mk((N,), 51), mk((M,), 52)
     if form == 'dgrad_bf16':
@@ -288,12 +277,11 @@ def test_narrow_tail_units(M, N, Kd, form, cluster, monkeypatch):
         aux = mk((M, N), 54)
         kw = dict(epi='f32', bias=bias, row_scale=rs, aux=aux)
         r = (a.float() @ b.float().t() + bias) * rs[:, None] + aux
-    monkeypatch.setenv('VT_TAIL_UNITS', '1')
-    got = K().gemm(a, b, M, N, Kd, force_cluster=cluster, force_tail=2, **kw)
-    off = K().gemm(a, b, M, N, Kd, force_cluster=cluster, force_tail=1, **kw)
+    got = K().gemm(a, b, M, N, Kd, force_bn=bn, **kw)
+    again = K().gemm(a, b, M, N, Kd, force_bn=bn, **kw)
     tol = 1e-5 if form == 'fwd_f32_residual' else 4e-3
     assert rel(got, r) < tol
-    assert torch.equal(got, off)
+    assert torch.equal(got, again)
 
 
 @pytest.mark.parametrize('M,N,Kd', [(12552, 768, 3072), (1032, 200, 2048), (1025, 768, 2304), (1040, 384, 4096), (12552, 3072, 768)])
@@ -333,39 +321,36 @@ def test_remainder_rows_split(M, N, Kd, form, monkeypatch):
     assert rel(got[m0:], one[m0:]) < (2e-5 if f32 else 8e-3)
 
 
-@pytest.mark.parametrize('cluster', [1, 3], ids=['single-cta', 'cta-pair'])
+@pytest.mark.parametrize('staged', ['0', '1'], ids=['register', 'staged'])
 @pytest.mark.parametrize('M,N,Kd', [(12552, 3072, 768), (1000, 512, 128), (130, 96, 64)])
-def test_gelu_and_dgelu_epilogues_on_tma(M, N, Kd, cluster, monkeypatch):
-    """FC1 with z / h = gelu(z) leaving as two TMA boxes, and the FC2 data gradient with gelu'(z) multiplied in from a
-    TMA-loaded z box: both equal the generic epilogues bit for bit and match torch."""
+def test_gelu_and_dgelu_epilogues_deterministic(M, N, Kd, staged, monkeypatch):
+    """FC1 with z and h = gelu(z) from one epilogue, and the FC2 data gradient with gelu'(z) multiplied in, on the register
+    and on the staged epilogue: both match torch, and a second call gives the same bits."""
+    monkeypatch.setenv('VT_GEMM_STAGED_EPI', staged)
     a, b = mk((M, Kd), 60, 0.3).bfloat16(), mk((N, Kd), 61, 0.3).bfloat16()
     bias = mk((N,), 62)
-    monkeypatch.setenv('VT_TMA_GELU', '1')
-    z, h = K().gemm(a, b, M, N, Kd, epi='gelu', bias=bias, force_cluster=cluster)
+    z, h = K().gemm(a, b, M, N, Kd, epi='gelu', bias=bias)
     zr = ref_mm(a, b, False, False) + bias
     assert rel(z, zr) < 4e-3 and rel(h, torch.nn.functional.gelu(zr)) < 4e-3
-    monkeypatch.setenv('VT_TMA_GELU', '0')
-    z0, _ = K().gemm(a, b, M, N, Kd, epi='gelu', bias=bias, force_cluster=cluster)
-    # h is taken from the bf16-rounded z: identical to the stand-alone GELU kernel on z (the generic fused epilogue rounds later)
-    assert torch.equal(z, z0) and torch.equal(h, K().gelu(z))
+    z_again, _ = K().gemm(a, b, M, N, Kd, epi='gelu', bias=bias)
+    # h is taken from the bf16-rounded z: identical to the stand-alone GELU kernel on z
+    assert torch.equal(z, z_again) and torch.equal(h, K().gelu(z))
     g = mk((M, Kd), 63, 0.3).bfloat16()
     w = mk((Kd, N), 64, 0.3).bfloat16()                       # [n_out = Kd, k_in = N], read MN-major
-    monkeypatch.setenv('VT_TMA_DGELU', '0')
-    d0 = K().gemm(g, w, M, N, Kd, b_mn=True, epi='dgelu', aux=z, force_cluster=cluster)
-    monkeypatch.setenv('VT_TMA_DGELU', '1')
-    d1 = K().gemm(g, w, M, N, Kd, b_mn=True, epi='dgelu', aux=z, force_cluster=cluster)
+    d = K().gemm(g, w, M, N, Kd, b_mn=True, epi='dgelu', aux=z)
+    d_again = K().gemm(g, w, M, N, Kd, b_mn=True, epi='dgelu', aux=z)
     zz = z.float().requires_grad_(True)
     torch.nn.functional.gelu(zz).sum().backward()
-    assert rel(d1, (g.float() @ w.float()) * zz.grad) < 4e-3
-    assert torch.equal(d0, d1)
+    assert rel(d_again, (g.float() @ w.float()) * zz.grad) < 4e-3
+    assert torch.equal(d, d_again)
 
 
-@pytest.mark.parametrize('res', ['0', '1'], ids=['generic-epilogue', 'tma-residual'])
+@pytest.mark.parametrize('staged', ['0', '1'], ids=['register', 'staged'])
 @pytest.mark.parametrize('M,N,Kd', [(12544, 768, 768), (1000, 256, 64), (12552, 768, 3072)])
-def test_second_bias_after_row_scale(M, N, Kd, res, monkeypatch):
+def test_second_bias_after_row_scale(M, N, Kd, staged, monkeypatch):
     """out = s(m) (A B^T + bias) + bias2 + aux: the bias of a second linear layer folded into the GEMM (merged proj +
-    temporal_fc), through the generic, the TMA-residual and the remainder-row paths."""
-    monkeypatch.setenv('VT_TMA_RES', res)
+    temporal_fc), on the register and on the staged fp32 epilogue."""
+    monkeypatch.setenv('VT_GEMM_STAGED_EPI', staged)
     a, b = mk((M, Kd), 70).bfloat16(), mk((N, Kd), 71).bfloat16()
     bias, bias2, rs, aux = mk((N,), 72), mk((N,), 73), mk((M,), 74), mk((M, N), 75)
     out = K().gemm(a, b, M, N, Kd, epi='f32', bias=bias, bias2=bias2, row_scale=rs, aux=aux)
@@ -373,15 +358,13 @@ def test_second_bias_after_row_scale(M, N, Kd, res, monkeypatch):
     assert rel(out, r) < 1e-5
 
 
+@pytest.mark.parametrize('init', [9.0, 0.0], ids=['stale', 'zeroed'])
 @pytest.mark.parametrize('M,N,Kd', [(768, 768, 12544), (2304, 768, 12608), (96, 448, 20000)])
-def test_split_k_into_a_prezeroed_output(M, N, Kd):
-    """Weight-gradient form (both operands MN-major, split-K by TMA reduce-add): with out_zeroed the library skips its own
-    memset and accumulates into what the caller zeroed (gradient arena / DDP bucket); without it stale contents are harmless."""
+def test_split_k_into_a_prezeroed_output(M, N, Kd, init):
+    """Weight-gradient form (both operands MN-major, split-K): the output is written in full, so a stale-filled and a
+    zero-filled output both end up equal to the product."""
     a, b = mk((Kd, M), 80).bfloat16(), mk((Kd, N), 81).bfloat16()
     r = a.float().t() @ b.float()
-    stale = torch.full((M, N), 9.0, device='cuda')
-    K().gemm(a, b, M, N, Kd, a_mn=True, b_mn=True, epi='f32', split_ok=True, out=stale)
-    assert rel(stale, r) < 1e-5
-    zeroed = torch.zeros((M, N), device='cuda')
-    K().gemm(a, b, M, N, Kd, a_mn=True, b_mn=True, epi='f32', split_ok=True, out=zeroed, out_zeroed=True)
-    assert rel(zeroed, r) < 1e-5
+    out = torch.full((M, N), init, device='cuda')
+    K().gemm(a, b, M, N, Kd, a_mn=True, b_mn=True, epi='f32', split_ok=True, out=out)
+    assert rel(out, r) < 1e-5

@@ -342,10 +342,12 @@ def test_exact_persistent_walk(form, M, N, Kd, tb, monkeypatch):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize('bn', [128, 192, 256])
-def test_exact_split_k(bn, monkeypatch):
+@pytest.mark.parametrize('zeroed', [False, True], ids=['sentinel', 'zeroed'])
+def test_exact_split_k(zeroed, bn, monkeypatch):
     """weight-gradient form (both operands MN-major) with forced splits that do not divide the k-block count: partials
-    through the workspace, summed into a stale output and into a pre-zeroed one (out_zeroed).  The kernels these calls
-    take are the cells of test_exact_cell with one split; test_gpu_gemm_staged_f32 checks which one a split call picks."""
+    through the workspace, summed into a sentinel-filled output and into a zeroed one: prior contents never matter.  The
+    kernels these calls take are the cells of test_exact_cell with one split; test_gpu_gemm_staged_f32 checks which one a
+    split call picks."""
     for M, N, Kd, splits in ((776, 200, 12552, (2, 5, 16)), (768, 768, 3072, (5, 7)), (136, 72, 584, (3,))):
         A, B, a, b = int_operands(M, N, Kd, 1, 1, seed=M + Kd, pad=8)
         X.exact_premise(Kd)
@@ -355,15 +357,14 @@ def test_exact_split_k(bn, monkeypatch):
             assert kb % sp, (kb, sp)
             for staged in (0, 1):
                 monkeypatch.setenv('VT_GEMM_STAGED_EPI', str(staged))
-                for zeroed in (False, True):
-                    buf = torch.zeros((M + 3, N), device='cuda') if zeroed else \
-                        torch.full((M + 3, N), SENT32, dtype=torch.int32, device='cuda').view(torch.float32)
-                    tail = buf[M:].clone()
-                    K().gemm(a, b, M, N, Kd, a_mn=True, b_mn=True, epi='f32', split_ok=True, force_splits=sp,
-                             force_bn=bn, out=buf[:M], out_zeroed=zeroed)
-                    tag = (M, N, Kd, sp, bn, staged, zeroed)
-                    assert torch.equal(buf[:M].view(torch.int32), ref.view(torch.int32)), tag
-                    assert torch.equal(buf[M:].view(torch.int32), tail.view(torch.int32)), tag
+                buf = torch.zeros((M + 3, N), device='cuda') if zeroed else \
+                    torch.full((M + 3, N), SENT32, dtype=torch.int32, device='cuda').view(torch.float32)
+                tail = buf[M:].clone()
+                K().gemm(a, b, M, N, Kd, a_mn=True, b_mn=True, epi='f32', split_ok=True, force_splits=sp,
+                         force_bn=bn, out=buf[:M])
+                tag = (M, N, Kd, sp, bn, staged, zeroed)
+                assert torch.equal(buf[:M].view(torch.int32), ref.view(torch.int32)), tag
+                assert torch.equal(buf[M:].view(torch.int32), tail.view(torch.int32)), tag
 
 
 @pytest.mark.gpu

@@ -30,9 +30,13 @@ def test_graphed_step_matches_eager_and_tracks_weight_updates():
     step = GraphedTrainStep(net, (x, y))
     for trial in range(2):
         x2 = torch.randn(2, 4, 3, 48, 48).cuda()
+        for g in step.static_grads:              # no gradient may depend on what its storage held before the replay
+            g.fill_(float('nan'))
         torch.manual_seed(123 + trial)
         loss_g = float(step(x2, y).detach())
         gg = {n: p.grad.clone() for n, p in net.named_parameters()}
+        nonfinite = [n for n, g in gg.items() if not bool(torch.isfinite(g).all())]
+        assert not nonfinite, nonfinite
         for p in net.parameters():
             p.grad = None
         torch.manual_seed(123 + trial)

@@ -366,15 +366,14 @@ class CudaKernels:
     # -- GEMM ---------------------------------------------------------------------------------
     def gemm(self, a, b, M, N, Kdim, *, a_mn=False, b_mn=False, epi='bf16', bias=None, bias2=None, out=None, out2=None,
              aux=None, out_row=None, aux_row=None, row_scale=None, out_rows=None, split_ok=False,
-             force_splits=0, force_bn=0, force_cluster=0, debug=None, row_map=None, force_tail=0, tag=None, out_zeroed=False):
-        """row_map: affine description of out_row / aux_row (ops.affine_row_maps) for the fp32 residual epilogue — lets the
-        kernel move 32 x 32 boxes by TMA through a tensor map of the token stream instead of per-thread rows.  tag: role label of the launch
+             force_splits=0, force_bn=0, row_map=None, tag=None):
+        """row_map: affine description of out_row / aux_row (ops.affine_row_maps) for the fp32 residual epilogue — the kernel
+        computes each row's output and residual addresses from it instead of reading the index arrays.  tag: role label of the launch
         ('qkv', 'proj', ...) for profilers that wrap this method (bench.py); ignored here."""
         p, out, out2 = self._gemm_params(a, b, M, N, Kdim, torch.bfloat16, a_mn=a_mn, b_mn=b_mn, epi=epi, bias=bias, bias2=bias2,
                                          out=out, out2=out2, aux=aux, out_row=out_row, aux_row=aux_row, row_scale=row_scale,
                                          out_rows=out_rows, split_ok=split_ok, force_splits=force_splits, force_bn=force_bn,
-                                         force_cluster=force_cluster, debug=debug, row_map=row_map, force_tail=force_tail,
-                                         out_zeroed=out_zeroed)
+                                         row_map=row_map)
         _check(load_library().vt_gemm(C.byref(p), _stream()), 'vt_gemm')
         return (out, out2) if epi == 'gelu' else out
 
@@ -418,7 +417,7 @@ class CudaKernels:
 
     def _gemm_params(self, a, b, M, N, Kdim, op_dtype, *, a_mn=False, b_mn=False, epi='bf16', bias=None, bias2=None, out=None,
                      out2=None, aux=None, out_row=None, aux_row=None, row_scale=None, out_rows=None, split_ok=False,
-                     force_splits=0, force_bn=0, force_cluster=0, debug=None, row_map=None, force_tail=0, out_zeroed=False):
+                     force_splits=0, force_bn=0, row_map=None):
         """vt_gemm_params of one call (operands of dtype op_dtype), with the output allocated when not given."""
         _rows2d(_req(a, op_dtype, 'gemm.a'), 'gemm.a')
         _rows2d(_req(b, op_dtype, 'gemm.b'), 'gemm.b')
@@ -462,10 +461,7 @@ class CudaKernels:
         if split_ok and epi == 'f32':
             ws = self.workspace(a.device, 16 * M * N * 4)
             p.workspace, p.workspace_bytes = ws.data_ptr(), ws.numel() * 4
-        p.force_splits, p.force_bn, p.force_cluster = force_splits, force_bn, force_cluster
-        p.force_tail = force_tail
-        p.out_zeroed = int(bool(out_zeroed) and out is not None)
-        p.debug = _ptr(debug)
+        p.force_splits, p.force_bn = force_splits, force_bn
         p.map_special_base = -1
         if row_map is not None:
             if epi != 'f32' or aux is None:

@@ -93,7 +93,7 @@ class GradientBuckets:
         self._pending = [len(ps) for ps in self._bucket_params]
 
     def reset_counters(self):
-        """CUDA-graph replays run no Python hooks: the captured graph already contains the zeroing and the
+        """CUDA-graph replays run no Python hooks: the captured graph already contains the gradient writes and the
         all-reduces in the right order; only the host-side bookkeeping is reset."""
         self._pending = [0 for _ in self._bucket_params]
 
@@ -142,23 +142,19 @@ class GradientBuckets:
             self._arrived[bi] = []
             self._launch(bi)
 
-    def backward_into_buckets(self, loss, params, zero_first=False):
+    def backward_into_buckets(self, loss, params):
         """Backward of `loss` with the gradients landing in the flat buckets and every bucket's all-reduce issued as soon as
-        it is complete (the body of a captured data-parallel step, graph.GraphedTrainStep; also usable eagerly after
-        zero_grad()).  Uses torch.autograd.grad, so nothing is ACCUMULATED: weight-gradient GEMMs may therefore write
-        directly into their bucket slice (ops.GRAD_DEST), other gradients are copied in by grad_ready().
-        zero_first: zero the buckets here (16 memsets, part of a captured step) and let the split-K weight-gradient GEMMs
-        skip their own per-output memsets (73 per TimeSformer-B step)."""
+        it is complete (the body of a captured data-parallel step, graph.GraphedTrainStep; also usable eagerly while every
+        p.grad is its bucket view, as zero_grad() leaves it).  Uses torch.autograd.grad, so nothing is ACCUMULATED:
+        weight-gradient GEMMs may therefore write directly into their bucket slice (ops.GRAD_DEST), other gradients are
+        copied in by grad_ready().  Every parameter's slice is overwritten in full, so the buckets need no zeroing first."""
         from . import ops
         params = list(params)
         self._pending = [len(ps) for ps in self._bucket_params]
         self._arrived = [[] for _ in self._bucket_params]
         handles = [p.register_hook(lambda g, p=p: self.grad_ready(p, g)) for p in params]
         if self.direct_wgrad:
-            if zero_first:
-                for b in self.buckets:
-                    b.zero_()
-            ops.set_grad_destinations({p.data_ptr(): v for p, v in self._view.items()}, zeroed=zero_first)
+            ops.set_grad_destinations({p.data_ptr(): v for p, v in self._view.items()})
         try:
             grads = torch.autograd.grad(loss, params)
         finally:

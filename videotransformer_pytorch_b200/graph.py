@@ -68,7 +68,7 @@ class GraphedTrainStep:
 
     loss_fn : callable taking the input tensors and returning a scalar loss (typically an nn.Module whose
               forward computes the loss); its parameters' .grad are (re)written by every call.
-    reducer : optional ddp.GradientBuckets — zeroing and the bucket all-reduces become part of the graph.
+    reducer : optional ddp.GradientBuckets — the bucket all-reduces become part of the graph.
     """
 
     def __init__(self, loss_fn: Callable, example_inputs: Sequence[torch.Tensor], reducer=None,
@@ -99,13 +99,6 @@ class GraphedTrainStep:
         torch.cuda.synchronize(dev)
 
         from . import _lib
-        if reducer is None:
-            mats = [p for p in self.params if p.dim() >= 2]
-            self._grad_arena = torch.zeros(sum((p.numel() + 3) // 4 * 4 for p in mats), dtype=torch.float32, device=dev)
-            self._grad_views, off = {}, 0
-            for p in mats:                      # 16-byte aligned slices (TMA stores)
-                self._grad_views[p.data_ptr()] = self._grad_arena[off:off + p.numel()]
-                off += (p.numel() + 3) // 4 * 4
         self.graph = torch.cuda.CUDAGraph()
         launches_before = _lib.launch_count()
         self._zero(set_to_none=True)
@@ -118,19 +111,13 @@ class GraphedTrainStep:
                 # captured kernels.  (.backward() would route them through per-parameter AccumulateGrad nodes, which
                 # are bound to the stream they were first created on and may execute outside the capture.)
                 if reducer is None:
-                    # weight gradients land in one flat arena zeroed by a single memset per step (their split-K GEMMs
-                    # accumulate by TMA reduce-add and would otherwise zero each output themselves: 73 memsets)
-                    self._grad_arena.zero_()
-                    ops.set_grad_destinations(self._grad_views, zeroed=True)
-                    try:
-                        grads = torch.autograd.grad(self.static_loss, self.params)
-                    finally:
-                        ops.set_grad_destinations(None)
+                    # the gradients are allocated in the graph's private pool, so every replay rewrites the same tensors
+                    grads = torch.autograd.grad(self.static_loss, self.params)
                 else:
                     # per-parameter tensor hooks fire as soon as a gradient is final: weight gradients are written by
                     # their GEMM straight into the flat buckets, the rest is copied there, and completed buckets are
                     # all-reduced on the side stream while backward continues
-                    grads = reducer.backward_into_buckets(self.static_loss, self.params, zero_first=True)
+                    grads = reducer.backward_into_buckets(self.static_loss, self.params)
         finally:
             self.arena.recording = False
             ops.set_mask_arena(None)

@@ -187,28 +187,24 @@ def drop_path_scale(p: float, training: bool, n0: int, repeat: int, device):
 
 
 # While a data-parallel step is being captured (graph.GraphedTrainStep with ddp.GradientBuckets) this maps the address of a
-# weight parameter to its slice of the flat gradient bucket: the weight-gradient GEMM then writes (zero + split-K TMA
-# reduce-add) straight into the bucket and no gather copy precedes the all-reduce (SURVEY C1).  Never set in eager mode,
-# where autograd ACCUMULATES the returned gradient into p.grad — returning p.grad's own storage would double it.
+# weight parameter to its slice of the flat gradient bucket: the weight-gradient GEMM then writes straight into the bucket
+# and no gather copy precedes the all-reduce (SURVEY C1).  The GEMM writes every element of its destination (split-K
+# partials are summed in a workspace), so whatever the slice held before never matters.  Never set in eager mode, where
+# autograd ACCUMULATES the returned gradient into p.grad — returning p.grad's own storage would double it.
 GRAD_DEST = None
-GRAD_DEST_ZEROED = False
 
 
-def set_grad_destinations(table, zeroed=False):
-    """table: {parameter data_ptr: fp32 view the weight-gradient GEMM of that parameter writes to} or None.
-    zeroed: the views were zeroed after the previous backward (one memset of the arena / buckets per step), so the split-K
-    GEMMs skip their own per-output memset."""
-    global GRAD_DEST, GRAD_DEST_ZEROED
+def set_grad_destinations(table):
+    """table: {parameter data_ptr: fp32 view the weight-gradient GEMM of that parameter writes to} or None."""
+    global GRAD_DEST
     GRAD_DEST = table
-    GRAD_DEST_ZEROED = bool(zeroed) and table is not None
 
 
 def _wgrad(dout, act, n_out, k_in, m_tok, tag=None, wptr=None):
     """dW[n_out, k_in] = dout[m_tok, n_out]^T @ act[m_tok, k_in]  (both operands MN-major, split-K).
     wptr: data_ptr() of the fp32 parameter this is the gradient of (see GRAD_DEST)."""
-    out = _grad_dest(wptr, n_out, k_in)
-    return K().gemm(dout, act, n_out, k_in, m_tok, a_mn=True, b_mn=True, epi='f32', split_ok=True, tag=tag, out=out,
-                    out_zeroed=out is not None and GRAD_DEST_ZEROED)
+    return K().gemm(dout, act, n_out, k_in, m_tok, a_mn=True, b_mn=True, epi='f32', split_ok=True, tag=tag,
+                    out=_grad_dest(wptr, n_out, k_in))
 
 
 def _grad_dest(wptr, n_out, k_in):
