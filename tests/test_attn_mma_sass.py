@@ -1,5 +1,6 @@
 """Compiler-side checks of the tensor-core attention kernels (csrc/vt_attention_mma.cu); they need nvcc / cuobjdump, no GPU.
-Every instantiation loads its tiles with cp.async (LDGSTS) and its MMA fragments with ldmatrix (LDSM), and none spills."""
+Every instantiation loads its tiles with cp.async (LDGSTS) and its MMA fragments with ldmatrix (LDSM), none spills, and
+the head-dim-64 dK / dV kernel keeps the three CTAs per SM it is launched for."""
 import os
 import re
 import shutil
@@ -30,7 +31,9 @@ def test_attention_kernels_use_cp_async_and_ldmatrix():
         assert 'HMMA' in body, name
 
 
-def test_attention_kernels_do_not_spill():
+@pytest.fixture(scope='module')
+def ptxas_stats():
+    """{kernel: (spill store bytes, spill load bytes, registers)} of the tiled kernels, from ptxas -v"""
     from videotransformer_pytorch_b200 import build
     try:
         nvcc = build.nvcc_path()
@@ -44,7 +47,18 @@ def test_attention_kernels_do_not_spill():
     log = res.stdout + res.stderr
     assert res.returncode == 0, log
     kernels = re.findall(r"Compiling entry function '(\w*attn_mma_\w*)'[^\n]*\n(?:[^\n]*\n)?[^\n]*?(\d+) bytes spill stores, "
-                         r"(\d+) bytes spill loads", log)
+                         r"(\d+) bytes spill loads[^\n]*\n[^\n]*Used (\d+) registers", log)
     assert len(kernels) == 8, log
-    spilling = [k for k, st, ld in kernels if int(st) or int(ld)]
+    return {k: (int(st), int(ld), int(regs)) for k, st, ld, regs in kernels}
+
+
+def test_attention_kernels_do_not_spill(ptxas_stats):
+    spilling = [k for k, (st, ld, _) in ptxas_stats.items() if st or ld]
     assert not spilling, spilling
+
+
+def test_dkv_kernel_hd64_keeps_three_ctas_per_sm(ptxas_stats):
+    """__launch_bounds__(128, 3): three CTAs of 128 threads share the 64K-register file, registers allocated per thread
+    in multiples of 8"""
+    (name, (_, _, regs)), = [(k, v) for k, v in ptxas_stats.items() if 'attn_mma_dkv_kernelILi64' in k]
+    assert 3 * 128 * (-(-regs // 8) * 8) <= 65536, (name, regs)
