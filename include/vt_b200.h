@@ -356,6 +356,19 @@ typedef struct {
   int32_t B, T, C, H, W, kt, kh, kw, st, sh, sw, pt, ph, pw, To, Ho, Wo, Kpad;
 } vt_im2col3d_params;
 int vt_im2col3d_bf16(const vt_im2col3d_params* p, void* stream);
+/* The same operand from the decoder's uint8 clip x [B,T,H,W,C] (channels last), in the reference's order:
+ *   ToTensor + Normalize (data_transform.py:62-64, :534-539), v = ((u / 255) - mean[c]) / std[c], each op rounded to
+ *   nearest in fp32 (bit for bit the reference's float clip);
+ *   then the batch-level Mixup / CutMix of mixup.py:102-114 against sample B-1-b when plan != NULL (plan = device
+ *   float[6] {mode, lam, yl, yh, xl, xh} as in vt_im2col_u8_mix_params; mode 1: v*lam + o*(1-lam) with (1-lam) taken
+ *   in fp32, mode 2: o inside rows [yl,yh) x cols [xl,xh));
+ *   then the transpose and Conv3d zero padding (video_transformer.py:912): a tap outside the clip is 0 in normalised space.
+ *   Each value is rounded to bf16 once, after the blend.  cols as in vt_im2col3d_bf16 (16-byte aligned, Kpad % 8 == 0). */
+typedef struct {
+  const uint8_t* x; const float* mean; const float* std; const float* plan; void* cols;
+  int32_t B, T, C, H, W, kt, kh, kw, st, sh, sw, pt, ph, pw, To, Ho, Wo, Kpad;
+} vt_im2col3d_u8_params;
+int vt_im2col3d_u8_bf16(const vt_im2col3d_u8_params* p, void* stream);
 
 /* Token preparation (MaskFeat.forward_features :915-919 + SpatioTemporalClsPositionalEncoding):
  *   x[b,0,:]   = cls_token + pos_cls

@@ -181,9 +181,16 @@ class MaxpoolBwdParams(C.Structure):
     _fields_ = [('dy', c_vp), ('idx', c_vp), ('dx', c_vp)] + _MP_DIMS
 
 
+_I3_DIMS = [(n, c_i32) for n in ('B', 'T', 'C', 'H', 'W', 'kt', 'kh', 'kw', 'st', 'sh', 'sw', 'pt', 'ph', 'pw', 'To', 'Ho', 'Wo',
+                                  'Kpad')]
+
+
 class Im2col3dParams(C.Structure):
-    _fields_ = [('x', c_vp), ('cols', c_vp)] + [(n, c_i32) for n in (
-        'B', 'T', 'C', 'H', 'W', 'kt', 'kh', 'kw', 'st', 'sh', 'sw', 'pt', 'ph', 'pw', 'To', 'Ho', 'Wo', 'Kpad')]
+    _fields_ = [('x', c_vp), ('cols', c_vp)] + _I3_DIMS
+
+
+class Im2col3dU8Params(C.Structure):
+    _fields_ = [('x', c_vp), ('mean', c_vp), ('std', c_vp), ('plan', c_vp), ('cols', c_vp)] + _I3_DIMS
 
 
 class MvitTokensFwdParams(C.Structure):
@@ -285,7 +292,7 @@ EXPORTS = ['vt_version', 'vt_last_error', 'vt_sm_count', 'vt_set_reserved_sms', 
            'vt_cls_rows', 'vt_gather_cast_colsum_blocks', 'vt_gather_cast_colsum_bf16', 'vt_gelu_bwd_colsum_blocks', 'vt_gelu_bwd_colsum_bf16',
            'vt_gather_cast_bf16', 'vt_gelu_fwd_bf16', 'vt_gelu_bwd_bf16', 'vt_attn_fwd', 'vt_attn_bwd', 'vt_im2col_bf16', 'vt_im2col_u8_bf16', 'vt_col2im_f32', 'vt_hog',
            'vt_pool_fwd', 'vt_pool_bwd_scratch', 'vt_pool_bwd', 'vt_xattn_fwd', 'vt_xattn_bwd', 'vt_maxpool_fwd',
-           'vt_maxpool_bwd', 'vt_im2col3d_bf16', 'vt_mvit_tokens_fwd', 'vt_mvit_tokens_bwd', 'vt_mse_blocks',
+           'vt_maxpool_bwd', 'vt_im2col3d_bf16', 'vt_im2col3d_u8_bf16', 'vt_mvit_tokens_fwd', 'vt_mvit_tokens_bwd', 'vt_mse_blocks',
            'vt_mse_fwd', 'vt_mse_bwd', 'vt_opt_norm2', 'vt_opt_sgd', 'vt_opt_adamw',
            'vt_linear_small_fwd', 'vt_linear_small_bwd', 'vt_softmax_ce', 'vt_scale_by_scalar',
            'vt_im2col_u8_mix_bf16', 'vt_pos_resize_fwd', 'vt_pos_resize_bwd', 'vt_topk_hits',
@@ -1128,6 +1135,34 @@ class CudaKernels:
         p.To, p.Ho, p.Wo = out
         p.Kpad = kpad
         _check(lib.vt_im2col3d_bf16(C.byref(p), _stream()), 'vt_im2col3d_bf16')
+        return cols, out
+
+    def im2col3d_u8(self, x, mean, std, plan, kernel, stride, padding, kpad):
+        """x u8 [B,T,H,W,C] -> (cols bf16 [B*To*Ho*Wo, kpad], (To,Ho,Wo)): im2col3d of the normalised clip, mixed against
+        the flipped batch when plan (fp32 [6] device tensor {mode, lam, yl, yh, xl, xh}) is given"""
+        lib = load_library()
+        x = _req(x, torch.uint8, 'im2col3d_u8.x').contiguous()
+        if x.dim() != 5:
+            raise RuntimeError(f'im2col3d_u8: expected a [B, T, H, W, C] clip, got shape {tuple(x.shape)}')
+        B, T, H, W, Cc = x.shape
+        mean = _req(mean, torch.float32, 'im2col3d_u8.mean').contiguous()
+        std = _req(std, torch.float32, 'im2col3d_u8.std').contiguous()
+        if mean.numel() != Cc or std.numel() != Cc:
+            raise RuntimeError(f'im2col3d_u8: mean and std must hold {Cc} floats')
+        if plan is not None and (plan.numel() < 6 or not plan.is_contiguous()):
+            raise RuntimeError('im2col3d_u8: plan must hold 6 contiguous floats {mode, lam, yl, yh, xl, xh}')
+        out = tuple((n + 2 * pd - k) // s + 1 for n, pd, k, s in zip((T, H, W), padding, kernel, stride))
+        cols = torch.empty((B * out[0] * out[1] * out[2], kpad), dtype=torch.bfloat16, device=x.device)
+        p = Im2col3dU8Params()
+        p.x, p.mean, p.std, p.cols = x.data_ptr(), mean.data_ptr(), std.data_ptr(), cols.data_ptr()
+        p.plan = None if plan is None else _req(plan, torch.float32, 'im2col3d_u8.plan').data_ptr()
+        p.B, p.T, p.C, p.H, p.W = B, T, Cc, H, W
+        p.kt, p.kh, p.kw = kernel
+        p.st, p.sh, p.sw = stride
+        p.pt, p.ph, p.pw = padding
+        p.To, p.Ho, p.Wo = out
+        p.Kpad = kpad
+        _check(lib.vt_im2col3d_u8_bf16(C.byref(p), _stream()), 'vt_im2col3d_u8_bf16')
         return cols, out
 
     def mvit_tokens_fwd(self, t, wmask, mask_token, cls_token, pos_s, pos_t, pos_cls, B, T, HW):

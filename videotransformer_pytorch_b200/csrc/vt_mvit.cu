@@ -1014,6 +1014,96 @@ __global__ void im2col3d_kernel(const float* __restrict__ x, __nv_bfloat16* __re
   }
 }
 
+// The same operand from the decoder's uint8 clip [B, T, H, W, C].  One CTA owns the output rows (b, ot, oh0..oh0+ohb-1):
+//   1. it stages the C x kt x R source lines those rows read (R = (ohb-1)*sh + kh) in shared memory as bf16
+//      [c][dt][r][Wp], Wp = W + 2*pw: normalised, mixed and rounded once per CTA, each line widened by pw zeros per side
+//      and lines outside the clip all zeros, so the gather below has no bounds tests;
+//   2. its rows of cols are one contiguous span (rows are ow-, then oh-major), written with 16-byte stores, consecutive
+//      threads on consecutive chunks; a column -> window offset table (-1 = pad column) replaces the per-element
+//      (c, dt, dh, dw) decode.
+struct I3U8Dims {
+  I3Dims g;
+  int ohb, R, Wp, Kreal;
+};
+
+// ToTensor + Normalize as the reference runs them in fp32 (pic.float().div(255), then sub_(mean).div_(std)): no
+// contraction, no reciprocal, so the value is bit for bit the reference's float clip
+__device__ __forceinline__ float u8_normalize(uint8_t u, float mean, float std) {
+  return __fdiv_rn(__fsub_rn(__fdiv_rn((float)u, 255.f), mean), std);
+}
+
+__global__ void __launch_bounds__(256) im2col3d_u8_kernel(const uint8_t* __restrict__ x, const float* __restrict__ mean,
+                                                          const float* __restrict__ stdv, const float* __restrict__ plan,
+                                                          __nv_bfloat16* __restrict__ cols, I3U8Dims u) {
+  extern __shared__ __align__(16) unsigned char i3u8_smem[];
+  const I3Dims& d = u.g;
+  int* tab = reinterpret_cast<int*>(i3u8_smem);                          // [Kpad]
+  __nv_bfloat16* win = reinterpret_cast<__nv_bfloat16*>(tab + d.Kpad);  // [C][kt][R][Wp]
+  const int hblocks = (d.Ho + u.ohb - 1) / u.ohb;
+  const int hb = blockIdx.x % hblocks;
+  const int ot = (blockIdx.x / hblocks) % d.To;
+  const int b = blockIdx.x / (hblocks * d.To);
+  const int oh0 = hb * u.ohb;
+  const int noh = min(u.ohb, d.Ho - oh0);
+  int mode = 0, yl = 0, yh = 0, xl = 0, xh = 0;
+  float lam = 1.f;
+  if (plan) {
+    mode = (int)plan[0];
+    lam = plan[1];
+    yl = (int)plan[2], yh = (int)plan[3], xl = (int)plan[4], xh = (int)plan[5];
+  }
+  const float lam_o = __fsub_rn(1.0f, lam);
+
+  for (int k = threadIdx.x; k < d.Kpad; k += blockDim.x) {
+    int off = -1;
+    if (k < u.Kreal) {
+      const int dw = k % d.kw, dh = (k / d.kw) % d.kh, dt = (k / (d.kw * d.kh)) % d.kt, c = k / (d.kw * d.kh * d.kt);
+      off = ((c * d.kt + dt) * u.R + dh) * u.Wp + dw;
+    }
+    tab[k] = off;
+  }
+  const long long clip = (long long)d.T * d.H * d.W * d.C;
+  const uint8_t* xs = x + b * clip;
+  const uint8_t* xf = x + (d.B - 1 - b) * clip;                          // x.flip(0)[b]
+  const int staged = d.C * d.kt * u.R * u.Wp;
+  for (int e = threadIdx.x; e < staged; e += blockDim.x) {
+    const int xw = e % u.Wp, line = e / u.Wp;
+    const int r = line % u.R, dt = (line / u.R) % d.kt, c = line / (u.R * d.kt);
+    const int ti = ot * d.st - d.pt + dt, hi = oh0 * d.sh - d.ph + r, wi = xw - d.pw;
+    float v = 0.f;                                                       // Conv3d padding: 0 after Normalize
+    if (ti >= 0 && ti < d.T && hi >= 0 && hi < d.H && wi >= 0 && wi < d.W) {
+      const long long o = (((long long)ti * d.H + hi) * d.W + wi) * d.C + c;
+      const float m = mean[c], s = stdv[c];
+      v = u8_normalize(xs[o], m, s);
+      if (mode == 1) {
+        v = __fadd_rn(__fmul_rn(v, lam), __fmul_rn(u8_normalize(xf[o], m, s), lam_o));   // x*lam + x.flip(0)*(1-lam)
+      } else if (mode == 2 && hi >= yl && hi < yh && wi >= xl && wi < xh) {
+        v = u8_normalize(xf[o], m, s);                                   // x[..., yl:yh, xl:xh] = x.flip(0)[...]
+      }
+    }
+    win[e] = __float2bfloat16_rn(v);
+  }
+  __syncthreads();
+
+  const int cpr = d.Kpad / 8;                                            // 16-byte chunks per row
+  const long long row0 = (((long long)b * d.To + ot) * d.Ho + oh0) * d.Wo;
+  uint4* dst = reinterpret_cast<uint4*>(cols + row0 * d.Kpad);
+  const int chunks = noh * d.Wo * cpr;
+  const __nv_bfloat16 zero = __float2bfloat16_rn(0.f);
+  for (int q = threadIdx.x; q < chunks; q += blockDim.x) {
+    const int rl = q / cpr, k0 = (q - rl * cpr) * 8;
+    const int ohl = rl / d.Wo, ow = rl - ohl * d.Wo;
+    const __nv_bfloat16* src = win + ohl * d.sh * u.Wp + ow * d.sw;
+    __align__(16) __nv_bfloat16 h[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int off = tab[k0 + j];
+      h[j] = off >= 0 ? src[off] : zero;
+    }
+    dst[q] = *reinterpret_cast<const uint4*>(h);
+  }
+}
+
 // ================================================================================================
 // token preparation
 // ================================================================================================
@@ -1454,6 +1544,46 @@ extern "C" int vt_im2col3d_bf16(const vt_im2col3d_params* p, void* stream) {
   const long long n = (long long)p->B * p->To * p->Ho * p->Wo * ((p->Kpad + p->kw - 1) / p->kw);
   im2col3d_kernel<<<flat_blocks(n, 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(p->x, static_cast<__nv_bfloat16*>(p->cols), d);
   return check_launch("im2col3d_kernel");
+}
+
+extern "C" int vt_im2col3d_u8_bf16(const vt_im2col3d_u8_params* p, void* stream) {
+  VT_REQUIRE(p && p->x && p->mean && p->std && p->cols, "vt_im2col3d_u8_bf16: null pointer");
+  VT_REQUIRE(p->B > 0 && p->T > 0 && p->C > 0 && p->H > 0 && p->W > 0 && p->kt > 0 && p->kh > 0 && p->kw > 0 && p->st > 0 &&
+                 p->sh > 0 && p->sw > 0 && p->pt >= 0 && p->ph >= 0 && p->pw >= 0, "vt_im2col3d_u8_bf16: bad dims");
+  VT_REQUIRE(p->To == (p->T + 2 * p->pt - p->kt) / p->st + 1 && p->Ho == (p->H + 2 * p->ph - p->kh) / p->sh + 1 &&
+                 p->Wo == (p->W + 2 * p->pw - p->kw) / p->sw + 1 && p->To > 0 && p->Ho > 0 && p->Wo > 0,
+             "vt_im2col3d_u8_bf16: output dims inconsistent");
+  const int kreal = p->C * p->kt * p->kh * p->kw;
+  VT_REQUIRE(p->Kpad >= kreal && p->Kpad % 8 == 0, "vt_im2col3d_u8_bf16: Kpad must cover C*kt*kh*kw and be a multiple of 8");
+  VT_REQUIRE(reinterpret_cast<uintptr_t>(p->cols) % 16 == 0, "vt_im2col3d_u8_bf16: cols must be 16-byte aligned");
+  const int Wp = p->W + 2 * p->pw;
+  auto smem_for = [&](int ohb) {
+    return (size_t)p->Kpad * sizeof(int) + (size_t)p->C * p->kt * ((ohb - 1) * p->sh + p->kh) * Wp * sizeof(__nv_bfloat16);
+  };
+  // rows per CTA: the most that keep the window within the default 48 KB (fewer source lines staged twice); one row
+  // may take up to I3U8_SMEM_MAX
+  constexpr size_t I3U8_SMEM_DEFAULT = 48 * 1024, I3U8_SMEM_MAX = 200 * 1024;
+  int ohb = 4;
+  while (ohb > 1 && smem_for(ohb) > I3U8_SMEM_DEFAULT) ohb /= 2;
+  const size_t smem = smem_for(ohb);
+  VT_REQUIRE(smem <= I3U8_SMEM_MAX, "vt_im2col3d_u8_bf16: the staged window (%zu bytes for W=%d, C=%d, kt=%d, kh=%d) does not fit in shared memory",
+             smem, p->W, p->C, p->kt, p->kh);
+  if (smem > I3U8_SMEM_DEFAULT) {
+    static size_t max_set = I3U8_SMEM_DEFAULT;
+    if (smem > max_set) {
+      cudaError_t e = cudaFuncSetAttribute(im2col3d_u8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)I3U8_SMEM_MAX);
+      VT_REQUIRE(e == cudaSuccess, "vt_im2col3d_u8_bf16: smem attribute: %s", cudaGetErrorString(e));
+      max_set = I3U8_SMEM_MAX;
+    }
+  }
+  const long long blocks = (long long)p->B * p->To * ((p->Ho + ohb - 1) / ohb);
+  VT_REQUIRE(blocks <= 0x7fffffffLL, "vt_im2col3d_u8_bf16: grid too large");
+  const I3U8Dims u{{p->B, p->T, p->C, p->H, p->W, p->kt, p->kh, p->kw, p->st, p->sh, p->sw, p->pt, p->ph, p->pw, p->To, p->Ho,
+                    p->Wo, p->Kpad},
+                   ohb, (ohb - 1) * p->sh + p->kh, Wp, kreal};
+  im2col3d_u8_kernel<<<(unsigned)blocks, 256, smem, static_cast<cudaStream_t>(stream)>>>(
+      p->x, p->mean, p->std, p->plan, static_cast<__nv_bfloat16*>(p->cols), u);
+  return check_launch("im2col3d_u8_kernel");
 }
 
 extern "C" int vt_mvit_tokens_fwd(const vt_mvit_tokens_fwd_params* p, void* stream) {

@@ -21,6 +21,7 @@ import torch.nn as nn
 from . import mvit_ops, ops
 from .ops import RowsNormFn
 from .transformer import InferencePrecision, ShadowWeights, _f32
+from .video_transformer import _ByteClipInput
 
 HEAD_DIM = 96   # the kernels are specialised for MViT-B's head width (patch_embed_dim 96, heads double with dim)
 
@@ -207,9 +208,12 @@ def create_multiscale_vision_transformers(*, spatial_size, temporal_size, depth=
     return MultiscaleVisionTransformers(pos, blocks, nn.LayerNorm(plan[-1]['dim_out'], eps=1e-6))
 
 
-class MaskFeat(InferencePrecision, nn.Module):
+class MaskFeat(_ByteClipInput, InferencePrecision, nn.Module):
     """forward(x[B,T,3,H,W], target_x[B,T,h,w,dc], mask[B,t,h,w], cube_marker) -> (pred[B,T,h,w,dc], loss);
-    forward_features(x, mask=None) -> [B, 1+t*h*w, embed_dims]."""
+    forward_features(x, mask=None) -> [B, 1+t*h*w, embed_dims].
+
+    x may also be the decoder's uint8 clip [B, T, H, W, 3] on the device, or a mixup.MixedClip wrapping one: ToTensor,
+    Normalize (set_input_normalization) and Mixup / CutMix then happen inside the Conv3d patch-operand kernel."""
 
     def __init__(self, img_size=224, num_frames=16, input_channels=3, feature_dim=10, patch_embed_dim=96,
                  conv_patch_embed_kernel=(3, 7, 7), conv_patch_embed_stride=(2, 4, 4), conv_patch_embed_padding=(1, 3, 3),
@@ -255,9 +259,14 @@ class MaskFeat(InferencePrecision, nn.Module):
 
     # ------------------------------------------------------------------------------------------
     def forward_features(self, x, mask=None):
-        if x.dim() != 5 or x.shape[1] != self.num_frames or x.shape[-1] != self.img_size or x.shape[-2] != self.img_size:
-            raise RuntimeError(f'MaskFeat: expected [B, {self.num_frames}, C, {self.img_size}, {self.img_size}], got {tuple(x.shape)}')
+        x, norm, plan = self._unwrap_clip(x, mean_std=True)
         conv = self.patch_embed.patch_model
+        n, s, c = self.num_frames, self.img_size, conv.in_channels
+        if norm is not None:
+            if x.dim() != 5 or tuple(x.shape[1:]) != (n, s, s, c):
+                raise RuntimeError(f'MaskFeat: expected a uint8 clip [B, {n}, {s}, {s}, {c}], got {tuple(x.shape)}')
+        elif x.dim() != 5 or x.shape[1] != n or x.shape[-1] != s or x.shape[-2] != s:
+            raise RuntimeError(f'MaskFeat: expected [B, {n}, C, {s}, {s}], got {tuple(x.shape)}')
         pos = self.mvit.cls_positional_encoding
         T, H, W = pos.patch_embed_shape
         B = x.shape[0]
@@ -271,7 +280,7 @@ class MaskFeat(InferencePrecision, nn.Module):
         x0 = ops.run(
             mvit_ops.ConvTokensFn, x, _f32(conv.weight), _f32(conv.bias), _f32(self.mask_token), _f32(pos.cls_token), _f32(pos.pos_embed_spatial),
             _f32(pos.pos_embed_temporal), _f32(pos.pos_embed_class), wmask,
-            self._shadow.get_padded('conv', conv.weight, kpad), (self.kernel, self.stride, self.padding))
+            self._shadow.get_padded('conv', conv.weight, kpad), (self.kernel, self.stride, self.padding), norm, plan)
         return self.mvit(x0)
 
     def center_frame_mask(self, mask, cube_marker):

@@ -8,9 +8,9 @@ Two input kinds:
   * float clips [B,T,C,H,W] / [B,C,H,W] (the reference's path, after CPU normalisation): mixed in place with the same
     tensor ops as the reference; returns (x, soft_target).
   * uint8 clips [B,T,H,W,3] straight from the decoder (SURVEY §8f rank 2): nothing is touched here — the draw is
-    packaged as a `MixedClip` (clip + a 6-float device plan) that TimeSformer / ViViT consume; the blend with the flipped
-    batch then happens inside the patch-operand kernel (`vt_im2col_u8_mix_bf16`) together with ToTensor + Normalize, so
-    the mixed fp32 clip never exists in memory.
+    packaged as a `MixedClip` (clip + a 6-float device plan) that TimeSformer / ViViT / MaskFeat consume; the blend with
+    the flipped batch then happens inside the patch-operand kernel (`vt_im2col_u8_mix_bf16`, `vt_im2col3d_u8_bf16`)
+    together with ToTensor + Normalize, so the mixed fp32 clip never exists in memory.
 """
 from __future__ import annotations
 

@@ -40,15 +40,22 @@ def _bhnd(view, H, hd):
 
 
 class ConvTokensFn(torch.autograd.Function):
-    """x0[b,0] = cls + pos_cls;  x0[b,1+l] = conv3d(x)[b,l]*(1-w) + mask_token*w + pos_s[l%HW] + pos_t[l//HW]."""
+    """x0[b,0] = cls + pos_cls;  x0[b,1+l] = conv3d(x)[b,l]*(1-w) + mask_token*w + pos_s[l%HW] + pos_t[l//HW].
+
+    x is the float clip [B, T, C, H, W], or the decoder's uint8 clip [B, T, H, W, C] with norm = (mean, std) device
+    tensors and an optional Mixup / CutMix plan (mixup.MixedClip.plan): the operand kernel then normalises and mixes."""
 
     @staticmethod
-    def forward(ctx, x, conv_w, conv_b, mask_token, cls_token, pos_s, pos_t, pos_cls, wmask, conv_wh, geom):
+    def forward(ctx, x, conv_w, conv_b, mask_token, cls_token, pos_s, pos_t, pos_cls, wmask, conv_wh, geom, norm=None,
+                plan=None):
         k = K()
         kernel, stride, padding = geom
         C0 = conv_w.shape[0]
         kpad = conv_wh.shape[1]
-        cols, (To, Ho, Wo) = k.im2col3d(x.float(), kernel, stride, padding, kpad)
+        if x.dtype == torch.uint8:
+            cols, (To, Ho, Wo) = k.im2col3d_u8(x, norm[0], norm[1], plan, kernel, stride, padding, kpad)
+        else:
+            cols, (To, Ho, Wo) = k.im2col3d(x.float(), kernel, stride, padding, kpad)
         B = x.shape[0]
         M = cols.shape[0]
         t = k.gemm(cols, conv_wh, M, C0, kpad, bias=conv_b, epi='f32')
@@ -84,7 +91,7 @@ class ConvTokensFn(torch.autograd.Function):
         else:
             d_mask = torch.zeros(mshape, dtype=dx0.dtype, device=dx0.device)
         return (None, d_w.contiguous(), d_b, d_mask, d_cls.reshape(cshape).clone(), d_pos_s, d_pos_t,
-                d_cls.reshape(pcshape).clone(), None, None, None)
+                d_cls.reshape(pcshape).clone(), None, None, None, None, None)
 
 
 class PoolAttnFn(torch.autograd.Function):

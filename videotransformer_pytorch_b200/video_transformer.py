@@ -43,22 +43,39 @@ class _ByteClipInput:
         does it on the CPU: data_transform.py ToTensor + Normalize with data_trainer.py:69-73's mean / std)."""
         self._input_norm = (tuple(float(m) for m in mean), tuple(float(s) for s in std))
         self._input_norm_dev = None
+        self._input_mean_std_dev = None
+
+    def input_normalization(self):
+        """(mean, std) tuples applied to uint8 clips; (0.45,) * 3 and (0.225,) * 3 until set_input_normalization."""
+        return getattr(self, '_input_norm', ((0.45, 0.45, 0.45), (0.225, 0.225, 0.225)))
 
     def _norm_tensors(self, device):
         cached = getattr(self, '_input_norm_dev', None)
         if cached is None or cached[0].device != device:
-            mean, std = getattr(self, '_input_norm', ((0.45, 0.45, 0.45), (0.225, 0.225, 0.225)))
+            mean, std = self.input_normalization()
             scale = torch.tensor([1.0 / (255.0 * s) for s in std], dtype=torch.float32, device=device)
             shift = torch.tensor([-m / s for m, s in zip(mean, std)], dtype=torch.float32, device=device)
             cached = self._input_norm_dev = (scale, shift)
         return cached
 
-    def _unwrap_clip(self, x):
-        """-> (tensor, (scale, shift) | None, mix plan | None)"""
+    def input_mean_std(self, device):
+        """The normalisation as fp32 device tensors (mean [C], std [C]), for kernels that apply the reference's
+        (u / 255 - mean) / std op by op."""
+        cached = getattr(self, '_input_mean_std_dev', None)
+        if cached is None or cached[0].device != device:
+            mean, std = self.input_normalization()
+            cached = self._input_mean_std_dev = (torch.tensor(mean, dtype=torch.float32, device=device),
+                                                 torch.tensor(std, dtype=torch.float32, device=device))
+        return cached
+
+    def _unwrap_clip(self, x, mean_std=False):
+        """-> (tensor, (scale, shift) | None, mix plan | None); (mean, std) in place of (scale, shift) when mean_std"""
         plan = None
         if isinstance(x, MixedClip):
             x, plan = x.clip, x.plan
-        norm = self._norm_tensors(x.device) if x.dtype == torch.uint8 else None
+        norm = None
+        if x.dtype == torch.uint8:
+            norm = self.input_mean_std(x.device) if mean_std else self._norm_tensors(x.device)
         if plan is not None and norm is None:
             raise RuntimeError('MixedClip must wrap a uint8 clip (float clips are mixed by Mixup.__call__ itself)')
         return x, norm, plan
