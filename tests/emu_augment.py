@@ -1,5 +1,5 @@
-"""CPU twin of vt_resized_crop_u8 / vt_color_jitter_u8 for the host-logic tests: the kernel table of tests/emu_eval.py plus
-an fp32 restatement of both kernels' arithmetic (every product, sum and quotient rounded separately, as the kernels do
+"""CPU twin of vt_resized_crop_u8 / vt_color_jitter_u8 (EmuKernels in tests/emu_kernels.py runs it): an fp32
+restatement of both kernels' arithmetic (every product, sum and quotient rounded separately, as the kernels do
 with __fmul_rn / __fadd_rn / __fdiv_rn), so the twin gives the kernels' bytes.  TEST INFRASTRUCTURE ONLY."""
 from __future__ import annotations
 
@@ -7,8 +7,6 @@ import ctypes as C
 
 import numpy as np
 import torch
-
-from tests.emu_eval import EmuKernelsEval
 
 f32 = np.float32
 
@@ -94,24 +92,3 @@ def parse(desc, cls, n):
     raw = desc.cpu().numpy().tobytes()
     return [cls.from_buffer_copy(raw, k * C.sizeof(cls)) for k in range(n)]
 
-
-class EmuKernelsAugment(EmuKernelsEval):
-    def resized_crop_u8(self, src, desc, out, err=None):
-        from videotransformer_pytorch_b200 import _lib
-        n, T, S = out.shape[:3]
-        self.calls.append(('resized_crop_u8', n, T, S))
-        flat = src.cpu().numpy()
-        for k, d in enumerate(parse(desc, _lib.CropDesc, n)):
-            frames = flat[d.src_offset:d.src_offset + T * d.H * d.W * 3].reshape(T, d.H, d.W, 3)
-            out[k] = resize_window(frames, (d.crop_y, d.crop_x, d.crop_h, d.crop_w), (d.RH, d.RW), (d.oy, d.ox), S,
-                                   d.filter, d.flip)
-        return out
-
-    def color_jitter_u8(self, frames, desc):
-        from videotransformer_pytorch_b200 import _lib
-        n = frames.shape[0]
-        self.calls.append(('color_jitter_u8', n))
-        for k, d in enumerate(parse(desc, _lib.JitterDesc, n)):
-            ops = [(d.op[s], d.factor[s], d.one_minus[s]) for s in range(d.n_ops)]
-            frames[k] = jitter_frames(frames[k], ops)
-        return frames

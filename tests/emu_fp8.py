@@ -1,5 +1,5 @@
-"""CPU twin of the fp8 inference forms (vt_quant_rows_e4m3, vt_gemm_e4m3) for the host-logic tests and as the quantising
-fp64 model of the GPU tests.  TEST INFRASTRUCTURE ONLY.
+"""CPU twin of the fp8 inference forms (vt_quant_rows_e4m3, vt_gemm_e4m3; EmuKernels in tests/emu_kernels.py runs it with
+fp8_forms=True) for the host-logic tests and as the quantising fp64 model of the GPU tests.  TEST INFRASTRUCTURE ONLY.
 
 The quantiser's scale is a power of two, so x / scale is exact and the only rounding is the cast to e4m3 (round to nearest
 even, saturating at +-448).  `quant_rows_twin` takes that cast from torch (clamp first: torch turns values past +-448 into
@@ -9,7 +9,6 @@ from __future__ import annotations
 
 import torch
 
-from tests.emu_eval import EmuKernelsEval
 from videotransformer_pytorch_b200._lib import E4M3
 
 E4M3_MAX = 448.0
@@ -57,19 +56,3 @@ def quant_rows_twin(x: torch.Tensor) -> E4M3:
 def dequant(t: E4M3, dtype=torch.float64) -> torch.Tensor:
     return t.q.to(dtype) * t.scale.to(dtype)[:, None]
 
-
-class EmuKernelsFp8(EmuKernelsEval):
-    """The forward-only twin plus the e4m3 forms: quant_rows_e4m3 is the twin above, gemm_e4m3 dequantises both operands
-    (exact: e4m3 values times powers of two) and runs the emulated GEMM with the same epilogue.  Calls are recorded as
-    ('quant_e4m3', M, K) and ('gemm_e4m3', M, N, K, ..., epi)."""
-    fp8_forms = True
-
-    def quant_rows_e4m3(self, x):
-        self.calls.append(('quant_e4m3',) + tuple(x.shape))
-        return quant_rows_twin(x)
-
-    def gemm_e4m3(self, a, b, M, N, Kdim, *, epi='bf16', **kw):
-        assert isinstance(a, E4M3) and isinstance(b, E4M3) and epi in ('bf16', 'f32', 'gelu_h')
-        out = self.gemm(dequant(a, self.f), dequant(b, self.f), M, N, Kdim, epi=epi, **kw)
-        self.calls[-1] = ('gemm_e4m3',) + self.calls[-1][1:]
-        return out

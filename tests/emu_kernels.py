@@ -7,6 +7,13 @@ goldens on a box without a GPU.  It mirrors each kernel's *contract* (include/vt
 ops; set `exact=True` to skip bf16 rounding (then results match the fp64 goldens to ~1e-6 in fp32 /
 1e-12 in fp64, which pins the host logic independent of kernel precision).
 The product package never imports this file.
+
+Every method has the name, parameters and defaults of its CudaKernels counterpart (tests/test_abi.py checks this).  The
+two capabilities ops.run asks a table for are constructor flags, off by default so that the `emu` fixture's table takes
+the saving (autograd) forms: `inference_forms` (the 'gelu_h' epilogue and the calls that leave their backward-only
+outputs unwritten) and `fp8_forms` (the e4m3 GEMM and row quantiser).  Calls that tests inspect are appended to `calls`,
+one record per call, led by the method's name; a forward form's record carries whether the backward-only outputs were
+asked for as its second field.
 """
 from __future__ import annotations
 
@@ -14,13 +21,31 @@ import math
 
 import torch
 
+from tests.emu_augment import jitter_frames, parse, resize_window
+from tests.emu_fp8 import dequant, quant_rows_twin
+from tests.emu_randaug import desc_ops, randaug_frames
+from videotransformer_pytorch_b200 import _lib
+
+
+def bicubic_rows(rows, grid, out_grid, scales):
+    """fp64 F.interpolate(mode='bicubic', align_corners=False, scale_factor=scales) of the row-major grid
+    rows [gh*gw, D] -> [oh*ow, D]"""
+    import torch.nn.functional as F
+    D = rows.shape[1]
+    g = rows.reshape(grid[0], grid[1], D).permute(2, 0, 1)[None]
+    y = F.interpolate(g, scale_factor=tuple(scales), mode='bicubic', align_corners=False)
+    assert tuple(y.shape[-2:]) == tuple(out_grid), (y.shape, out_grid)
+    return y[0].permute(1, 2, 0).reshape(-1, D)
+
 
 class EmuKernels:
     name = 'emu'
 
-    def __init__(self, exact=False, dtype=torch.float32):
+    def __init__(self, exact=False, dtype=torch.float32, *, inference_forms=False, fp8_forms=False):
         self.exact = exact
         self.f = dtype          # "fp32" storage type of the emulation (float64 for exact host-logic checks)
+        self.inference_forms = inference_forms
+        self.fp8_forms = fp8_forms
         self.calls = []
 
     # storage type standing in for bf16
@@ -85,18 +110,38 @@ class EmuKernels:
             else:
                 acc = acc + self._up(aux)
         val = acc.to(self.f) if epi == 'f32' else self._h(acc)
-        if out is None:
+        dst = None if epi == 'gelu_h' else out          # gelu_h: h from the bf16-rounded z, like the kernel
+        if dst is None:
             rows = out_rows if out_rows is not None else M
-            out = torch.empty((rows, N), dtype=val.dtype)
+            dst = torch.empty((rows, N), dtype=val.dtype)
         if out_row is not None:
             orow = self._idx(out_row)
             ok = orow >= 0
-            out[orow[ok]] = val[ok].to(out.dtype)
+            dst[orow[ok]] = val[ok].to(dst.dtype)
         else:
-            out[:M] = val.to(out.dtype)
+            dst[:M] = val.to(dst.dtype)
+        if epi == 'gelu_h':
+            h = self._gelu(dst)
+            return h if out is None else out.copy_(h)
+        return dst
+
+    def gemm_e4m3(self, a, b, M, N, Kdim, *, epi='bf16', bias=None, bias2=None, out=None, aux=None, out_row=None,
+                  aux_row=None, row_scale=None, out_rows=None, force_bn=0, row_map=None, tag=None):
+        """Dequantises both operands (exact: e4m3 values times powers of two) and runs the emulated GEMM with the same
+        epilogue."""
+        assert isinstance(a, _lib.E4M3) and isinstance(b, _lib.E4M3) and epi in ('bf16', 'f32', 'gelu_h')
+        out = self.gemm(dequant(a, self.f), dequant(b, self.f), M, N, Kdim, epi=epi, bias=bias, bias2=bias2, out=out, aux=aux,
+                        out_row=out_row, aux_row=aux_row, row_scale=row_scale, out_rows=out_rows, force_bn=force_bn,
+                        row_map=row_map, tag=tag)
+        self.calls[-1] = ('gemm_e4m3',) + self.calls[-1][1:]
         return out
 
-    def ln_fwd(self, x2d, gamma, beta, eps, in_row=None, rows=None, out_fp32=False):
+    def quant_rows_e4m3(self, x):
+        self.calls.append(('quant_rows_e4m3',) + tuple(x.shape))
+        return quant_rows_twin(x)
+
+    def ln_fwd(self, x2d, gamma, beta, eps, in_row=None, rows=None, out_fp32=False, stats=True):
+        self.calls.append(('ln_fwd', stats))
         x = self._up(x2d)
         if in_row is not None:
             x = x[self._idx(in_row)]
@@ -106,7 +151,8 @@ class EmuKernels:
         var = ((x - mu) ** 2).mean(-1, keepdim=True)
         rstd = torch.rsqrt(var + eps)
         y = (x - mu) * rstd * self._up(gamma) + self._up(beta)
-        return (y.to(self.f) if out_fp32 else self._h(y)), mu[:, 0].to(self.f), rstd[:, 0].to(self.f)
+        y = y.to(self.f) if out_fp32 else self._h(y)
+        return (y, mu[:, 0].to(self.f), rstd[:, 0].to(self.f)) if stats else (y, None, None)
 
     def ln_bwd(self, dy, x2d, mean, rstd, gamma, in_row=None, out_row=None, dres=None, dx=None, n_aux=0):
         x = self._up(x2d)
@@ -157,6 +203,10 @@ class EmuKernels:
         return self._h(v)
 
     def gelu(self, z):
+        self.calls.append(('gelu',))
+        return self._gelu(z)
+
+    def _gelu(self, z):
         zz = self._up(z)
         return self._h(0.5 * zz * (1 + torch.erf(zz / math.sqrt(2.0))))
 
@@ -183,17 +233,17 @@ class EmuKernels:
         pdf = torch.exp(-0.5 * zz * zz) / math.sqrt(2 * math.pi)
         return self._h(self._up(dh) * (cdf + zz * pdf))
 
-    def attn_fwd(self, qkv, Bp, N, H, hd, scale, want_probs=False, impl=0):
-        self.calls.append(('attn', 'fwd', N))
+    def attn_fwd(self, qkv, Bp, N, H, hd, scale, want_probs=False, impl=0, want_lse=True):
+        self.calls.append(('attn_fwd', want_lse, N))
         q = self._up(qkv).reshape(Bp, N, 3, H, hd).permute(2, 0, 3, 1, 4)
         s = (q[0] @ q[1].transpose(-1, -2)) * scale
         lse = torch.logsumexp(s, dim=-1)
         p = torch.exp(s - lse[..., None])
         o = (p @ q[2]).transpose(1, 2).reshape(Bp * N, H * hd)
-        return self._h(o), lse.to(self.f), (p.to(self.f) if want_probs else None)
+        return self._h(o), (lse.to(self.f) if want_lse else None), (p.to(self.f) if want_probs else None)
 
     def attn_bwd(self, qkv, ctx, dctx, lse, Bp, N, H, hd, scale, impl=0):
-        self.calls.append(('attn', 'bwd', N))
+        self.calls.append(('attn_bwd', N))
         q = self._up(qkv).reshape(Bp, N, 3, H, hd).permute(2, 0, 3, 1, 4)
         Q, Kk, V = q[0], q[1], q[2]
         O = self._up(ctx).reshape(Bp, N, H, hd).transpose(1, 2)
@@ -260,6 +310,79 @@ class EmuKernels:
         xx = self._up(cols).reshape(B, Tp, Hp, Wp, C, tube, ph, pw).permute(0, 1, 5, 4, 2, 6, 3, 7)
         return xx.reshape(shape).to(self.f)
 
+    def topk_hits(self, logits, labels, views, ks, hits, samples, probs=None):
+        self.calls.append(('topk_hits', views, tuple(ks)))
+        B = labels.numel()
+        C = logits.shape[1]
+        z = logits.float().reshape(B, views, C)
+        m = z[:, 0]
+        for v in range(1, views):                           # views summed in order, then scaled by fp32 1/V (as the kernel does)
+            m = m + z[:, v]
+        m = m * torch.tensor(1.0 / views, dtype=torch.float32)
+        ok = (labels >= 0) & (labels < C)
+        ml = m.gather(1, labels.clamp(0, C - 1).reshape(B, 1))
+        rank = (m > ml).sum(1)
+        rank = torch.where(ok & ~torch.isnan(ml[:, 0]), rank, torch.full_like(rank, C))
+        for i, k in enumerate(ks):
+            hits[i] += int((rank < k).sum())
+        samples[0] += B
+        if probs is not None:
+            probs.copy_(m.softmax(-1))
+
+    def forward_only_calls(self):
+        """The recorded calls that show a forward-only form: gelu_h GEMMs and calls without their statistics."""
+        return [c for c in self.calls if (c[0] == 'gemm' and c[-1] == 'gelu_h') or
+                (c[0] in ('ln_fwd', 'attn_fwd', 'xattn_fwd', 'pool_fwd', 'maxpool_fwd') and c[1] is False)]
+
+    # ------------------------------------------------------------------------------------------
+    # positional-embedding resize: fp64 F.interpolate and its autograd
+    # ------------------------------------------------------------------------------------------
+    def pos_resize_fwd(self, src, grid, out_grid, scales, out=None):
+        self.calls.append(('pos_resize_fwd', tuple(grid), tuple(out_grid)))
+        y = bicubic_rows(src.double(), grid, out_grid, scales).to(self.f)
+        return y if out is None else out.copy_(y)
+
+    def pos_resize_bwd(self, dout, grid, out_grid, scales, out=None):
+        self.calls.append(('pos_resize_bwd', tuple(grid), tuple(out_grid)))
+        with torch.enable_grad():
+            x = torch.zeros(grid[0] * grid[1], dout.shape[1], dtype=torch.float64, requires_grad=True)
+            (gx,) = torch.autograd.grad(bicubic_rows(x, grid, out_grid, scales), x, dout.double())
+        gx = gx.to(self.f)
+        return gx if out is None else out.copy_(gx)
+
+    # ------------------------------------------------------------------------------------------
+    # clip transforms: the fp32 restatements of tests/emu_augment.py and tests/emu_randaug.py
+    # ------------------------------------------------------------------------------------------
+    def resized_crop_u8(self, src, desc, out, err=None):
+        n, T, S = out.shape[:3]
+        self.calls.append(('resized_crop_u8', n, T, S))
+        flat = src.cpu().numpy()
+        for k, d in enumerate(parse(desc, _lib.CropDesc, n)):
+            frames = flat[d.src_offset:d.src_offset + T * d.H * d.W * 3].reshape(T, d.H, d.W, 3)
+            out[k] = resize_window(frames, (d.crop_y, d.crop_x, d.crop_h, d.crop_w), (d.RH, d.RW), (d.oy, d.ox), S,
+                                   d.filter, d.flip)
+        return out
+
+    def color_jitter_u8(self, frames, desc):
+        n = frames.shape[0]
+        self.calls.append(('color_jitter_u8', n))
+        for k, d in enumerate(parse(desc, _lib.JitterDesc, n)):
+            ops = [(d.op[s], d.factor[s], d.one_minus[s]) for s in range(d.n_ops)]
+            frames[k] = jitter_frames(frames[k], ops)
+        return frames
+
+    def rand_augment_u8(self, frames, desc, err=None):
+        n = frames.shape[0]
+        self.calls.append(('rand_augment_u8', n))
+        for k, d in enumerate(parse(desc, _lib.RandAugDesc, n)):
+            if not 0 <= d.n_ops <= _lib.RANDAUG_MAX_OPS or any(not 0 <= d.op[s] < 14 for s in range(d.n_ops)):
+                frames[k] = 0
+                if err is not None:
+                    err.fill_(1)
+                continue
+            frames[k] = randaug_frames(frames[k], desc_ops(d))
+        return frames
+
     # ------------------------------------------------------------------------------------------
     # MViT / MaskFeat kernels (include/vt_b200.h, second half)
     # ------------------------------------------------------------------------------------------
@@ -287,11 +410,14 @@ class EmuKernels:
         out = (pooled - mu) * rstd * gamma + beta
         return out, pooled, mu, rstd
 
-    def pool_fwd(self, src, H, hd, thw, stride, w, gamma, beta, eps):
+    def pool_fwd(self, src, H, hd, thw, stride, w, gamma, beta, eps, stats=True):
+        self.calls.append(('pool_fwd', stats))
         out, pooled, mu, rstd = self._pool_core(self._up(src), H, hd, thw, stride, self._up(w), self._up(gamma),
                                                 self._up(beta), eps)
-        return self._h(out), pooled.to(self.f), mu.reshape(-1).to(self.f), rstd.reshape(-1).to(self.f), \
-            self.pool_out_thw(thw, stride)
+        thw_o = self.pool_out_thw(thw, stride)
+        if not stats:
+            return self._h(out), None, None, None, thw_o
+        return self._h(out), pooled.to(self.f), mu.reshape(-1).to(self.f), rstd.reshape(-1).to(self.f), thw_o
 
     def pool_bwd(self, dout, pooled, mean, rstd, gamma, src, w, din, H, hd, thw, stride):
         shp = pooled.shape[:-1] + (1,)
@@ -310,15 +436,15 @@ class EmuKernels:
         din.copy_(self._h(gx).to(din.dtype))
         return gw.reshape(hd, 27).to(self.f), (d * xh).sum((0, 1, 2)).to(self.f), d.sum((0, 1, 2)).to(self.f)
 
-    def xattn_fwd(self, q, k, v, scale, impl=0):
-        self.calls.append(('xattn', tuple(q.shape), k.shape[2]))
+    def xattn_fwd(self, q, k, v, scale, impl=0, want_lse=True):
+        self.calls.append(('xattn_fwd', want_lse, tuple(q.shape), k.shape[2]))
         Q, Kk, V = self._up(q), self._up(k), self._up(v)
         B, H, Nq, hd = Q.shape
         s = (Q @ Kk.transpose(-1, -2)) * scale
         lse = torch.logsumexp(s, dim=-1)
         p = torch.exp(s - lse[..., None])
         o = (p @ V).transpose(1, 2).reshape(B, Nq, H * hd)
-        return self._h(o), lse.to(self.f)
+        return self._h(o), (lse.to(self.f) if want_lse else None)
 
     def xattn_bwd(self, q, k, v, o, dout, lse, scale, dq, impl=0):
         Q, Kk, V = self._up(q), self._up(k), self._up(v)
@@ -334,8 +460,9 @@ class EmuKernels:
         dq.copy_(self._h(dS @ Kk).to(dq.dtype))
         return (dS.transpose(-1, -2) @ Q).to(self.f), dV.to(self.f)
 
-    def maxpool_fwd(self, x, thw, kernel, stride):
+    def maxpool_fwd(self, x, thw, kernel, stride, want_idx=True):
         import torch.nn.functional as F
+        self.calls.append(('maxpool_fwd', want_idx))
         B, L1, D = x.shape
         T, H, W = thw
         xx = self._up(x)
@@ -343,7 +470,7 @@ class EmuKernels:
         y, idx = F.max_pool3d(vol, tuple(kernel), tuple(stride), tuple(k // 2 for k in kernel), return_indices=True)
         out_thw = tuple(y.shape[2:])
         yy = torch.cat([xx[:, :1], y.reshape(B, D, -1).transpose(1, 2)], dim=1)
-        return yy.to(self.f), idx.reshape(B, D, -1), out_thw        # idx is opaque to the host logic
+        return yy.to(self.f), (idx.reshape(B, D, -1) if want_idx else None), out_thw        # idx is opaque to the host logic
 
     def maxpool_bwd(self, dy, idx, thw, kernel, stride):
         B, Lo1, D = dy.shape
@@ -362,6 +489,24 @@ class EmuKernels:
         cols = u.permute(0, 2, 3, 4, 1, 5, 6, 7).reshape(B * To * Ho * Wo, -1)
         cols = F.pad(cols, (0, kpad - cols.shape[1]))
         return self._h(cols), (To, Ho, Wo)
+
+    def im2col3d_u8(self, x, mean, std, plan, kernel, stride, padding, kpad):
+        """Twin of vt_im2col3d_u8_bf16, with its rounding points: every op below is one fp32 op rounded to nearest (torch
+        on the CPU contracts nothing): ToTensor u / 255, Normalize (. - mean) / std, Mixup v*lam + o*(1 - lam) with
+        (1 - lam) in fp32, CutMix a copy; then zero padding and one bf16 rounding in im2col3d."""
+        f32 = torch.float32
+        v = (x.to(f32) / 255.0 - mean.to(f32).view(1, 1, 1, 1, -1)) / std.to(f32).view(1, 1, 1, 1, -1)   # [B,T,H,W,C]
+        if plan is not None:
+            plan = plan.to('cpu', f32)
+            mode = int(plan[0])
+            if mode == 1:
+                lam = plan[1]
+                v = v * lam + v.flip(0) * (torch.ones((), dtype=f32) - lam)
+            elif mode == 2:
+                yl, yh, xl, xh = (int(t) for t in plan[2:6])
+                v = v.clone()
+                v[:, :, yl:yh, xl:xh] = v.flip(0)[:, :, yl:yh, xl:xh]
+        return self.im2col3d(v.permute(0, 1, 4, 2, 3), kernel, stride, padding, kpad)
 
     def mvit_tokens_fwd(self, t, wmask, mask_token, cls_token, pos_s, pos_t, pos_cls, B, T, HW):
         C = t.shape[1]

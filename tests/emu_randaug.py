@@ -1,5 +1,5 @@
-"""CPU twin of vt_rand_augment_u8 for the host-logic tests: the kernel table of tests/emu_augment.py plus an fp32
-restatement of the kernel's arithmetic (every product and sum of the warp coordinates rounded separately, in the kernel's
+"""CPU twin of vt_rand_augment_u8 (EmuKernels in tests/emu_kernels.py runs it): an fp32 restatement of the kernel's
+arithmetic (every product and sum of the warp coordinates rounded separately, in the kernel's
 order; the sharpness blur in exact integers; statistics per frame and channel), so the twin gives the kernel's bytes.
 TEST INFRASTRUCTURE ONLY."""
 from __future__ import annotations
@@ -7,7 +7,7 @@ from __future__ import annotations
 import numpy as np
 import torch
 
-from tests.emu_augment import EmuKernelsAugment, blend_u8, jitter_frames, parse
+from tests.emu_augment import blend_u8, jitter_frames
 
 f32 = np.float32
 GEOMETRIC, SHARPNESS = (1, 2, 3, 4, 5), 9
@@ -132,17 +132,3 @@ def randaug_frames(frames, ops):
 def desc_ops(d):
     return [(d.op[s], d.arg[s], d.one_minus[s], list(d.theta[s])) for s in range(d.n_ops)]
 
-
-class EmuKernelsRandAug(EmuKernelsAugment):
-    def rand_augment_u8(self, frames, desc, err=None):
-        from videotransformer_pytorch_b200 import _lib
-        n = frames.shape[0]
-        self.calls.append(('rand_augment_u8', n))
-        for k, d in enumerate(parse(desc, _lib.RandAugDesc, n)):
-            if not 0 <= d.n_ops <= _lib.RANDAUG_MAX_OPS or any(not 0 <= d.op[s] < 14 for s in range(d.n_ops)):
-                frames[k] = 0
-                if err is not None:
-                    err.fill_(1)
-                continue
-            frames[k] = randaug_frames(frames[k], desc_ops(d))
-        return frames

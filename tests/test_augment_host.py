@@ -1,18 +1,14 @@
 """GPU clip transforms, host side, on the CPU: the restated parameter draws against torchvision's get_params, the kernels'
 fp32 twin (tests/emu_augment.py) against torchvision's jitter (bit for bit) and F.interpolate's resize (within the stated
 pre-rounding bound), the whole host path under emulation against the reference goldens (oracle/make_augment_golden.py),
-descriptor packing of mixed sizes, and the C struct layouts."""
-import ctypes
-import os
-import shutil
-import subprocess
-
+and descriptor packing of mixed sizes."""
 import numpy as np
 import pytest
 import torch
 
-from tests.conftest import ROOT, load_golden
-from tests.emu_augment import EmuKernelsAugment, axis_weights, jitter_frames, parse, resize_window
+from tests.conftest import load_golden
+from tests.emu_augment import axis_weights, jitter_frames, parse, resize_window
+from tests.emu_kernels import EmuKernels
 
 PIPELINES = ('train', 'mim', 'val', 'test')
 SIZE_CLASSES = [(256, 340), (320, 427), (340, 256), (40, 56), (16, 200), (480, 640)]
@@ -31,7 +27,7 @@ def resize_bound(n_in_h, n_in_w, RH, RW, filter_id):
 def emu_aug():
     from videotransformer_pytorch_b200 import _lib
     old = _lib.K
-    _lib.K = EmuKernelsAugment(exact=True)
+    _lib.K = EmuKernels(exact=True, inference_forms=True)
     yield _lib.K
     _lib.K = old
 
@@ -242,25 +238,3 @@ def test_errors(emu_aug):
         A.create_video_transform(32, is_training=False, interpolation='bicubic', device='cpu')(
             [torch.zeros(1, 600, 600, 3, dtype=torch.uint8)])
     assert emu_aug.calls == []
-
-
-@pytest.mark.parametrize('struct', ['vt_crop_desc', 'vt_resized_crop_params', 'vt_jitter_desc', 'vt_color_jitter_params'])
-def test_struct_layout_matches_the_header(tmp_path, struct):
-    from videotransformer_pytorch_b200 import _lib
-    if not shutil.which('gcc'):
-        pytest.skip('gcc not available')
-    cls = {'vt_crop_desc': _lib.CropDesc, 'vt_resized_crop_params': _lib.ResizedCropParams,
-           'vt_jitter_desc': _lib.JitterDesc, 'vt_color_jitter_params': _lib.ColorJitterParams}[struct]
-    lines = ['#include <stdio.h>', '#include <stddef.h>', f'#include "{os.path.join(ROOT, "include", "vt_b200.h")}"',
-             'int main(void) {', f'  printf("size %zu\\n", sizeof({struct}));']
-    lines += [f'  printf("{f} %zu\\n", offsetof({struct}, {f}));' for f, _ in cls._fields_]
-    lines += ['  return 0;', '}']
-    src = tmp_path / 'layout.c'
-    src.write_text('\n'.join(lines))
-    subprocess.check_call(['gcc', str(src), '-o', str(tmp_path / 'layout')])
-    out = subprocess.run([str(tmp_path / 'layout')], capture_output=True, text=True, check=True).stdout
-    got = dict((ln.split()[0], int(ln.split()[1])) for ln in out.splitlines())
-    assert got['size'] == ctypes.sizeof(cls)
-    for f, _ in cls._fields_:
-        assert got[f] == getattr(cls, f).offset, f
-    assert 'vt_resized_crop_u8' in _lib.EXPORTS and 'vt_color_jitter_u8' in _lib.EXPORTS

@@ -1,19 +1,19 @@
-"""Forward-only evaluation path, host side, on CPU with the kernel table replaced by the twin of tests/emu_eval.py:
-the no_grad forward of every golden configuration against the goldens and bit for bit against the grad-enabled forward,
-which kernel forms each took, the top-k counter twin against a plain-torch restatement of the test step, inference mode
-between training steps, and a linear probe."""
+"""Forward-only evaluation path, host side, on CPU with the kernel table replaced by the twin of tests/emu_kernels.py with
+its forward-only forms: the no_grad forward of every golden configuration against the goldens and bit for bit against
+the grad-enabled forward, which kernel forms each took, the top-k counter twin against a plain-torch restatement of the
+test step, inference mode between training steps, and a linear probe."""
 import pytest
 import torch
 
 from tests.conftest import rel_err
-from tests.emu_eval import EmuKernelsEval
+from tests.emu_kernels import EmuKernels
 
 
 @pytest.fixture
 def emu():
     from videotransformer_pytorch_b200 import _lib
     old = _lib.K
-    _lib.K = EmuKernelsEval(exact=True)
+    _lib.K = EmuKernels(exact=True, inference_forms=True)
     yield _lib.K
     _lib.K = old
 
@@ -187,10 +187,9 @@ def _tiny_timesformer():
 def test_inference_mode_between_training_steps(table):
     """An eval forward under torch.inference_mode() (Lightning's default for validation), then a training step, then eval
     again: the cached index maps and weight shadows made under inference mode must not reach autograd."""
-    from tests.emu_kernels import EmuKernels
     from videotransformer_pytorch_b200 import _lib, ops
     old = _lib.K
-    _lib.K = EmuKernels(exact=True) if table == 'emu' else EmuKernelsEval(exact=True)
+    _lib.K = EmuKernels(exact=True, inference_forms=table == 'emu_eval')
     try:
         ops.token_maps.cache_clear()
         ops.frame_maps.cache_clear()
@@ -213,7 +212,6 @@ def test_inference_mode_between_training_steps(table):
 def test_linear_probe_head_gradients_match():
     """linear_prob (model_trainer.py:198-201): backbone under no_grad in eval mode, only the head trained.  The head's
     gradients are the same whether the backbone took the forward-only path or the saving forward."""
-    from tests.emu_kernels import EmuKernels
     from videotransformer_pytorch_b200 import _lib, cross_entropy
     from videotransformer_pytorch_b200.transformer import ClassificationHead
     m = _tiny_timesformer().eval()
@@ -223,14 +221,14 @@ def test_linear_probe_head_gradients_match():
     old = _lib.K
     grads = []
     try:
-        for table in (EmuKernelsEval(exact=True), EmuKernels(exact=True)):
+        for table in (EmuKernels(exact=True, inference_forms=True), EmuKernels(exact=True)):
             _lib.K = table
             head.zero_grad(set_to_none=True)
             with torch.no_grad():
                 f = m(x)
             cross_entropy(head(f), labels).backward()
             grads.append([p.grad.clone() for p in head.parameters()])
-            if isinstance(table, EmuKernelsEval):
+            if table.inference_forms:
                 assert any(c[-1] == 'gelu_h' for c in table.calls if c[0] == 'gemm')
     finally:
         _lib.K = old

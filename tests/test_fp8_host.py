@@ -1,18 +1,14 @@
-"""FP8 inference forms, host side, on the CPU: the quantiser twin against an exact fp64 restatement of e4m3 rounding, the
-ABI structs against the header, and the fp8 forward-only forms of the models on the emulated kernel table (which launches
-they issue, that grad-enabled calls never take them, shadow re-quantisation, and the errors)."""
-import ctypes
+"""FP8 inference forms, host side, on the CPU: the quantiser twin against an exact fp64 restatement of e4m3 rounding, and
+the fp8 forward-only forms of the models on the emulated kernel table (which launches they issue, that grad-enabled calls
+never take them, shadow re-quantisation, and the errors)."""
 import math
-import os
-import shutil
-import subprocess
 
 import pytest
 import torch
 
-from tests.conftest import ROOT, rel_err
-from tests.emu_eval import EmuKernelsEval
-from tests.emu_fp8 import EmuKernelsFp8, e4m3_cast, e4m3_round_fp64, quant_rows_twin
+from tests.conftest import rel_err
+from tests.emu_fp8 import e4m3_cast, e4m3_round_fp64, quant_rows_twin
+from tests.emu_kernels import EmuKernels
 
 
 def _e4m3_grid():
@@ -71,33 +67,12 @@ def test_quant_rows_twin(dtype, K):
     assert bool((ratio >= 0.5).all() & (ratio <= 1.0).all())         # the scale uses the top binade of e4m3
 
 
-@pytest.mark.parametrize('struct', ['vt_gemm_e4m3_params', 'vt_quant_rows_params'])
-def test_struct_layout_matches_the_header(tmp_path, struct):
-    from videotransformer_pytorch_b200 import _lib
-    if not shutil.which('gcc'):
-        pytest.skip('gcc not available')
-    cls = {'vt_gemm_e4m3_params': _lib.GemmE4m3Params, 'vt_quant_rows_params': _lib.QuantRowsParams}[struct]
-    lines = ['#include <stdio.h>', '#include <stddef.h>', f'#include "{os.path.join(ROOT, "include", "vt_b200.h")}"',
-             'int main(void) {', f'  printf("size %zu\\n", sizeof({struct}));']
-    lines += [f'  printf("{f} %zu\\n", offsetof({struct}, {f}));' for f, _ in cls._fields_]
-    lines += ['  return 0;', '}']
-    src = tmp_path / 'layout.c'
-    src.write_text('\n'.join(lines))
-    subprocess.check_call(['gcc', str(src), '-o', str(tmp_path / 'layout')])
-    out = subprocess.run([str(tmp_path / 'layout')], capture_output=True, text=True, check=True).stdout
-    got = dict((ln.split()[0], int(ln.split()[1])) for ln in out.splitlines())
-    assert got['size'] == ctypes.sizeof(cls)
-    for f, _ in cls._fields_:
-        assert got[f] == getattr(cls, f).offset, f
-    assert 'vt_gemm_e4m3' in _lib.EXPORTS and 'vt_quant_rows_e4m3' in _lib.EXPORTS
-
-
 # ------------------------------------------------------------------------------------------------ host logic
 @pytest.fixture
 def table():
     from videotransformer_pytorch_b200 import _lib, ops
     old = _lib.K
-    _lib.K = EmuKernelsFp8(exact=True)
+    _lib.K = EmuKernels(exact=True, inference_forms=True, fp8_forms=True)
     ops.token_maps.cache_clear()
     ops.frame_maps.cache_clear()
     yield _lib.K
@@ -149,8 +124,8 @@ def test_fp8_forward_only_launches(table, kind, attention_type):
     assert g8[0][0] == 'gemm' and all(c[0] == 'gemm_e4m3' for c in g8[1:])          # patch embed bf16, the rest e4m3
     for i, c in enumerate(calls):
         if c[0] == 'gemm_e4m3':                                    # A quantised per token right before, M x K rows
-            assert calls[i - 1][0] == 'quant_e4m3' and calls[i - 1][1:] == (c[1], c[3]), (calls[i - 1], c)
-    n_quant = sum(c[0] == 'quant_e4m3' for c in calls)
+            assert calls[i - 1][0] == 'quant_rows_e4m3' and calls[i - 1][1:] == (c[1], c[3]), (calls[i - 1], c)
+    n_quant = sum(c[0] == 'quant_rows_e4m3' for c in calls)
     assert n_quant == len(g8) - 1                                  # cached shadows: no weight is re-quantised
     assert 0 < rel_err(y8, y16) < 0.1
     with torch.inference_mode():
@@ -168,7 +143,7 @@ def test_fp8_grad_enabled_calls_are_untouched(table):
         torch.manual_seed(3)
         y = m(x)
         y.square().sum().backward()
-        assert not any(c[0] in ('quant_e4m3', 'gemm_e4m3') for c in table.calls)
+        assert not any(c[0] in ('quant_rows_e4m3', 'gemm_e4m3') for c in table.calls)
         runs.append((y.detach(), [p.grad.clone() for p in m.parameters()], list(table.calls)))
     assert torch.equal(runs[0][0], runs[1][0]) and runs[0][2] == runs[1][2]
     assert all(torch.equal(a, b) for a, b in zip(runs[0][1], runs[1][1]))
@@ -176,7 +151,7 @@ def test_fp8_grad_enabled_calls_are_untouched(table):
     m = _tiny().set_inference_precision('fp8')
     table.calls.clear()
     m(x)
-    assert not any(c[0] in ('quant_e4m3', 'gemm_e4m3') for c in table.calls)
+    assert not any(c[0] in ('quant_rows_e4m3', 'gemm_e4m3') for c in table.calls)
 
 
 def test_fp8_shadows_requantise_on_parameter_change(table):
@@ -225,7 +200,7 @@ def test_fp8_maskfeat_forward_only(table, maskfeat_golden):
     n_proj = sum(b.dim != b.dim_out for b in m.mvit.blocks)
     assert len(g8) - 1 == 4 * n_blocks + n_proj
     # FC1 and the width-changing proj share one quantisation of norm2(x)
-    assert sum(c[0] == 'quant_e4m3' for c in table.calls) == 4 * n_blocks
+    assert sum(c[0] == 'quant_rows_e4m3' for c in table.calls) == 4 * n_blocks
     # each e4m3 operand carries ~2.7 % rel-L2 rounding error; over the 16 random-weight blocks of this MViT it grows to
     # ~21 % of the features (the exact emulation of the same quantisation against the fp64 oracle shows the same)
     assert 0 < rel_err(f8, f16) < 0.3
@@ -248,7 +223,7 @@ def test_fp8_errors(table, monkeypatch):
     _lib.check_fp8_device('cuda:0')
     # a kernel table without the e4m3 forms: no fallback to bf16
     m.set_inference_precision('fp8')
-    _lib.K = EmuKernelsEval(exact=True)
+    _lib.K = EmuKernels(exact=True, inference_forms=True, fp8_forms=False)
     with pytest.raises(RuntimeError, match='no fp8 forms'), torch.no_grad():
         m(torch.randn(1, 4, 3, 32, 32))
     m.set_inference_precision('bf16')

@@ -8,7 +8,8 @@ import numpy as np
 import pytest
 import torch
 
-from tests.emu_augment import EmuKernelsAugment, resize_window
+from tests.emu_augment import resize_window
+from tests.emu_kernels import EmuKernels
 from tests.test_augment_host import PIPELINES, _golden_cases, _golden_clips, _preround, resize_bound
 
 pytestmark = pytest.mark.gpu
@@ -102,7 +103,7 @@ def test_pipelines_against_goldens_and_twin(name):
         out = tf([torch.from_numpy(clips[i]).permute(0, 2, 3, 1).to(dev) for i in ids]).cpu()
         assert int(tf.err) == 0
         old = _lib.K
-        _lib.K = EmuKernelsAugment(exact=True)
+        _lib.K = EmuKernels(exact=True, inference_forms=True)
         try:
             torch.manual_seed(seed)
             twin = mk('cpu')([torch.from_numpy(clips[i]).permute(0, 2, 3, 1) for i in ids])
@@ -219,7 +220,7 @@ def test_models_and_hog_fed_the_transformed_clip():
         torch.manual_seed(21)
         x = mk(None)([c.to(dev) for c in clips])
         old = _lib.K
-        _lib.K = EmuKernelsAugment(exact=True)
+        _lib.K = EmuKernels(exact=True, inference_forms=True)
         try:
             torch.manual_seed(21)
             host = mk('cpu')(clips)

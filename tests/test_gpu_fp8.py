@@ -14,7 +14,8 @@ import pytest
 import torch
 
 from tests.conftest import rel_err
-from tests.emu_fp8 import E4M3_MAX, EmuKernelsFp8, quant_rows_twin
+from tests.emu_fp8 import E4M3_MAX, quant_rows_twin
+from tests.emu_kernels import EmuKernels
 
 pytestmark = pytest.mark.gpu
 
@@ -249,7 +250,7 @@ def _emu_forward(build_model, x, fn=None):
     """The fp8 forward on the quantising fp64 emulation: same quantised operands, everything else in fp64."""
     from videotransformer_pytorch_b200 import _lib, ops
     old = _lib.K
-    _lib.K = EmuKernelsFp8(exact=True, dtype=torch.float64)
+    _lib.K = EmuKernels(exact=True, dtype=torch.float64, inference_forms=True, fp8_forms=True)
     ops.token_maps.cache_clear()
     ops.frame_maps.cache_clear()
     try:

@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from tests.conftest import rel_err
-from tests.emu_mvit_u8 import EmuKernelsU8
+from tests.emu_kernels import EmuKernels
 from tests.test_mvit_u8_host import IMAGENET_NORM, REF_NORM, build, reference_float_clip
 
 pytestmark = pytest.mark.gpu
@@ -56,7 +56,7 @@ def test_kernel_equals_twin(geom, plan):
     pl = None if spec is None else torch.tensor([spec[0], spec[1], *spec[2]], dtype=torch.float32)
     mean, std = IMAGENET_NORM if B == 4 else REF_NORM
     cols = _kernel_cols(u8, mean, std, pl).cpu()
-    twin, _ = EmuKernelsU8(exact=False).im2col3d_u8(u8, torch.tensor(mean), torch.tensor(std), pl, *FILTER, KPAD)
+    twin, _ = EmuKernels(exact=False).im2col3d_u8(u8, torch.tensor(mean), torch.tensor(std), pl, *FILTER, KPAD)
     assert not cols.isnan().any()
     assert torch.equal(cols, twin)
 

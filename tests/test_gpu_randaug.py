@@ -6,7 +6,8 @@ import pytest
 import torch
 
 from tests.emu_augment import resize_window
-from tests.emu_randaug import GEOMETRIC, EmuKernelsRandAug, desc_ops, near_tie_mask, randaug_frames
+from tests.emu_kernels import EmuKernels
+from tests.emu_randaug import GEOMETRIC, desc_ops, near_tie_mask, randaug_frames
 from tests.test_randaug_host import (CONTENTS, MAGNITUDES, OBJECTIVES, SIZES, _check_against_golden, _golden,
                                      _golden_ops, content, slot)
 
@@ -96,7 +97,7 @@ def test_pipelines_against_goldens_and_twin(objective):
         out = tf([torch.from_numpy(clips[i]).permute(0, 2, 3, 1).to(dev) for i in ids]).cpu()
         assert int(tf.err) == 0
         old = _lib.K
-        _lib.K = EmuKernelsRandAug(exact=True)
+        _lib.K = EmuKernels(exact=True, inference_forms=True)
         try:
             torch.manual_seed(seed)
             twin_tf = mk('cpu')
@@ -182,7 +183,7 @@ def test_models_and_hog_fed_the_transformed_clip():
         torch.manual_seed(21)
         x = mk(None)([c.to(dev) for c in clips])
         old = _lib.K
-        _lib.K = EmuKernelsRandAug(exact=True)
+        _lib.K = EmuKernels(exact=True, inference_forms=True)
         try:
             torch.manual_seed(21)
             host = mk('cpu')(clips)

@@ -147,8 +147,8 @@ def test_timesformer_joint_space_time_through_vt_attn(golden, emu, name):
     check_grads({n: p.grad for n, p in m.named_parameters()}, g, 2e-4)
     n = 1 + c['num_frames'] * (c['img_size'] // c['patch_size']) ** 2
     assert n == (289 if name == 'timesformer_joint_n289' else 17)
-    assert ('attn', 'fwd', n) in emu.calls and ('attn', 'bwd', n) in emu.calls
-    assert not any(c_[0] == 'xattn' for c_ in emu.calls)
+    assert ('attn_fwd', True, n) in emu.calls and ('attn_bwd', n) in emu.calls
+    assert not any(c_[0].startswith('xattn') for c_ in emu.calls)
 
 
 def test_timesformer_accepts_uint8_clip(golden, emu):

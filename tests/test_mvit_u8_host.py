@@ -1,17 +1,11 @@
-"""MaskFeat's uint8 input path without a GPU: the ABI of vt_im2col3d_u8_bf16, its CPU twin (tests/emu_mvit_u8.py) against
-the reference's float pipeline, a loop-for-loop walk-through of the kernel's CTA -> staged window -> 16-byte store
+"""MaskFeat's uint8 input path without a GPU: the CPU twin of vt_im2col3d_u8_bf16 (EmuKernels.im2col3d_u8) against the
+reference's float pipeline, a loop-for-loop walk-through of the kernel's CTA -> staged window -> 16-byte store
 mapping, and MaskFeat on the CPU emulation fed uint8 clips."""
-import ctypes
-import os
-import shutil
-import subprocess
-
 import numpy as np
 import pytest
 import torch
 
-from tests.conftest import ROOT
-from tests.emu_mvit_u8 import EmuKernelsU8
+from tests.emu_kernels import EmuKernels
 
 REF_NORM = ((0.45, 0.45, 0.45), (0.225, 0.225, 0.225))                 # data_trainer.py defaults
 IMAGENET_NORM = ((0.485, 0.456, 0.406), (0.229, 0.224, 0.225))
@@ -26,25 +20,6 @@ def reference_float_clip(u8, mean, std):
     return x.sub_(m).div_(s).contiguous()
 
 
-def test_params_struct_matches_header(tmp_path):
-    from videotransformer_pytorch_b200 import _lib
-    if not shutil.which('gcc'):
-        pytest.skip('no gcc')
-    cls = _lib.Im2col3dU8Params
-    lines = ['#include <stdio.h>', '#include <stddef.h>', f'#include "{os.path.join(ROOT, "include", "vt_b200.h")}"',
-             'int main(void) {', '  printf("size %zu\\n", sizeof(vt_im2col3d_u8_params));']
-    lines += [f'  printf("{f} %zu\\n", offsetof(vt_im2col3d_u8_params, {f}));' for f, _ in cls._fields_]
-    lines += ['  return 0;', '}']
-    (tmp_path / 'layout.c').write_text('\n'.join(lines))
-    subprocess.check_call(['gcc', str(tmp_path / 'layout.c'), '-o', str(tmp_path / 'layout')])
-    out = subprocess.run([str(tmp_path / 'layout')], capture_output=True, text=True, check=True).stdout
-    got = dict((k, int(v)) for k, v in (ln.split() for ln in out.splitlines()))
-    assert got['size'] == ctypes.sizeof(cls)
-    for f, _ in cls._fields_:
-        assert got[f] == getattr(cls, f).offset, f
-    assert 'vt_im2col3d_u8_bf16' in _lib.EXPORTS
-
-
 @pytest.mark.parametrize('norm', [REF_NORM, IMAGENET_NORM], ids=['reference', 'imagenet'])
 def test_twin_is_the_reference_float_clip_for_every_byte(norm):
     """A 1x1x1 conv makes cols the normalised clip itself: the twin equals the reference's fp32 clip bit for bit for all
@@ -52,7 +27,7 @@ def test_twin_is_the_reference_float_clip_for_every_byte(norm):
     mean, std = norm
     u = torch.arange(256, dtype=torch.uint8)
     u8 = torch.stack([u, u.flip(0), u.roll(97)], dim=-1).view(1, 1, 16, 16, 3)
-    em = EmuKernelsU8(exact=True)
+    em = EmuKernels(exact=True)
     cols, out = em.im2col3d_u8(u8, torch.tensor(mean), torch.tensor(std), None, (1, 1, 1), (1, 1, 1), (0, 0, 0), 8)
     assert out == (1, 16, 16) and cols.dtype == torch.float32
     ref = reference_float_clip(u8, mean, std).permute(0, 1, 3, 4, 2).reshape(256, 3)
@@ -161,7 +136,7 @@ def test_kernel_walk_covers_cols_once_and_matches_twin(case, plan):
     pl = None if WALK_PLANS[plan] is None else _plan(*WALK_PLANS[plan])
     cols, hits = walk_kernel(u8, mean, std, pl, kernel, stride, padding, kpad)
     assert (hits == 1).all()
-    twin, _ = EmuKernelsU8(exact=False).im2col3d_u8(u8, torch.tensor(mean), torch.tensor(std), pl, kernel, stride, padding, kpad)
+    twin, _ = EmuKernels(exact=False).im2col3d_u8(u8, torch.tensor(mean), torch.tensor(std), pl, kernel, stride, padding, kpad)
     assert torch.equal(cols, twin.float())
 
 
@@ -172,16 +147,6 @@ def test_rows_per_cta_at_maskfeat_sizes():
 
 
 # ---- MaskFeat on the CPU emulation ------------------------------------------------------------------------
-@pytest.fixture
-def emu_u8():
-    """The CPU kernel table with the uint8 Conv3d operand (the `emu` fixture's table plus im2col3d_u8)."""
-    from videotransformer_pytorch_b200 import _lib
-    old = _lib.K
-    _lib.K = EmuKernelsU8(exact=True)
-    yield _lib.K
-    _lib.K = old
-
-
 def build(g):
     from videotransformer_pytorch_b200 import MaskFeat
     kw = dict(g.kwargs)
@@ -200,7 +165,7 @@ def _clip(g, B, seed):
 
 
 @pytest.mark.parametrize('norm', [None, IMAGENET_NORM], ids=['default', 'imagenet'])
-def test_maskfeat_uint8_equals_reference_normalised_clip(maskfeat_golden, emu_u8, norm):
+def test_maskfeat_uint8_equals_reference_normalised_clip(maskfeat_golden, emu, norm):
     g = maskfeat_golden('maskfeat_s32')
     m = build(g).train()
     if norm is not None:
@@ -223,7 +188,7 @@ def test_maskfeat_uint8_equals_reference_normalised_clip(maskfeat_golden, emu_u8
 
 
 @pytest.mark.parametrize('seed', [0, 1, 2, 5])
-def test_maskfeat_mixed_uint8_equals_float_mixup(maskfeat_golden, emu_u8, seed):
+def test_maskfeat_mixed_uint8_equals_float_mixup(maskfeat_golden, emu, seed):
     """Mixup on the uint8 batch (a MixedClip) against the package's float Mixup on the reference-normalised clip, same
     numpy seed: CutMix copies are exact; the Mixup blend differs from the reference's by how 1 - lam is rounded (fp64
     scalar vs fp32), at most an ulp per element."""
@@ -246,7 +211,7 @@ def test_maskfeat_mixed_uint8_equals_float_mixup(maskfeat_golden, emu_u8, seed):
         assert float((f8 - ff).norm() / ff.norm()) < 1e-5
 
 
-def test_maskfeat_rejects_bad_uint8_inputs(maskfeat_golden, emu_u8):
+def test_maskfeat_rejects_bad_uint8_inputs(maskfeat_golden, emu):
     from videotransformer_pytorch_b200 import MixedClip
     g = maskfeat_golden('maskfeat_s32')
     m = build(g)

@@ -1,21 +1,19 @@
 """GPU RandAugment, host side, on the CPU: the restated draws against torchvision's RandAugment, the kernel's fp32 twin
 (tests/emu_randaug.py) against torchvision's _apply_op over every op, sign, magnitude, size and several kinds of content
 (bit for bit, except warped pixels whose fp64 source coordinate lies within the derived bound of a half-integer), the twin
-and the whole host path under emulation against the reference goldens (oracle/make_randaug_golden.py), errors,
-descriptor packing and the C struct layouts."""
+and the whole host path under emulation against the reference goldens (oracle/make_randaug_golden.py), errors
+and descriptor packing."""
 import ctypes
 import math
-import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-from tests.conftest import ROOT, load_golden
+from tests.conftest import load_golden
 from tests.emu_augment import parse
-from tests.emu_randaug import GEOMETRIC, EmuKernelsRandAug, near_tie_mask, randaug_frames
+from tests.emu_kernels import EmuKernels
+from tests.emu_randaug import GEOMETRIC, near_tie_mask, randaug_frames
 
 OBJECTIVES = ('supervised', 'mim')
 SIZES = (224, 256, 32, 17, 3, 2)
@@ -27,7 +25,7 @@ CONTENTS = ('random', 'smooth', 'constant_frame', 'constant_channel', 'two_value
 def emu_ra():
     from videotransformer_pytorch_b200 import _lib
     old = _lib.K
-    _lib.K = EmuKernelsRandAug(exact=True)
+    _lib.K = EmuKernels(exact=True, inference_forms=True)
     yield _lib.K
     _lib.K = old
 
@@ -281,25 +279,3 @@ def test_errors(emu_ra):
     val = A.create_video_transform(224, is_training=False, auto_augment='rand_aug', device='cpu')  # eval: not applied
     assert val.rand_augment is None
     assert emu_ra.calls == []
-
-
-@pytest.mark.parametrize('struct', ['vt_randaug_desc', 'vt_rand_augment_params'])
-def test_struct_layout_matches_the_header(tmp_path, struct):
-    from videotransformer_pytorch_b200 import _lib
-    if not shutil.which('gcc'):
-        pytest.skip('gcc not available')
-    cls = {'vt_randaug_desc': _lib.RandAugDesc, 'vt_rand_augment_params': _lib.RandAugmentParams}[struct]
-    lines = ['#include <stdio.h>', '#include <stddef.h>', f'#include "{os.path.join(ROOT, "include", "vt_b200.h")}"',
-             'int main(void) {', f'  printf("size %zu\\n", sizeof({struct}));',
-             '  printf("max_ops %d\\n", VT_RANDAUG_MAX_OPS);']
-    lines += [f'  printf("{f} %zu\\n", offsetof({struct}, {f}));' for f, _ in cls._fields_]
-    lines += ['  return 0;', '}']
-    src = tmp_path / 'layout.c'
-    src.write_text('\n'.join(lines))
-    subprocess.check_call(['gcc', str(src), '-o', str(tmp_path / 'layout')])
-    out = subprocess.run([str(tmp_path / 'layout')], capture_output=True, text=True, check=True).stdout
-    got = dict((ln.split()[0], int(ln.split()[1])) for ln in out.splitlines())
-    assert got['size'] == ctypes.sizeof(cls) and got['max_ops'] == _lib.RANDAUG_MAX_OPS
-    for f, _ in cls._fields_:
-        assert got[f] == getattr(cls, f).offset, f
-    assert 'vt_rand_augment_u8' in _lib.EXPORTS

@@ -129,6 +129,11 @@ class Im2colParams(C.Structure):
                 ('W', c_i32), ('tube', c_i32), ('ph', c_i32), ('pw', c_i32)]
 
 
+class Col2imParams(C.Structure):
+    _fields_ = [('cols', c_vp), ('dx', c_vp), ('B', c_i32), ('T', c_i32), ('C', c_i32), ('H', c_i32), ('W', c_i32),
+                ('tube', c_i32), ('ph', c_i32), ('pw', c_i32)]
+
+
 class Im2colU8Params(C.Structure):
     _fields_ = [('x', c_vp), ('scale', c_vp), ('shift', c_vp), ('cols', c_vp), ('B', c_i32), ('T', c_i32), ('C', c_i32),
                 ('H', c_i32), ('W', c_i32), ('tube', c_i32), ('ph', c_i32), ('pw', c_i32)]
@@ -848,8 +853,8 @@ class CudaKernels:
         cols = _req(cols, torch.float32, 'col2im.cols').contiguous()
         B, T, Cc, H, W = shape
         dx = torch.empty(shape, dtype=torch.float32, device=cols.device)
-        p = Im2colParams()
-        p.x, p.cols = cols.data_ptr(), dx.data_ptr()   # same POD layout: (src, dst, dims)
+        p = Col2imParams()
+        p.cols, p.dx = cols.data_ptr(), dx.data_ptr()
         p.B, p.T, p.C, p.H, p.W, p.tube, p.ph, p.pw = B, T, Cc, H, W, tube, ph, pw
         _check(lib.vt_col2im_f32(C.byref(p), _stream()), 'vt_col2im_f32')
         return dx
