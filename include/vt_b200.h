@@ -85,8 +85,8 @@ typedef struct {
   int64_t workspace_bytes;
   int32_t force_splits;    /* 0 = heuristic, >0 = exactly this many K splits (tests) */
   int32_t force_bn;        /* 0 = heuristic, 128 / 192 / 256 (tests) */
-  int32_t force_cluster;   /* accepted for ABI compatibility; every tile runs on one CTA */
-  void* debug;             /* unused, NULL */
+  int32_t force_cluster;   /* unused; kept for ABI compatibility */
+  void* debug;             /* unused; kept for ABI compatibility */
   /* Affine description of out_row / aux_row for VT_EPI_F32 with aux (the residual scatter of the divided space-time blocks),
    * map_period = 0: none.  GEMM row m -> outer = m / map_period, inner = m % map_period.  Rows with inner < map_skip are
    * "special" (the per-frame cls replicas of the spatial pass): no addend, written to out + map_special_base +
@@ -96,7 +96,7 @@ typedef struct {
    * transformer.py:250, :279-280, :352-356, :375-377) computed in the epilogue instead of read from index arrays; the
    * out_row / aux_row arrays, when also given, must describe the same mapping. */
   int32_t map_period, map_skip, map_tcount;
-  int32_t force_tail;      /* accepted for ABI compatibility; non-zero only disables the remainder-row split (vt_gemm_rows) */
+  int32_t force_tail;      /* unused; kept for ABI compatibility */
   int64_t map_stride_t, map_stride_p, map_stride_b, map_base;
   int64_t map_special_base, map_special_stride;
   const float* bias2;      /* VT_EPI_F32 with aux only: out = s(m) * (acc + bias[n]) + bias2[n] + aux — the bias of a second

@@ -29,8 +29,8 @@ fitted: the A-S constant is the published one and the rest follow from the opera
 Random operands.  Gaussian operands accumulate in fp32 with an error of at most K 2^-23 (|A||B|)_mn, the bound of a
 truncating adder (unit roundoff 2^-23) summing K products; split-K adds S - 1 more additions of the partials.  The
 epilogue adds at most four roundings of the sum of its terms' magnitudes T = |s| (|A||B| + |bias|) + |aux| + |bias2|:
-three for s (acc + bias) + (aux + bias2) in either order (the tensor-core epilogue's fmaf(s, acc + bias, aux + bias2), the
-remainder-rows kernel's ((s (acc + bias)) + aux) + bias2), and one for the second-order terms.
+three for s (acc + bias) + (aux + bias2) in either order (fmaf(s, acc + bias, aux + bias2) or ((s (acc + bias)) + aux) +
+bias2), and one for the second-order terms.
 """
 
 import math

@@ -23,7 +23,6 @@ check_ln_forward, ln_backward, ln_backward_bound, check_dgamma_dbeta, ln_plan = 
 ROW_WARPS = P.ROW_WARPS              # rows per CTA step of every warp-per-row kernel
 LN_CTAS_PER_SM = 4                   # ln_blocks / row_blocks(rows, 4) / vt_ln_bwd_blocks
 COLSUM_ROWS = 512                    # colsum_kernel: rows per chunk, walked by 8 row lanes
-COLSUM_WROWS = 64                    # colsum_wide_kernel: rows per chunk (8 per row lane); partials summed by 8 chunk lanes
 GCC_CTAS_PER_SM = 2                  # vt_gather_cast_colsum_blocks
 GBC_CTAS_PER_SM, GBC_UNROLL = 4, 2   # vt_gelu_bwd_colsum_blocks: 2 rows per CTA step
 RT_TALL_MIN, RT_LANES = 32, 64       # reduce_rows: tall kernel from 32 partial rows, 64 row lanes, then 16 + 4 lanes
@@ -48,12 +47,9 @@ def reduce_depth(S):
     return S if S < RT_TALL_MIN else cdiv(S, RT_LANES) + 3 + 15
 
 
-def colsum_n(M, wide, counters=True):
+def colsum_n(M, counters=True):
     """n of the colsum bound over M rows: rows per row lane + 8 lanes + the chunk partials (summed in order by the last CTA,
-    by reduce_rows in the two-launch form, or by 8 interleaved chunk lanes in the wide kernel)"""
-    if wide:
-        chunks = cdiv(M, COLSUM_WROWS)
-        return COLSUM_WROWS // ROW_WARPS + ROW_WARPS + cdiv(chunks, ROW_WARPS) + ROW_WARPS
+    or by reduce_rows in the two-launch form)"""
     chunks = cdiv(M, COLSUM_ROWS)
     return cdiv(min(M, COLSUM_ROWS), ROW_WARPS) + ROW_WARPS + (chunks if counters else reduce_depth(chunks))
 

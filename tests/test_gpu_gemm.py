@@ -284,43 +284,6 @@ def test_short_last_row_tile_deterministic(bn, M, N, Kd, form):
     assert torch.equal(got, again)
 
 
-@pytest.mark.parametrize('M,N,Kd', [(12552, 768, 3072), (1032, 200, 2048), (1025, 768, 2304), (1040, 384, 4096), (12552, 3072, 768)])
-@pytest.mark.parametrize('form', ['fwd_bf16', 'dgrad_bf16', 'fwd_f32_residual', 'dgrad_f32_plain'])
-def test_remainder_rows_split(M, N, Kd, form, monkeypatch):
-    """M a few rows past a multiple of 128 (12552 = 98 x 128 + 8): the full row tiles run on the tensor cores, the last rows
-    as CUDA-core dot products (vt_gemm_rows.cu).  Checked against fp32 torch, and row for row against the one-kernel path."""
-    a = mk((M, Kd), 60).bfloat16()
-    bias, rs = mk((N,), 61), mk((M,), 62)
-    if form == 'dgrad_bf16':
-        b = mk((Kd, N), 63).bfloat16()
-        kw = dict(b_mn=True, epi='bf16', row_scale=rs)
-        r = (a.float() @ b.float()) * rs[:, None]
-    elif form == 'dgrad_f32_plain':
-        b = mk((Kd, N), 63).bfloat16()
-        kw = dict(b_mn=True, epi='f32', bias=bias)
-        r = a.float() @ b.float() + bias
-    elif form == 'fwd_bf16':
-        b = mk((N, Kd), 63).bfloat16()
-        kw = dict(epi='bf16', bias=bias)
-        r = a.float() @ b.float().t() + bias
-    else:
-        b = mk((N, Kd), 63).bfloat16()
-        aux = mk((M, N), 64)
-        kw = dict(epi='f32', bias=bias, row_scale=rs, aux=aux)
-        r = (a.float() @ b.float().t() + bias) * rs[:, None] + aux
-    monkeypatch.setenv('VT_ROWS_SPLIT', '1')
-    got = K().gemm(a, b, M, N, Kd, **kw)
-    monkeypatch.setenv('VT_ROWS_SPLIT', '0')
-    one = K().gemm(a, b, M, N, Kd, **kw)
-    f32 = form in ('fwd_f32_residual', 'dgrad_f32_plain')
-    tol = 1e-5 if f32 else 4e-3
-    assert rel(got, r) < tol
-    m0 = M // 128 * 128
-    assert rel(got[:m0], one[:m0]) < 1e-6                      # the full row tiles: tensor-core kernel either way
-    assert rel(got[m0:], r[m0:].to(got.device)) < tol          # the remainder rows on their own
-    assert rel(got[m0:], one[m0:]) < (2e-5 if f32 else 8e-3)
-
-
 @pytest.mark.parametrize('staged', ['0', '1'], ids=['register', 'staged'])
 @pytest.mark.parametrize('M,N,Kd', [(12552, 3072, 768), (1000, 512, 128), (130, 96, 64)])
 def test_gelu_and_dgelu_epilogues_deterministic(M, N, Kd, staged, monkeypatch):

@@ -2,13 +2,13 @@
 
 A. Exact regime (tests/gemm_exact.py): integer operands and dyadic epilogue operands make every fp32 step exact, so each
    output must equal the float64 result rounded once, bit for bit: every form, both epilogue paths, every tile width and
-   operand layout, tile / k-block edges, split-K, the persistent walk on reduced grids and the remainder-rows kernels.
+   operand layout, tile / k-block edges, split-K, the persistent walk on reduced grids and M a few rows past a tile.
    Which kernel each configuration reaches is read from torch.profiler, in one session in a child process
-   (test_dispatch_reaches_every_cell): a profiler session per case, in the process that runs the suite, left the later
-   sessions of that process without records of kernels that had already run, and so blinded the profiler checks of
-   other modules.
+   (test_dispatch_reaches_every_tensor_core_cell): a profiler session per case, in the process that runs the suite, left
+   the later sessions of that process without records of kernels that had already run, and so blinded the profiler
+   checks of other modules.
 B. Every operand is a view into a NaN-filled allocation (padded pitch, rows past K / M / N), and every output lives in a
-   sentinel-filled buffer with a padded pitch, so a read the tensor maps or the remainder path should have clipped turns
+   sentinel-filled buffer with a padded pitch, so a read the tensor maps should have clipped turns
    outputs into NaN, and a stray write changes a sentinel.
 C. GELU over all 65 536 bf16 inputs, stand-alone and through the GEMM epilogues, against the float64 GELU within the
    derived per-element bound of tests/gemm_exact.py.
@@ -96,9 +96,6 @@ def parse_cell(name):
     if m:
         bn, ta, tb = map(int, m.groups())
         return ('f32', 3, bn, ta, tb)
-    m = re.search(r'rows_(nt|nn)_kernel(?:<(\d+)>)?', name)
-    if m:
-        return ('rows_' + m.group(1), int(m.group(2) or 0), 0, 0, 0)
     return None
 
 
@@ -235,24 +232,18 @@ CELL_SHAPES = ((129, 200, 136), (1, 8, 8), (8, 72, 40), (127, 776, 72))
 @pytest.mark.parametrize('form', FORMS)
 def test_exact_cell(form, staged, bn, ta, tb, monkeypatch):
     """every form x epilogue path x tile width x operand layout on small edge shapes, bit for bit (the kernel each of
-    these configurations reaches: test_dispatch_reaches_every_cell)"""
+    these configurations reaches: test_dispatch_reaches_every_tensor_core_cell)"""
     monkeypatch.setenv('VT_GEMM_STAGED_EPI', str(staged))
     for i, (M, N, Kd) in enumerate(CELL_SHAPES):
         for j, var in enumerate(variants(form)):
             run_exact(form, M, N, Kd, ta=ta, tb=tb, bn=bn, seed=100 * i + j, pad=8 * (1 + (i + j) % 2), **var)
 
 
-# the remainder-rows shapes: (M, N, K, B MN-major, the rows kernel rows_split_point and launch_gemm_rows pick)
-ROWS_SHAPES = ((1032, 200, 2048, 0, ('rows_nt', 0)), (1040, 768, 2048, 1, ('rows_nn', 2)),
-               (1032, 1024, 2048, 1, ('rows_nn', 4)), (12552, 768, 3072, 0, ('rows_nt', 0)),
-               (12552, 768, 3072, 1, ('rows_nn', 2)))
-
-
 def dispatch_probe():
-    """Body of the child process of test_dispatch_reaches_every_cell: one vt_gemm call per configuration of
-    test_exact_cell (shape 129 x 200 x 136) and per remainder-rows shape, all inside one torch.profiler session, with
-    every operand allocated before it.  Prints one JSON line: the configurations in call order and the cells of the
-    GEMM kernels in launch order."""
+    """Body of the child process of test_dispatch_reaches_every_tensor_core_cell: one vt_gemm call per configuration
+    of test_exact_cell (shape 129 x 200 x 136), all inside one torch.profiler session, with every operand allocated
+    before it.  Prints one JSON line: the configurations in call order and the cells of the GEMM kernels in launch
+    order."""
     import itertools
     import json
     import os
@@ -267,12 +258,7 @@ def dispatch_probe():
             kw['out2'] = torch.empty((M, N), dtype=torch.bfloat16, device='cuda')
         if form == 'dgelu':
             kw['aux'] = dgelu_z(M, N, 2)[0].bfloat16().cuda()
-        calls.append(([form, staged, bn, ta, tb], {'VT_GEMM_STAGED_EPI': str(staged), 'VT_ROWS_SPLIT': '0'},
-                      (a, b, M, N, Kd), kw))
-    for Mr, Nr, Kr, tb, _ in ROWS_SHAPES:
-        _, _, a, b = int_operands(Mr, Nr, Kr, 0, tb, seed=3, pad=8)
-        calls.append((['rows', Mr, Nr, Kr, tb], {'VT_GEMM_STAGED_EPI': '1', 'VT_ROWS_SPLIT': '1'}, (a, b, Mr, Nr, Kr),
-                      dict(b_mn=bool(tb), epi='bf16')))
+        calls.append(([form, staged, bn, ta, tb], {'VT_GEMM_STAGED_EPI': str(staged)}, (a, b, M, N, Kd), kw))
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         for _, env, args, kw in calls:
@@ -285,11 +271,10 @@ def dispatch_probe():
 
 
 @pytest.mark.gpu
-def test_dispatch_reaches_every_cell():
-    """The kernel cell each configuration of test_exact_cell reaches, and the remainder-rows kernel of each shape of
-    test_exact_remainder_rows: every (kernel, SE, BN, TA, TB) cell of the bf16 wgmma GEMM that the dispatch can reach.
-    Calls run in order on one stream, so the i-th GEMM kernel launched belongs to the i-th call (the remainder-rows
-    calls launch the tensor-core kernel and then the rows kernel)."""
+def test_dispatch_reaches_every_tensor_core_cell():
+    """The kernel cell each configuration of test_exact_cell reaches: every (kernel, SE, BN, TA, TB) cell of the bf16
+    wgmma GEMM that the dispatch can reach.  Calls run in order on one stream, so the i-th GEMM kernel launched belongs
+    to the i-th call."""
     import json
     import os
     import subprocess
@@ -301,22 +286,15 @@ def test_dispatch_reaches_every_cell():
     assert res.returncode == 0, res.stdout[-2000:] + res.stderr[-4000:]
     out = json.loads(res.stdout.strip().splitlines()[-1])
     configs, kernels = out['configs'], [tuple(k) for k in out['kernels']]
-    n_cells = sum(1 for c in configs if c[0] != 'rows')
-    rows = [c for c in configs if c[0] == 'rows']
-    assert len(kernels) == n_cells + 2 * len(rows), (len(kernels), n_cells, len(rows))
+    assert len(kernels) == len(configs), (len(kernels), len(configs))
     reached = {}
-    for cfg, cell in zip(configs[:n_cells], kernels[:n_cells]):
+    for cfg, cell in zip(configs, kernels):
         form, staged, bn, ta, tb = cfg
         want = expected_cell(form, staged, bn, ta, tb) if bn else (cell[0], cell[1], cell[2], ta, tb)
         assert cell == want, (cfg, cell, want)
         reached.setdefault(cell, []).append(cfg)
-    for i, (Mr, Nr, Kr, tb, rk) in enumerate(ROWS_SHAPES):
-        head, tail = kernels[n_cells + 2 * i], kernels[n_cells + 2 * i + 1]
-        assert head[0] == 'wgmma' and tail[:2] == rk, (Mr, Nr, Kr, tb, head, tail)
-        reached.setdefault(tail, []).append(['rows', Mr, Nr, Kr, tb])
     want_cells = {('wgmma', se, bn, ta, tb) for se in (0, 1, 2) for bn in (128, 192, 256) for ta in (0, 1) for tb in (0, 1)}
     want_cells |= {('f32', 3, bn, ta, tb) for bn in (128, 192) for ta in (0, 1) for tb in (0, 1)}
-    want_cells |= {('rows_nt', 0, 0, 0, 0), ('rows_nn', 2, 0, 0, 0), ('rows_nn', 4, 0, 0, 0)}
     assert want_cells <= set(reached), sorted(want_cells - set(reached))
     for cell in sorted(reached):
         print(cell, '<-', reached[cell][:3], f'({len(reached[cell])} configurations)')
@@ -368,11 +346,12 @@ def test_exact_split_k(zeroed, bn, monkeypatch):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize('M,N,Kd,tb,kernel', ROWS_SHAPES)
-def test_exact_remainder_rows(M, N, Kd, tb, kernel, monkeypatch):
-    """VT_ROWS_SPLIT=1 on the shapes rows_split_point accepts: the last 8 / 16 rows as CUDA-core dot products, with every
-    epilogue operand of the bf16 and fp32 forms (that `kernel` runs: test_dispatch_reaches_every_cell)"""
-    monkeypatch.setenv('VT_ROWS_SPLIT', '1')
+@pytest.mark.parametrize('M,N,Kd,tb', [(1032, 200, 2048, 0), (1040, 768, 2048, 1), (1032, 1024, 2048, 1),
+                                      (12552, 768, 3072, 0), (12552, 768, 3072, 1), (1025, 768, 2304, 0),
+                                      (1025, 768, 2304, 1), (1040, 384, 4096, 0), (1040, 384, 4096, 1)])
+def test_exact_remainder_rows(M, N, Kd, tb):
+    """M 1 to 16 rows past a multiple of 128 with long K: a last row of tiles that is nearly all padding, with every
+    epilogue operand of the bf16 and fp32 forms"""
     for form, var in (('bf16', dict(bias=True, rs=True)), ('f32', dict(bias=True, rs=True, aux=True, bias2=True)),
                       ('f32', dict(aux=True)), ('bf16', {})):
         run_exact(form, M, N, Kd, tb=tb, seed=N, pad=8, **var)
@@ -501,27 +480,25 @@ def gauss(shape, seed):
     return torch.randn(shape, generator=g)
 
 
-D_CASES = [  # name, M, N, K, ta, tb, form, epilogue operands, extra gemm arguments, env
-    ('qkv', 12552, 2304, 768, 0, 0, 'bf16', ('bias',), {}, {}),
-    ('proj+res', 12552, 768, 768, 0, 0, 'f32', ('bias', 'rs', 'aux', 'bias2'), {}, {}),
-    ('fc1', 12552, 3072, 768, 0, 0, 'bf16', ('bias',), {}, {}),
-    ('fc2+res', 12552, 768, 3072, 0, 0, 'f32', ('bias', 'aux'), {}, {}),
-    ('fc2 rows split', 12552, 768, 3072, 0, 0, 'f32', ('bias', 'rs', 'aux', 'bias2'), {}, {'VT_ROWS_SPLIT': '1'}),
-    ('fc1 dgrad', 12552, 768, 3072, 0, 1, 'bf16', ('rs',), {}, {}),
-    ('qkv dgrad', 12552, 768, 2304, 0, 1, 'f32', (), {}, {}),
-    ('fc2 dgrad', 12552, 3072, 768, 0, 1, 'bf16', (), {}, {}),
-    ('fc1 wgrad split', 3072, 768, 12552, 1, 1, 'f32', (), dict(split_ok=True), {}),
-    ('fc2 wgrad split 5', 768, 3072, 12552, 1, 1, 'f32', (), dict(split_ok=True, force_splits=5), {}),
-    ('mvit s1 fc2', 50184, 96, 384, 0, 0, 'f32', ('bias', 'aux'), {}, {}),
+D_CASES = [  # name, M, N, K, ta, tb, form, epilogue operands, extra gemm arguments
+    ('qkv', 12552, 2304, 768, 0, 0, 'bf16', ('bias',), {}),
+    ('proj+res', 12552, 768, 768, 0, 0, 'f32', ('bias', 'rs', 'aux', 'bias2'), {}),
+    ('fc1', 12552, 3072, 768, 0, 0, 'bf16', ('bias',), {}),
+    ('fc2+res', 12552, 768, 3072, 0, 0, 'f32', ('bias', 'aux'), {}),
+    ('fc2+res rs bias2', 12552, 768, 3072, 0, 0, 'f32', ('bias', 'rs', 'aux', 'bias2'), {}),
+    ('fc1 dgrad', 12552, 768, 3072, 0, 1, 'bf16', ('rs',), {}),
+    ('qkv dgrad', 12552, 768, 2304, 0, 1, 'f32', (), {}),
+    ('fc2 dgrad', 12552, 3072, 768, 0, 1, 'bf16', (), {}),
+    ('fc1 wgrad split', 3072, 768, 12552, 1, 1, 'f32', (), dict(split_ok=True)),
+    ('fc2 wgrad split 5', 768, 3072, 12552, 1, 1, 'f32', (), dict(split_ok=True, force_splits=5)),
+    ('mvit s1 fc2', 50184, 96, 384, 0, 0, 'f32', ('bias', 'aux'), {}),
 ]
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize('case', D_CASES, ids=[c[0] for c in D_CASES])
-def test_random_operands_within_fp64_bound(case, monkeypatch):
-    name, M, N, Kd, ta, tb, form, epi_ops, extra, env = case
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
+def test_random_operands_within_fp64_bound(case):
+    name, M, N, Kd, ta, tb, form, epi_ops, extra = case
     A, B = gauss((M, Kd), M + N).bfloat16().double(), gauss((N, Kd), Kd).bfloat16().double()
     a = (A.t() if ta else A).contiguous().bfloat16().cuda()
     b = (B.t() if tb else B).contiguous().bfloat16().cuda()

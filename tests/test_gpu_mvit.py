@@ -56,9 +56,7 @@ def test_layernorm_small(D, rows):
                                             ((2, 3, 3), (1, 1, 1), 2, 1), ((4, 16, 16), (1, 8, 8), 1, 3),
                                             ((8, 14, 14), (1, 2, 2), 4, 2), ((8, 7, 7), (1, 1, 1), 8, 2),
                                             ((2, 9, 11), (2, 2, 2), 2, 1), ((3, 28, 28), (1, 4, 4), 2, 2)])
-@pytest.mark.parametrize('gen', ['0', '1'], ids=['gen1', 'gen2'])
-def test_pool_fwd_bwd(thw, stride, H, B, gen, monkeypatch):
-    monkeypatch.setenv('VT_POOL_V2', gen)          # both generations of the pooling kernels (4 channels per lane = gen2)
+def test_pool_fwd_bwd(thw, stride, H, B):
     N1 = 1 + thw[0] * thw[1] * thw[2]
     d = H * HD
     qkv = rn((B * N1, 3 * d), 10).bfloat16()

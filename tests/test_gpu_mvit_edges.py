@@ -5,8 +5,9 @@ and to reject seeded defects in tests/test_mvit_pool_bounds.py), each stage agai
 outputs of the stage before.  The kernels are driven through ctypes: every output sits between NaN guard rows and starts
 as NaN, the other two slots of a packed q/k/v input hold NaN, and so do the rows past the last token, the dout rows past
 the end and the whole scratch, so a missing store, a store outside the output, or a read of the wrong slot, past the end
-or of scratch nobody wrote shows.  Both kernel generations run (VT_POOL_V2 = 0 / 1): their din must agree bit for bit,
-each must give the same dw bits over two calls, and dgamma / dbeta must not depend on whether they are adjacent.
+or of scratch nobody wrote shows.  Both kernel generations of the backward run: the second on 8-byte aligned views, the
+first on the same problem as a view 4 bytes into its row.  Their din must agree bit for bit, each must give the same dw
+bits over two calls, and dgamma / dbeta must not depend on whether they are adjacent.
 """
 import math
 
@@ -115,16 +116,15 @@ def _bits(t):
     return t.contiguous().view(torch.int16 if t.dtype == torch.bfloat16 else torch.int32)
 
 
-def _gen(monkeypatch, gen):
-    monkeypatch.setenv('VT_POOL_V2', '1' if gen == 2 else '0')
-
-
 @pytest.mark.parametrize('case', R.CASES, ids=R.case_id)
-def test_pool_kernels_against_fp64(case, monkeypatch):
+def test_pool_kernels_against_fp64(case):
     thw, stride, H, B, layout, regime = case
     x, w, gam, bet, dout = R.make_inputs(B, H, thw, stride, regime, seed=sum(thw) * 7 + H)
-    run = PoolRun(x, w, gam, bet, H, thw, stride, layout)
-    fwd = run.fwd()
+    runs = {gen: PoolRun(x, w, gam, bet, H, thw, stride, layout, misalign=gen == 1) for gen in (1, 2)}
+    fwds = {gen: run.fwd() for gen, run in runs.items()}
+    fwd = fwds[2]
+    for n in fwd:
+        assert torch.equal(_bits(fwds[1][n]), _bits(fwd[n])), f'{n}: the forward depends on the alignment of its input'
     xh = R.heads(x, H)
     rep = R.Report()
     R.check_forward(xh, w, gam, bet, thw, stride, fwd, rep)
@@ -132,8 +132,7 @@ def test_pool_kernels_against_fp64(case, monkeypatch):
     for dt in (torch.float32, torch.bfloat16):
         d = dout.to(dt)
         got = {}
-        for gen in (1, 2):
-            _gen(monkeypatch, gen)
+        for gen, run in runs.items():
             got[gen] = run.bwd(d)
             again = run.bwd(d)
             for n in got[gen]:
@@ -145,22 +144,21 @@ def test_pool_kernels_against_fp64(case, monkeypatch):
     print(f'[mvit-edges] {R.case_id(case)}: {rep}')
 
 
-def test_misaligned_view_falls_back_to_first_generation(monkeypatch):
-    """a view 4 bytes into its row cannot take the 8-byte loads of the second generation: with VT_POOL_V2=1 it must give
-    the first generation's bits, which differ from the second's at this shape (dw sums in another order)"""
+def test_misaligned_view_takes_first_generation():
+    """a view 4 bytes into its row cannot take the 8-byte loads of the second generation: it must take the first, whose
+    dw bits differ from the second's at this shape (dw sums in another order), and give the aligned view's other bits"""
     thw, stride, H, B = (4, 16, 16), (1, 2, 2), 2, 1
     x, w, gam, bet, dout = R.make_inputs(B, H, thw, stride, seed=21)
     res = {}
-    for key, gen, mis in (('gen1', 1, False), ('gen2', 2, False), ('mis', 2, True)):
-        _gen(monkeypatch, gen)
+    for key, mis in (('aligned', False), ('mis', True)):
         run = PoolRun(x, w, gam, bet, H, thw, stride, 0, misalign=mis)
         fwd = run.fwd()
         res[key] = (fwd, run.bwd(dout))
     for n in ('pooled', 'out', 'mean', 'rstd'):
-        assert torch.equal(_bits(res['mis'][0][n]), _bits(res['gen1'][0][n])), n
-    assert not torch.equal(_bits(res['gen2'][1]['dw']), _bits(res['gen1'][1]['dw']))
-    for n in ('din', 'dw', 'dgamma', 'dbeta'):
-        assert torch.equal(_bits(res['mis'][1][n]), _bits(res['gen1'][1][n])), n
+        assert torch.equal(_bits(res['mis'][0][n]), _bits(res['aligned'][0][n])), n
+    assert not torch.equal(_bits(res['mis'][1]['dw']), _bits(res['aligned'][1]['dw']))
+    for n in ('din', 'dpooled', 'dgamma', 'dbeta'):
+        assert torch.equal(_bits(res['mis'][1][n]), _bits(res['aligned'][1][n])), n
     rep = R.Report()
     xh = R.heads(x, H)
     R.check_forward(xh, w, gam, bet, thw, stride, res['mis'][0], rep)
@@ -169,12 +167,11 @@ def test_misaligned_view_falls_back_to_first_generation(monkeypatch):
 
 
 @pytest.mark.parametrize('gen', [1, 2])
-def test_dgamma_dbeta_separate_buffers(gen, monkeypatch):
+def test_dgamma_dbeta_separate_buffers(gen):
     """dgamma and dbeta in separate buffers (two reductions) give the bits of the adjacent [2, 96] form (one reduction)"""
-    _gen(monkeypatch, gen)
     thw, stride, H, B = (8, 14, 14), (1, 2, 2), 4, 3
     x, w, gam, bet, dout = R.make_inputs(B, H, thw, stride, seed=22)
-    run = PoolRun(x, w, gam, bet, H, thw, stride, 2)
+    run = PoolRun(x, w, gam, bet, H, thw, stride, 2, misalign=gen == 1)
     fwd = run.fwd()
     a, b = run.bwd(dout), run.bwd(dout, separate=True)
     for n in a:

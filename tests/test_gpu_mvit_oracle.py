@@ -30,9 +30,7 @@ def rn(shape, seed, scale=1.0):
 
 @pytest.mark.parametrize('thw,stride,H,B', [((8, 14, 14), (1, 2, 2), 4, 2), ((8, 28, 28), (1, 4, 4), 2, 1),
                                             ((4, 16, 16), (1, 8, 8), 1, 2), ((2, 5, 7), (1, 1, 1), 2, 1)])
-@pytest.mark.parametrize('gen', ['0', '1'], ids=['gen1', 'gen2'])
-def test_pool_kernels_vs_oracle_attention_pool(thw, stride, H, B, gen, monkeypatch):
-    monkeypatch.setenv('VT_POOL_V2', gen)
+def test_pool_kernels_vs_oracle_attention_pool(thw, stride, H, B):
     from oracle import mvit_oracle as MO
     N1 = 1 + thw[0] * thw[1] * thw[2]
     d = H * HD

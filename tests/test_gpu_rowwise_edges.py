@@ -209,7 +209,7 @@ def test_layernorm_against_fp64(case, monkeypatch):
 
 
 # ---- column sums -----------------------------------------------------------------------------------------------------
-def _colsum(v, wide, counters):
+def _colsum(v, counters):
     """vt_colsum_bf16 of v bf16 [M, N] (CPU) read 16 bytes into the rows of a NaN-filled [M + PAD, N + 16] buffer"""
     lib_, lib = _lib()
     M, N = v.shape
@@ -229,16 +229,13 @@ def _colsum(v, wide, counters):
 
 @pytest.mark.parametrize('M,N', [(1, 8), (511, 768), (512, 100), (513, 3072), (63, 96), (64, 2304), (65, 100), (12544, 768),
                                  (12552, 3072)])
-def test_colsum_against_fp64(M, N, monkeypatch):
+def test_colsum_against_fp64(M, N):
     v = torch.randn(M, N, generator=torch.Generator().manual_seed(M * 7 + N)).bfloat16()
     rep = R.Report()
-    for wide in (False, True):
-        monkeypatch.setenv('VT_COLSUM_WIDE', str(int(wide)))
-        for counters in (True, False):
-            a, b = _colsum(v, wide, counters), _colsum(v, wide, counters)
-            assert torch.equal(_bits(a), _bits(b)), 'colsum: two calls differ'
-            takes_wide = wide and counters and N % 8 == 0
-            R.check_colsum(f'colsum_{"wide" if takes_wide else "narrow"}', a, v, R.colsum_n(M, takes_wide, counters), rep)
+    for counters in (True, False):
+        a, b = _colsum(v, counters), _colsum(v, counters)
+        assert torch.equal(_bits(a), _bits(b)), 'colsum: two calls differ'
+        R.check_colsum('colsum', a, v, R.colsum_n(M, counters), rep)
     print(f'[rowwise-edges] colsum {M}x{N}: {rep}')
 
 
@@ -405,7 +402,7 @@ def test_temporal_block_fused_and_separate_column_sums_agree(monkeypatch):
     f, s = got[True], got[False]
     assert torch.equal(_bits(f['gs']), _bits(s['gs'])), 'the fused and separate producers give other bf16 rows'
     Mt = B * P * T
-    nf, ns = R.gcc_plan(Mt, _sm())[2], R.colsum_n(Mt, wide=False)
+    nf, ns = R.gcc_plan(Mt, _sm())[2], R.colsum_n(Mt)
     rep = R.Report()
     for name, rows in (('v', s['gs']), ('d_fc_b', s['unscaled'])):
         a = rows.double().abs().sum(0).cpu()

@@ -781,63 +781,3 @@ def test_residual_epilogue_segments_cover_every_row_once(B, T, P, kind):
     named[out_row.long()] = 1
     assert torch.equal(writes, named)                           # every mapped row written exactly once, no other row touched
     assert torch.equal(torch.nan_to_num(got, nan=-1.0), torch.nan_to_num(exp, nan=-1.0))
-
-
-# ---- vt_gemm_rows.cu: remainder rows of a GEMM on CUDA cores -------------------------------------------
-@pytest.mark.parametrize('CG,N,K,R', [(2, 48, 64, 8), (4, 96, 136, 5), (8, 200, 72, 8)])
-def test_rows_nn_kernel_thread_mapping(CG, N, K, R):
-    """rows_nn_kernel<CG>: CTA = CG * 8 output columns, thread = (8 consecutive columns) x (one of 256 / CG K slices, 8
-    consecutive k per step); slices summed by xor-shuffles over lane offsets CG, 2 CG, ... inside a warp, then across the 8
-    warps through shared memory.  Walked thread by thread against a plain matrix product."""
-    g = np.random.default_rng(0)
-    a = g.standard_normal((R, K))
-    w = g.standard_normal((K, N))
-    cols, slices = CG * 8, 256 // CG
-    out = np.full((R, N), np.nan)
-    for blk in range((N + cols - 1) // cols):
-        acc = np.zeros((256, R, 8))
-        for t in range(256):
-            cg, ks = t % CG, t // CG
-            n0 = blk * cols + cg * 8
-            if n0 >= N:
-                continue
-            for k in range(ks * 8, K, slices * 8):
-                for kk in range(8):                      # K % 8 == 0: a piece of 8 never straddles the end
-                    acc[t] += np.outer(a[:, k + kk], w[k + kk, n0:n0 + 8])
-        red = np.zeros((8, R, cols))
-        for warp in range(8):
-            lanes = acc[warp * 32:(warp + 1) * 32].copy()
-            o = CG
-            while o < 32:                                # v += shfl_xor(v, o)
-                lanes = lanes + lanes[np.arange(32) ^ o]
-                o <<= 1
-            for lane in range(CG):                       # lanes < CG hold the warp's sum for column group cg = lane
-                red[warp, :, lane * 8:lane * 8 + 8] = lanes[lane]
-        tot = red.sum(0)
-        for c in range(cols):
-            n = blk * cols + c
-            if n < N:
-                out[:, n] = tot[:, c]
-    assert rel(out, a @ w) < 1e-12
-
-
-@pytest.mark.parametrize('N,K,R', [(10, 768, 8), (7, 264, 3), (5, 3072, 8)])
-def test_rows_nt_kernel_lane_mapping(N, K, R):
-    """rows_nt_kernel: one warp per output column, lane l covers k = 8 l + 256 u (four pieces in flight per pass)."""
-    g = np.random.default_rng(1)
-    a = g.standard_normal((R, K))
-    w = g.standard_normal((N, K))
-    out = np.zeros((R, N))
-    for n in range(N):
-        lanes = np.zeros((32, R))
-        for lane in range(32):
-            k0 = lane * 8
-            while k0 < K:
-                for u in range(4):
-                    k = k0 + u * 256
-                    if k >= K:
-                        break
-                    lanes[lane] += a[:, k:k + 8] @ w[n, k:k + 8]
-                k0 += 4 * 256
-        out[:, n] = lanes.sum(0)                         # warp_sum
-    assert rel(out, a @ w.T) < 1e-12

@@ -146,17 +146,14 @@ def test_layernorm_model_with_spatial_maps_and_aux_rows():
 
 
 # ---- column sums, reduce_rows, cls_rows ----------------------------------------------------------------------------
-def colsum_model(v, wide, counters=True):
-    """fp32 column sums of v [M, N] (bf16 values) in the order of colsum_kernel / colsum_wide_kernel"""
+def colsum_model(v):
+    """fp32 column sums of v [M, N] (bf16 values) in the order of colsum_kernel"""
     M, N = v.shape
     v = v.float()
-    rows = R.COLSUM_WROWS if wide else R.COLSUM_ROWS
+    rows = R.COLSUM_ROWS
     chunks = R.cdiv(M, rows)
     w = torch.cat([v, v.new_zeros(chunks * rows - M, N)]).view(chunks, rows // R.ROW_WARPS, R.ROW_WARPS, N)
-    part = _seq(_seq(w.transpose(0, 1)).transpose(0, 1))            # [chunks, N]: lanes' rows in order, then the 8 lanes
-    if wide:
-        return _seq(_interleaved(part, 1, R.ROW_WARPS)[0])
-    return _seq(part)
+    return _seq(_seq(_seq(w.transpose(0, 1)).transpose(0, 1)))      # lanes' rows in order, then the 8 lanes, then the chunks
 
 
 def gcc_model(src, in_row, scale, unscaled=False, fp32_sums=False):
@@ -178,9 +175,8 @@ def test_colsum_models_sit_inside_their_bounds():
     rep = R.Report()
     for M, N in ((1, 8), (511, 96), (512, 100), (513, 768), (63, 64), (64, 72), (65, 256), (12544, 768), (12552, 3072)):
         v = torch.randn(M, N, generator=g).bfloat16()
-        for wide in (False, True) if N % 8 == 0 else (False,):
-            for counters in (True, False):
-                R.check_colsum('colsum', colsum_model(v, wide, counters), v, R.colsum_n(M, wide, counters), rep)
+        for counters in (True, False):
+            R.check_colsum('colsum', colsum_model(v), v, R.colsum_n(M, counters), rep)
     print(f'[rowwise-bounds] colsum: {rep}')
 
 

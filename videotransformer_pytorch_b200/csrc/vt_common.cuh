@@ -22,8 +22,8 @@ int check_launch(const char* what);   // cudaGetLastError -> error code
   } while (0)
 
 int sm_count();
-// Feature switch: environment variable `name` ("0" / "1") overrides the compiled default.  Paths that have not yet been
-// confirmed on hardware ship disabled and are exercised by the tests marked experimental.
+// Feature switch: environment variable `name` ("0" / "1") overrides the compiled default.  INTEGRATION.md §2 lists the
+// switches and their defaults; the tests set them to run both sides of each.
 bool feature_on(const char* name, bool dflt);
 // narrow-row LayerNorm (D = 32..256 step 32, vt_mvit.cu); vt_layernorm_fwd/bwd dispatch here when D % 128 != 0
 int layernorm_fwd_small(const vt_ln_fwd_params* p, void* stream);

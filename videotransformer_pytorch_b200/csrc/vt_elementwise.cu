@@ -525,87 +525,6 @@ colsum_kernel(const __nv_bfloat16* __restrict__ in, long long ld, int M, int N, 
   }
 }
 
-// Wide form (N % 8 == 0): CTA = 256 columns x 64 rows; a lane owns 8 adjacent columns (one 16-byte load per row), the 8
-// warps are row lanes and issue all 8 of their rows before the first add, so the whole CTA is one DRAM round trip deep
-// and a [12544 x 768] operand still spreads over 588 CTAs (with 256-row CTAs it was 150 CTAs walking 8 dependent
-// rounds: 16 us for 19 MB in the ncu capture, profiles/r2_*).  The 4-byte-load kernel above ran at ~0.3 of the HBM rate.
-// Partials per row chunk are summed by the last CTA of each column block — all 256 threads, 8 interleaved chunk lanes,
-// fixed order (deterministic).
-constexpr int COLSUM_WROWS = 64;
-constexpr bool VT_DEFAULT_COLSUM_WIDE = false;
-
-__global__ void __launch_bounds__(256)
-colsum_wide_kernel(const __nv_bfloat16* __restrict__ in, long long ld, int M, int N, float* __restrict__ ws,
-                   float* __restrict__ out, int* __restrict__ counters) {
-  const int lane = threadIdx.x & 31, rl = threadIdx.x >> 5;
-  const int col = blockIdx.x * 256 + lane * 8;
-  const int r0 = blockIdx.y * COLSUM_WROWS;
-  float acc[8];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-  if (col < N) {
-    const __nv_bfloat16* base = in + col;
-    uint4 u[COLSUM_WROWS / 8];
-#pragma unroll
-    for (int i = 0; i < COLSUM_WROWS / 8; ++i) {
-      const int r = r0 + rl + 8 * i;
-      u[i] = r < M ? *reinterpret_cast<const uint4*>(base + (long long)r * ld) : make_uint4(0u, 0u, 0u, 0u);
-    }
-#pragma unroll
-    for (int i = 0; i < COLSUM_WROWS / 8; ++i) {
-      const float2 a = unpack_bf16x2(u[i].x), b = unpack_bf16x2(u[i].y), c = unpack_bf16x2(u[i].z), d = unpack_bf16x2(u[i].w);
-      acc[0] += a.x; acc[1] += a.y; acc[2] += b.x; acc[3] += b.y; acc[4] += c.x; acc[5] += c.y; acc[6] += d.x; acc[7] += d.y;
-    }
-  }
-  __shared__ float sh[8][32][9];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) sh[rl][lane][j] = acc[j];
-  __syncthreads();
-  {
-    // thread t finalises column t of the block: lane t / 8, slot t % 8
-    const int l = threadIdx.x >> 3, j = threadIdx.x & 7;
-    float sum = 0.f;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) sum += sh[w][l][j];
-    const int c = blockIdx.x * 256 + threadIdx.x;
-    if (c < N) ws[(long long)blockIdx.y * N + c] = sum;
-  }
-  __shared__ int is_last;
-  __threadfence();
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const int done = atomicAdd(&counters[blockIdx.x], 1);
-    is_last = (done == (int)gridDim.y - 1);
-    if (is_last) counters[blockIdx.x] = 0;   // self-cleaning for the next call
-  }
-  __syncthreads();
-  if (!is_last) return;
-  __threadfence();
-  // chunk lane rl sums partial rows rl, rl + 8, ... of this lane's 8 columns; the 8 chunk lanes are then added in order
-#pragma unroll
-  for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-  if (col < N) {
-    for (int k = rl; k < (int)gridDim.y; k += 8) {
-      const float4 v0 = __ldcg(reinterpret_cast<const float4*>(ws + (long long)k * N + col));
-      const float4 v1 = __ldcg(reinterpret_cast<const float4*>(ws + (long long)k * N + col + 4));
-      acc[0] += v0.x; acc[1] += v0.y; acc[2] += v0.z; acc[3] += v0.w;
-      acc[4] += v1.x; acc[5] += v1.y; acc[6] += v1.z; acc[7] += v1.w;
-    }
-  }
-  __syncthreads();        // sh is reused
-#pragma unroll
-  for (int j = 0; j < 8; ++j) sh[rl][lane][j] = acc[j];
-  __syncthreads();
-  {
-    const int l = threadIdx.x >> 3, j = threadIdx.x & 7;
-    float sum = 0.f;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) sum += sh[w][l][j];
-    const int c = blockIdx.x * 256 + threadIdx.x;
-    if (c < N) out[c] = sum;
-  }
-}
-
 // ------------------------------------------------------------------------------------------------
 // im2col for non-overlapping patches / tubelets, and its adjoint
 //   cols[(b,t',hp,wp), ((c*tube+dt)*ph+i)*pw+j] = x[b, t'*tube+dt, c, hp*ph+i, wp*pw+j]
@@ -830,21 +749,13 @@ extern "C" int vt_gather_cast_bf16(const vt_gather_cast_params* p, void* stream)
 
 namespace vt { int launch_reduce_rows(const float*, float*, long long, int, long long, int, float, cudaStream_t); }
 
-extern "C" int vt_colsum_chunks(int32_t M) { return (M + COLSUM_WROWS - 1) / COLSUM_WROWS; }   // rows of the partial-sum workspace
-
+extern "C" int vt_colsum_chunks(int32_t M) { return (M + COLSUM_ROWS - 1) / COLSUM_ROWS; }   // rows of the partial-sum workspace
 
 extern "C" int vt_colsum_bf16(const vt_colsum_params* p, void* stream) {
   VT_REQUIRE(p && p->in && p->out && p->workspace && p->M > 0 && p->N > 0, "vt_colsum_bf16: bad params");
   VT_REQUIRE(p->N % 4 == 0 && p->ld % 2 == 0, "vt_colsum_bf16: N %% 4 and ld %% 2 required");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (p->counters && p->N % 8 == 0 && p->ld % 8 == 0 && (reinterpret_cast<uintptr_t>(p->in) & 15) == 0 &&
-      feature_on("VT_COLSUM_WIDE", VT_DEFAULT_COLSUM_WIDE)) {
-    dim3 wgrid((p->N + 255) / 256, (p->M + COLSUM_WROWS - 1) / COLSUM_WROWS);
-    colsum_wide_kernel<<<wgrid, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(p->in), p->ld, p->M, p->N, p->workspace, p->out,
-                                             p->counters);
-    return check_launch("colsum_wide_kernel");
-  }
-  const int chunks = (p->M + COLSUM_ROWS - 1) / COLSUM_ROWS;
+  const int chunks = vt_colsum_chunks(p->M);
   dim3 grid((p->N + 63) / 64, chunks);
   colsum_kernel<<<grid, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(p->in), p->ld, p->M, p->N, p->workspace, p->out,
                                       p->counters);

@@ -778,42 +778,12 @@ static int launch_gemm(const vt_gemm_params* q, GemmDev& d, cudaStream_t st) {
   return 0;
 }
 
-int launch_gemm_rows(const vt_gemm_params* q, int m0, void* stream);   // vt_gemm_rows.cu
-
 }  // namespace vt
-
-// M a few rows past a multiple of 128: tensor-core kernel on the full row tiles, CUDA-core dot products for the rest
-// (vt_gemm_rows.cu).  Plain row-major calls only; anything forced by a test goes through the one-kernel path.
-#ifndef VT_DEFAULT_ROWS_SPLIT
-#define VT_DEFAULT_ROWS_SPLIT false   // off: with persistent CTAs the 8-row tail tile costs less than the extra launch
-#endif
-static int rows_split_point(const vt_gemm_params* q) {
-  const int r = q->M % vt::BM;
-  if (r == 0 || r > 16 || q->M < 8 * vt::BM) return 0;
-  // the extra launch only pays where the partial row of tiles costs a long extra round: few n-tiles, long K
-  if (q->N > 1024 || q->K < 2048) return 0;
-  if (!vt::feature_on("VT_ROWS_SPLIT", VT_DEFAULT_ROWS_SPLIT)) return 0;
-  if (q->a_mn_major || (q->epilogue != VT_EPI_BF16 && q->epilogue != VT_EPI_F32)) return 0;
-  if (q->out_row || q->aux_row || q->map_period > 0 || q->debug || q->force_splits || q->force_bn || q->force_cluster || q->force_tail) return 0;
-  if (q->epilogue == VT_EPI_F32 && q->workspace && !q->aux && !q->bias && !q->row_scale) return 0;   // split-K candidates
-  if (q->K % 8 != 0 || q->lda % 8 != 0 || q->ldb % 8 != 0) return 0;
-  if ((reinterpret_cast<uintptr_t>(q->a) & 15) || (reinterpret_cast<uintptr_t>(q->b) & 15)) return 0;
-  return q->M - r;
-}
 
 static int gemm_dispatch(const vt_gemm_params* q, const float* a_scale, const float* b_scale, void* stream);
 
 extern "C" int vt_gemm(const vt_gemm_params* q, void* stream) {
-  using namespace vt;
   VT_REQUIRE(q != nullptr, "vt_gemm: null params");
-  const int m0 = (q->a && q->b && q->out && q->M > 0 && q->N > 0 && q->K > 0) ? rows_split_point(q) : 0;
-  if (m0 > 0) {
-    vt_gemm_params head = *q;
-    head.M = m0;
-    const int rc = gemm_dispatch(&head, nullptr, nullptr, stream);
-    if (rc) return rc;
-    return launch_gemm_rows(q, m0, stream);
-  }
   return gemm_dispatch(q, nullptr, nullptr, stream);
 }
 

@@ -1294,12 +1294,9 @@ int vt::layernorm_bwd_small(const vt_ln_bwd_params* p, void* stream) {
   return check_launch("ln_small_bwd_kernel");
 }
 
-// the 4-channels-per-lane kernels need 8-byte aligned token rows; VT_POOL_V2=0 selects the first generation
-#ifndef VT_DEFAULT_POOL_V2
-#define VT_DEFAULT_POOL_V2 true
-#endif
+// the 4-channels-per-lane kernels (second generation) need 8-byte aligned token rows; other views take the first
 static bool pool_v2(const void* ptr, long long bs, long long rs) {
-  return feature_on("VT_POOL_V2", VT_DEFAULT_POOL_V2) && ((uintptr_t)ptr & 7) == 0 && bs % 4 == 0 && rs % 4 == 0;
+  return ((uintptr_t)ptr & 7) == 0 && bs % 4 == 0 && rs % 4 == 0;
 }
 
 static int pool_dims_ok(int T, int Hin, int Win, int st, int sh, int sw, int To, int Ho, int Wo) {
