@@ -220,15 +220,17 @@ int vt_gelu_bwd_colsum_bf16(const vt_gelu_bwd_colsum_params* p, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
  * Multi-head softmax attention core on a packed qkv tensor (no projection):
- *   qkv bf16 [Bp, N, 3, H, hd] (the layout produced by transformer.py:167's reshape), hd = 64
+ *   qkv bf16 [Bp, N, 3, H, hd] (the layout produced by transformer.py:167's reshape), hd = 32, 64, 96 or 128 (every
+ *   kernel below at each; other widths are refused)
  *   ctx bf16 [Bp, N, H*hd] = softmax(q k^T * scale) v      (transformer.py:170-174)
  *   lse fp32 [Bp, H, N]   (saved for backward; NULL = not written, for every implementation);
  *   probs fp32 [Bp,H,N,N] optional (Attention returns it, :177; get_last_selfattention, video_transformer.py:258-261)
  * Three kernels behind one entry point: tensor-core flash kernels for any N > 32 (the spatial pass N = 197, the joint
  * space-time pass N = 1569; mma.sync bf16 with fp32 accumulators, K/V tiles double-buffered in shared memory by cp.async,
  * vt_attention_mma.cu), a warp-per-problem kernel for the temporal pass (N = 8, 18 816 problems/layer), and a generic
- * warp-per-query kernel for N <= 256 (ViViT N = 9, probs output).  With the tensor-core kernels the probs output comes
- * from a row-tile softmax kernel that fits 8 rows of scores in shared memory (N <= ~6000).
+ * warp-per-query kernel for N <= 256 (ViViT N = 9, probs output; its backward at hd 128 holds up to N = 208).  The
+ * whole-problem tensor-core kernels take hd 64 only; other widths run the 64-row tiles.  With the tensor-core kernels the
+ * probs output comes from a row-tile softmax kernel that fits 8 rows of scores in shared memory (N <= ~5000).
  * VT_ATTN_TCGEN05 selects the tensor-core kernel (the name is kept for ABI compatibility).
  * ------------------------------------------------------------------------------------------- */
 enum { VT_ATTN_AUTO = 0, VT_ATTN_GENERIC = 1, VT_ATTN_TCGEN05 = 2, VT_ATTN_WARP8 = 3 };

@@ -1,4 +1,5 @@
-// Tensor-core flash attention for sm_90a (mma.sync.m16n8k16, bf16 operands, fp32 accumulators), head dim 64 or 96.
+// Tensor-core flash attention for sm_90a (mma.sync.m16n8k16, bf16 operands, fp32 accumulators), head dim 32, 64, 96 or
+// 128 (vt_xattn_* takes 64 and 96).
 // One kernel family serves both entry points: the packed-qkv attention of vt_attn_* (the 197-token spatial pass) and the
 // strided pooling / long-sequence attention of vt_xattn_* (Nq != Nk).  Operands are addressed as
 // base + b * bs + h * hs + n * rs (bf16 rows, 16-byte aligned), so q / k / v / dq are read and written in place.
@@ -12,7 +13,7 @@
 // two-stage ring (the next tile's loads are in flight while the current tile's MMAs run); rows past Nq / Nk are
 // zero-filled by the copy (src-size 0) and never read.  MMA fragments come from ldmatrix.x4, the .trans form for operands
 // used transposed (V in P V, K in dS K, Q and dO in the dK / dV MMAs).  The HD + 8 pitch puts the 8 rows read by every
-// ldmatrix phase in distinct banks at both head dims, so no swizzle is needed.  MMAs whose operands are all padding are
+// ldmatrix phase in distinct banks at every head dim (row pitch 80, 144, 208 or 272 bytes), so no swizzle is needed.  MMAs whose operands are all padding are
 // skipped: a warp whose 16 rows lie past the end issues none, and on a partial last tile only the n8 blocks of S and the
 // k16 chunks of the second product that hold a valid key (dK / dV: query) run; the skipped terms are exact zeros.
 //
@@ -419,7 +420,7 @@ __device__ __forceinline__ void dkv_store(const float (&dk)[HD / 8][4], const fl
 // ------------------------------------------------------------------------------------------------ forward
 // shared memory: Q, then a ring of two (K, V) stages
 template <int HD, bool LSE>
-__global__ void __launch_bounds__(MMA_THREADS) attn_mma_fwd_kernel(const MmaAttn p) {
+__device__ __forceinline__ void mma_fwd(const MmaAttn& p) {
   constexpr int TILE = MT * (HD + 8);
   extern __shared__ __align__(16) uint8_t mma_smem[];
   __nv_bfloat16* Qs = reinterpret_cast<__nv_bfloat16*>(mma_smem);
@@ -459,7 +460,7 @@ __global__ void __launch_bounds__(MMA_THREADS) attn_mma_fwd_kernel(const MmaAttn
 // ------------------------------------------------------------------------------------------------ dQ
 // shared memory: Q, dO, a ring of two (K, V) stages, lse and delta of the CTA's rows
 template <int HD>
-__global__ void __launch_bounds__(MMA_THREADS) attn_mma_dq_kernel(const MmaAttn p) {
+__device__ __forceinline__ void mma_dq(const MmaAttn& p) {
   constexpr int TILE = MT * (HD + 8);
   extern __shared__ __align__(16) uint8_t mma_smem[];
   __nv_bfloat16* Qs = reinterpret_cast<__nv_bfloat16*>(mma_smem);
@@ -508,9 +509,8 @@ __global__ void __launch_bounds__(MMA_THREADS) attn_mma_dq_kernel(const MmaAttn 
 
 // ------------------------------------------------------------------------------------------------ dK / dV
 // shared memory: K, V, a ring of two (Q, dO, O) stages, the ring's two lse rows, lse and delta of the current query tile.
-// At head dim 64 three CTAs fit an SM (162 registers without spills, 75 KB); at 96 the register cap would spill.
 template <int HD>
-__global__ void __launch_bounds__(MMA_THREADS, HD == 64 ? 3 : 1) attn_mma_dkv_kernel(const MmaAttn p) {
+__device__ __forceinline__ void mma_dkv(const MmaAttn& p) {
   constexpr int TILE = MT * (HD + 8);
   extern __shared__ __align__(16) uint8_t mma_smem[];
   __nv_bfloat16* Ks = reinterpret_cast<__nv_bfloat16*>(mma_smem);
@@ -559,6 +559,27 @@ __global__ void __launch_bounds__(MMA_THREADS, HD == 64 ? 3 : 1) attn_mma_dkv_ke
   }
   if (active) dkv_store<HD>(dk, dv, p, b, h, k0 + rb, p.dk32 != nullptr);
 }
+
+// ------------------------------------------------------------------------------------------------ kernels
+// Head dims 64 (ViT-B) and 96 (MViT) are the attn_mma_* kernels.  The packed-qkv widths 32 and 128 run the same bodies
+// under their own names (attn_tc_*), so each width's resources can be checked and profiled on its own.  dK / dV: at head
+// dim 64 three CTAs fit an SM (162 registers without spills, 75 KB); at 96 and 128 the register cap of more would spill;
+// at 32 four fit.
+template <int HD>
+constexpr int dkv_min_ctas() { return HD == 32 ? 4 : HD == 64 ? 3 : 1; }
+
+template <int HD, bool LSE>
+__global__ void __launch_bounds__(MMA_THREADS) attn_mma_fwd_kernel(const MmaAttn p) { mma_fwd<HD, LSE>(p); }
+template <int HD>
+__global__ void __launch_bounds__(MMA_THREADS) attn_mma_dq_kernel(const MmaAttn p) { mma_dq<HD>(p); }
+template <int HD>
+__global__ void __launch_bounds__(MMA_THREADS, dkv_min_ctas<HD>()) attn_mma_dkv_kernel(const MmaAttn p) { mma_dkv<HD>(p); }
+template <int HD, bool LSE>
+__global__ void __launch_bounds__(MMA_THREADS) attn_tc_fwd_kernel(const MmaAttn p) { mma_fwd<HD, LSE>(p); }
+template <int HD>
+__global__ void __launch_bounds__(MMA_THREADS) attn_tc_dq_kernel(const MmaAttn p) { mma_dq<HD>(p); }
+template <int HD>
+__global__ void __launch_bounds__(MMA_THREADS, dkv_min_ctas<HD>()) attn_tc_dkv_kernel(const MmaAttn p) { mma_dkv<HD>(p); }
 
 // ------------------------------------------------------------------------------------------------ whole problems
 // Packed-qkv attention at head dim 64 and N <= WHOLE_MAX_N (Nq == Nk): a CTA owns one (b, h) problem and keeps its
@@ -745,29 +766,43 @@ static int launch(dim3 grid, int smem, const MmaAttn& a, cudaStream_t st, const 
   return check_launch(what);
 }
 
+template <int HD>
+static int mma_fwd_launch(const MmaAttn& a, dim3 grid, cudaStream_t st) {
+  if constexpr (HD == 64 || HD == 96) {
+    const char* what = "attn_mma_fwd_kernel";
+    if (a.lse) return launch<attn_mma_fwd_kernel<HD, true>>(grid, fwd_smem<HD>(), a, st, what);
+    return launch<attn_mma_fwd_kernel<HD, false>>(grid, fwd_smem<HD>(), a, st, what);
+  } else {
+    const char* what = "attn_tc_fwd_kernel";
+    if (a.lse) return launch<attn_tc_fwd_kernel<HD, true>>(grid, fwd_smem<HD>(), a, st, what);
+    return launch<attn_tc_fwd_kernel<HD, false>>(grid, fwd_smem<HD>(), a, st, what);
+  }
+}
+
+template <int HD>
+static int mma_bwd_launch(const MmaAttn& a, dim3 gq, dim3 gk, cudaStream_t st) {
+  int rc;
+  if constexpr (HD == 64 || HD == 96) {
+    if ((rc = launch<attn_mma_dq_kernel<HD>>(gq, dq_smem<HD>(), a, st, "attn_mma_dq_kernel"))) return rc;
+    return launch<attn_mma_dkv_kernel<HD>>(gk, dkv_smem<HD>(), a, st, "attn_mma_dkv_kernel");
+  } else {
+    if ((rc = launch<attn_tc_dq_kernel<HD>>(gq, dq_smem<HD>(), a, st, "attn_tc_dq_kernel"))) return rc;
+    return launch<attn_tc_dkv_kernel<HD>>(gk, dkv_smem<HD>(), a, st, "attn_tc_dkv_kernel");
+  }
+}
+
 int attn_mma_fwd(const MmaAttn& a, int B, int hd, cudaStream_t st) {
-  VT_REQUIRE(hd == 64 || hd == 96, "tensor-core attention: head dim %d unsupported (64 or 96)", hd);
+  VT_REQUIRE(attn_head_dim_ok(hd), "tensor-core attention: head dim %d unsupported (32, 64, 96 or 128)", hd);
   VT_REQUIRE((long long)B * a.H <= 65535, "tensor-core attention: B*H too large");
   const dim3 grid((a.Nq + MT - 1) / MT, B * a.H);
-  const char* what = "attn_mma_fwd_kernel";
-  if (hd == 64)
-    return a.lse ? launch<attn_mma_fwd_kernel<64, true>>(grid, fwd_smem<64>(), a, st, what)
-                 : launch<attn_mma_fwd_kernel<64, false>>(grid, fwd_smem<64>(), a, st, what);
-  return a.lse ? launch<attn_mma_fwd_kernel<96, true>>(grid, fwd_smem<96>(), a, st, what)
-               : launch<attn_mma_fwd_kernel<96, false>>(grid, fwd_smem<96>(), a, st, what);
+  return with_head_dim(hd, [&](auto d) { return mma_fwd_launch<d.value>(a, grid, st); });
 }
 
 int attn_mma_bwd(const MmaAttn& a, int B, int hd, cudaStream_t st) {
-  VT_REQUIRE(hd == 64 || hd == 96, "tensor-core attention: head dim %d unsupported (64 or 96)", hd);
+  VT_REQUIRE(attn_head_dim_ok(hd), "tensor-core attention: head dim %d unsupported (32, 64, 96 or 128)", hd);
   VT_REQUIRE((long long)B * a.H <= 65535, "tensor-core attention: B*H too large");
-  int rc;
   const dim3 gq((a.Nq + MT - 1) / MT, B * a.H), gk((a.Nk + MT - 1) / MT, B * a.H);
-  if (hd == 64) {
-    if ((rc = launch<attn_mma_dq_kernel<64>>(gq, dq_smem<64>(), a, st, "attn_mma_dq_kernel"))) return rc;
-    return launch<attn_mma_dkv_kernel<64>>(gk, dkv_smem<64>(), a, st, "attn_mma_dkv_kernel");
-  }
-  if ((rc = launch<attn_mma_dq_kernel<96>>(gq, dq_smem<96>(), a, st, "attn_mma_dq_kernel"))) return rc;
-  return launch<attn_mma_dkv_kernel<96>>(gk, dkv_smem<96>(), a, st, "attn_mma_dkv_kernel");
+  return with_head_dim(hd, [&](auto d) { return mma_bwd_launch<d.value>(a, gq, gk, st); });
 }
 
 bool attn_whole_ok(const MmaAttn& a, int hd) {

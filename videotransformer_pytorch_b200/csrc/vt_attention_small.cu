@@ -1,42 +1,62 @@
 // Temporal attention of the divided space-time block: 8 frames x 8 frames per (sample, patch, head) —
 // 18 816 independent 8x8x64 problems per layer at batch 8.  0.1 % of the FLOPs, so the kernel is built
 // to be bandwidth/latency lean instead of tensor-core shaped: one warp per problem, Q/K/V (and dO) rows
-// staged in shared memory (33-word pitch, conflict-free), lane (i, g) = query row i = lane/4 and quarter
-// g = lane%4:  scores for keys {2g, 2g+1} (full 64-dim dots), softmax across the 4 lanes of a row with two
-// shuffles, then the lane owns features [16g, 16g+16) of its output row.  Backward uses the same mapping
-// (dQ rows, then dK/dV rows) and recomputes P from the saved log-sum-exp.
+// staged in shared memory (HD / 2 + 1-word pitch, odd: conflict-free), lane (i, g) = query row i = lane/4 and quarter
+// g = lane%4:  scores for keys {2g, 2g+1} (full HD-dim dots), softmax across the 4 lanes of a row with two
+// shuffles, then the lane owns features [g HD/4, (g+1) HD/4) of its output row.  Backward uses the same mapping
+// (dQ rows, then dK/dV rows) and recomputes P from the saved log-sum-exp.  Instantiated at head dims 32, 64, 96 and 128;
+// at 96 and 128 a CTA has 4 warps so that the backward's staged rows stay within 48 KB of static shared memory.
 #include "vt_common.cuh"
 
 namespace vt {
 
 constexpr int SM_N = 8;
-constexpr int SM_HD = 64;
-constexpr int SM_PITCH = 33;
-constexpr int SM_WARPS = 8;
+
+template <int HD>
+struct Attn8 {
+  static constexpr int PITCH = HD / 2 + 1;     // words per staged row
+  static constexpr int FW = HD / 8;            // words of a lane's quarter of a row
+  static constexpr int CPR = HD / 8;           // 16-byte chunks per row
+  static constexpr int RPL = SM_N * CPR / 32;  // chunks of an 8-row operand per lane
+  static constexpr int WARPS = HD <= 64 ? 8 : 4;
+  // row and 16-byte chunk of chunk lane + 32 it of an 8-row operand (a whole number of rows per 32 chunks but at 96)
+  static __device__ __forceinline__ int row(int lane, int it) {
+    return 32 % CPR == 0 ? lane / CPR + 32 / CPR * it : (lane + 32 * it) / CPR;
+  }
+  static __device__ __forceinline__ int col(int lane, int it) { return 32 % CPR == 0 ? lane % CPR : (lane + 32 * it) % CPR; }
+};
 
 // software pipelining: the next problem's rows are fetched into registers while the current one is computed
-struct Rows8 { uint4 v[2]; };
-__device__ __forceinline__ Rows8 fetch_rows8(const __nv_bfloat16* base, long long row_stride, int lane) {
-  Rows8 r;
+template <int HD>
+struct Rows8 { uint4 v[Attn8<HD>::RPL]; };
+template <int HD>
+__device__ __forceinline__ Rows8<HD> fetch_rows8(const __nv_bfloat16* base, long long row_stride, int lane) {
+  using C = Attn8<HD>;
+  Rows8<HD> r;
 #pragma unroll
-  for (int it = 0; it < 2; ++it) {
-    const int row = (lane >> 3) + 4 * it, c = lane & 7;
+  for (int it = 0; it < C::RPL; ++it) {
+    const int row = C::row(lane, it), c = C::col(lane, it);
     r.v[it] = *reinterpret_cast<const uint4*>(base + (long long)row * row_stride + c * 8);
   }
   return r;
 }
-__device__ __forceinline__ void put_rows8(uint32_t* dst, const Rows8& r, int lane) {
+template <int HD>
+__device__ __forceinline__ void put_rows8(uint32_t* dst, const Rows8<HD>& r, int lane) {
+  using C = Attn8<HD>;
 #pragma unroll
-  for (int it = 0; it < 2; ++it) {
-    const int row = (lane >> 3) + 4 * it, c = lane & 7;
-    uint32_t* d = dst + row * SM_PITCH + c * 4;
+  for (int it = 0; it < C::RPL; ++it) {
+    const int row = C::row(lane, it), c = C::col(lane, it);
+    uint32_t* d = dst + row * C::PITCH + c * 4;
     d[0] = r.v[it].x; d[1] = r.v[it].y; d[2] = r.v[it].z; d[3] = r.v[it].w;
   }
 }
 
-__global__ void __launch_bounds__(SM_WARPS * 32)
+template <int HD>
+__global__ void __launch_bounds__(Attn8<HD>::WARPS * 32)
 attn8_fwd_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict__ ctx, float* __restrict__ lse,
                  int nprob, int H, float scale) {
+  using C = Attn8<HD>;
+  constexpr int SM_WARPS = C::WARPS, SM_PITCH = C::PITCH, FW = C::FW;
   __shared__ uint32_t sh[SM_WARPS][3][SM_N * SM_PITCH];
   __shared__ float shp[SM_WARPS][SM_N * 9];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -44,27 +64,27 @@ attn8_fwd_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
   uint32_t* Ks = sh[warp][1];
   uint32_t* Vs = sh[warp][2];
   float* Ps = shp[warp];
-  const long long rs = 3LL * H * SM_HD, cs = (long long)H * SM_HD;
+  const long long rs = 3LL * H * HD, cs = (long long)H * HD;
   const int i = lane >> 2, g = lane & 3;
   const int pstep = gridDim.x * SM_WARPS;
   int prob = blockIdx.x * SM_WARPS + warp;
-  Rows8 rq, rk, rv;
+  Rows8<HD> rq, rk, rv;
   if (prob < nprob) {
-    const __nv_bfloat16* b0 = qkv + (long long)(prob / H) * SM_N * rs + (prob % H) * SM_HD;
-    rq = fetch_rows8(b0, rs, lane); rk = fetch_rows8(b0 + cs, rs, lane); rv = fetch_rows8(b0 + 2 * cs, rs, lane);
+    const __nv_bfloat16* b0 = qkv + (long long)(prob / H) * SM_N * rs + (prob % H) * HD;
+    rq = fetch_rows8<HD>(b0, rs, lane); rk = fetch_rows8<HD>(b0 + cs, rs, lane); rv = fetch_rows8<HD>(b0 + 2 * cs, rs, lane);
   }
   for (; prob < nprob; prob += pstep) {
     const int bp = prob / H, h = prob - bp * H;
-    put_rows8(Qs, rq, lane); put_rows8(Ks, rk, lane); put_rows8(Vs, rv, lane);
+    put_rows8<HD>(Qs, rq, lane); put_rows8<HD>(Ks, rk, lane); put_rows8<HD>(Vs, rv, lane);
     __syncwarp();
     if (prob + pstep < nprob) {
       const int np = prob + pstep;
-      const __nv_bfloat16* b1 = qkv + (long long)(np / H) * SM_N * rs + (np % H) * SM_HD;
-      rq = fetch_rows8(b1, rs, lane); rk = fetch_rows8(b1 + cs, rs, lane); rv = fetch_rows8(b1 + 2 * cs, rs, lane);
+      const __nv_bfloat16* b1 = qkv + (long long)(np / H) * SM_N * rs + (np % H) * HD;
+      rq = fetch_rows8<HD>(b1, rs, lane); rk = fetch_rows8<HD>(b1 + cs, rs, lane); rv = fetch_rows8<HD>(b1 + 2 * cs, rs, lane);
     }
     float s0 = 0.f, s1 = 0.f;
 #pragma unroll 8
-    for (int w = 0; w < 32; ++w) {
+    for (int w = 0; w < HD / 2; ++w) {
       const float2 q = unpack_bf16x2(Qs[i * SM_PITCH + w]);
       const float2 k0 = unpack_bf16x2(Ks[(2 * g) * SM_PITCH + w]);
       const float2 k1 = unpack_bf16x2(Ks[(2 * g + 1) * SM_PITCH + w]);
@@ -84,35 +104,39 @@ attn8_fwd_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restric
     Ps[i * 9 + 2 * g + 1] = e1 * inv;
     if (g == 0 && lse) lse[(long long)prob * SM_N + i] = m + __logf(l);
     __syncwarp();
-    float acc[16];
+    float acc[2 * FW];
 #pragma unroll
-    for (int d = 0; d < 16; ++d) acc[d] = 0.f;
+    for (int d = 0; d < 2 * FW; ++d) acc[d] = 0.f;
 #pragma unroll
     for (int j = 0; j < SM_N; ++j) {
       const float p = Ps[i * 9 + j];
 #pragma unroll
-      for (int w = 0; w < 8; ++w) {
-        const float2 v = unpack_bf16x2(Vs[j * SM_PITCH + g * 8 + w]);
+      for (int w = 0; w < FW; ++w) {
+        const float2 v = unpack_bf16x2(Vs[j * SM_PITCH + g * FW + w]);
         acc[2 * w] = fmaf(p, v.x, acc[2 * w]);
         acc[2 * w + 1] = fmaf(p, v.y, acc[2 * w + 1]);
       }
     }
-    uint4 o0, o1;
-    o0.x = pack_bf16x2(acc[0], acc[1]);   o0.y = pack_bf16x2(acc[2], acc[3]);
-    o0.z = pack_bf16x2(acc[4], acc[5]);   o0.w = pack_bf16x2(acc[6], acc[7]);
-    o1.x = pack_bf16x2(acc[8], acc[9]);   o1.y = pack_bf16x2(acc[10], acc[11]);
-    o1.z = pack_bf16x2(acc[12], acc[13]); o1.w = pack_bf16x2(acc[14], acc[15]);
-    uint4* dst = reinterpret_cast<uint4*>(ctx + ((long long)bp * SM_N + i) * cs + h * SM_HD + g * 16);
-    dst[0] = o0;
-    dst[1] = o1;
+    uint4 o[FW / 4];
+#pragma unroll
+    for (int u = 0; u < FW / 4; ++u) {
+      o[u].x = pack_bf16x2(acc[8 * u], acc[8 * u + 1]);     o[u].y = pack_bf16x2(acc[8 * u + 2], acc[8 * u + 3]);
+      o[u].z = pack_bf16x2(acc[8 * u + 4], acc[8 * u + 5]); o[u].w = pack_bf16x2(acc[8 * u + 6], acc[8 * u + 7]);
+    }
+    uint4* dst = reinterpret_cast<uint4*>(ctx + ((long long)bp * SM_N + i) * cs + h * HD + g * (HD / 4));
+#pragma unroll
+    for (int u = 0; u < FW / 4; ++u) dst[u] = o[u];
     __syncwarp();
   }
 }
 
-__global__ void __launch_bounds__(SM_WARPS * 32)
+template <int HD>
+__global__ void __launch_bounds__(Attn8<HD>::WARPS * 32)
 attn8_bwd_kernel(const __nv_bfloat16* __restrict__ qkv, const __nv_bfloat16* __restrict__ ctx,
                  const __nv_bfloat16* __restrict__ dctx, const float* __restrict__ lse, __nv_bfloat16* __restrict__ dqkv,
                  int nprob, int H, float scale) {
+  using C = Attn8<HD>;
+  constexpr int SM_WARPS = C::WARPS, SM_PITCH = C::PITCH, FW = C::FW;
   __shared__ uint32_t sh[SM_WARPS][4][SM_N * SM_PITCH];
   __shared__ float shp[SM_WARPS][2][SM_N * 9];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -122,38 +146,38 @@ attn8_bwd_kernel(const __nv_bfloat16* __restrict__ qkv, const __nv_bfloat16* __r
   uint32_t* Gs = sh[warp][3];   // dO
   float* Ps = shp[warp][0];
   float* Ds = shp[warp][1];     // dS
-  const long long rs = 3LL * H * SM_HD, cs = (long long)H * SM_HD;
+  const long long rs = 3LL * H * HD, cs = (long long)H * HD;
   const int i = lane >> 2, g = lane & 3;
   const int pstep = gridDim.x * SM_WARPS;
   int prob = blockIdx.x * SM_WARPS + warp;
-  Rows8 rq, rk, rv, rg;
+  Rows8<HD> rq, rk, rv, rg;
   if (prob < nprob) {
-    const __nv_bfloat16* b0 = qkv + (long long)(prob / H) * SM_N * rs + (prob % H) * SM_HD;
-    rq = fetch_rows8(b0, rs, lane); rk = fetch_rows8(b0 + cs, rs, lane); rv = fetch_rows8(b0 + 2 * cs, rs, lane);
-    rg = fetch_rows8(dctx + (long long)(prob / H) * SM_N * cs + (prob % H) * SM_HD, cs, lane);
+    const __nv_bfloat16* b0 = qkv + (long long)(prob / H) * SM_N * rs + (prob % H) * HD;
+    rq = fetch_rows8<HD>(b0, rs, lane); rk = fetch_rows8<HD>(b0 + cs, rs, lane); rv = fetch_rows8<HD>(b0 + 2 * cs, rs, lane);
+    rg = fetch_rows8<HD>(dctx + (long long)(prob / H) * SM_N * cs + (prob % H) * HD, cs, lane);
   }
   for (; prob < nprob; prob += pstep) {
     const int bp = prob / H, h = prob - bp * H;
-    put_rows8(Qs, rq, lane); put_rows8(Ks, rk, lane); put_rows8(Vs, rv, lane); put_rows8(Gs, rg, lane);
+    put_rows8<HD>(Qs, rq, lane); put_rows8<HD>(Ks, rk, lane); put_rows8<HD>(Vs, rv, lane); put_rows8<HD>(Gs, rg, lane);
     __syncwarp();
     if (prob + pstep < nprob) {
       const int np = prob + pstep;
-      const __nv_bfloat16* b1 = qkv + (long long)(np / H) * SM_N * rs + (np % H) * SM_HD;
-      rq = fetch_rows8(b1, rs, lane); rk = fetch_rows8(b1 + cs, rs, lane); rv = fetch_rows8(b1 + 2 * cs, rs, lane);
-      rg = fetch_rows8(dctx + (long long)(np / H) * SM_N * cs + (np % H) * SM_HD, cs, lane);
+      const __nv_bfloat16* b1 = qkv + (long long)(np / H) * SM_N * rs + (np % H) * HD;
+      rq = fetch_rows8<HD>(b1, rs, lane); rk = fetch_rows8<HD>(b1 + cs, rs, lane); rv = fetch_rows8<HD>(b1 + 2 * cs, rs, lane);
+      rg = fetch_rows8<HD>(dctx + (long long)(np / H) * SM_N * cs + (np % H) * HD, cs, lane);
     }
-    // delta_i = dO_i . O_i  (each lane: its 16 features, then reduce over the 4 lanes of the row)
+    // delta_i = dO_i . O_i  (each lane: its HD / 4 features, then reduce over the 4 lanes of the row)
     float del = 0.f;
     {
-      const uint4* o4 = reinterpret_cast<const uint4*>(ctx + ((long long)bp * SM_N + i) * cs + h * SM_HD + g * 16);
+      const uint4* o4 = reinterpret_cast<const uint4*>(ctx + ((long long)bp * SM_N + i) * cs + h * HD + g * (HD / 4));
 #pragma unroll
-      for (int u = 0; u < 2; ++u) {
+      for (int u = 0; u < FW / 4; ++u) {
         const uint4 o = o4[u];
         const uint32_t ow[4] = {o.x, o.y, o.z, o.w};
 #pragma unroll
         for (int w = 0; w < 4; ++w) {
           const float2 a = unpack_bf16x2(ow[w]);
-          const float2 b = unpack_bf16x2(Gs[i * SM_PITCH + g * 8 + u * 4 + w]);
+          const float2 b = unpack_bf16x2(Gs[i * SM_PITCH + g * FW + u * 4 + w]);
           del = fmaf(a.x, b.x, fmaf(a.y, b.y, del));
         }
       }
@@ -162,7 +186,7 @@ attn8_bwd_kernel(const __nv_bfloat16* __restrict__ qkv, const __nv_bfloat16* __r
     }
     float s0 = 0.f, s1 = 0.f, p0 = 0.f, p1 = 0.f;   // scores and dP for keys 2g, 2g+1
 #pragma unroll 8
-    for (int w = 0; w < 32; ++w) {
+    for (int w = 0; w < HD / 2; ++w) {
       const float2 q = unpack_bf16x2(Qs[i * SM_PITCH + w]);
       const float2 d = unpack_bf16x2(Gs[i * SM_PITCH + w]);
       const float2 k0 = unpack_bf16x2(Ks[(2 * g) * SM_PITCH + w]);
@@ -181,63 +205,74 @@ attn8_bwd_kernel(const __nv_bfloat16* __restrict__ qkv, const __nv_bfloat16* __r
     Ds[i * 9 + 2 * g] = e0 * (p0 - del) * scale;
     Ds[i * 9 + 2 * g + 1] = e1 * (p1 - del) * scale;
     __syncwarp();
-    float aq[16], ak[16], av[16];
+    float aq[2 * FW], ak[2 * FW], av[2 * FW];
 #pragma unroll
-    for (int d = 0; d < 16; ++d) { aq[d] = 0.f; ak[d] = 0.f; av[d] = 0.f; }
-    // lane (i,g): dQ_i[16g..] = sum_j dS[i][j] K_j ;  as key row i: dK_i = sum_q dS[q][i] Q_q ; dV_i = sum_q P[q][i] dO_q
+    for (int d = 0; d < 2 * FW; ++d) { aq[d] = 0.f; ak[d] = 0.f; av[d] = 0.f; }
+    // lane (i,g): dQ_i[g HD/4..] = sum_j dS[i][j] K_j ;  as key row i: dK_i = sum_q dS[q][i] Q_q ; dV_i = sum_q P[q][i] dO_q
 #pragma unroll
     for (int j = 0; j < SM_N; ++j) {
       const float dsq = Ds[i * 9 + j];
       const float dsk = Ds[j * 9 + i];
       const float pk = Ps[j * 9 + i];
 #pragma unroll
-      for (int w = 0; w < 8; ++w) {
-        const float2 k = unpack_bf16x2(Ks[j * SM_PITCH + g * 8 + w]);
-        const float2 q = unpack_bf16x2(Qs[j * SM_PITCH + g * 8 + w]);
-        const float2 d = unpack_bf16x2(Gs[j * SM_PITCH + g * 8 + w]);
+      for (int w = 0; w < FW; ++w) {
+        const float2 k = unpack_bf16x2(Ks[j * SM_PITCH + g * FW + w]);
+        const float2 q = unpack_bf16x2(Qs[j * SM_PITCH + g * FW + w]);
+        const float2 d = unpack_bf16x2(Gs[j * SM_PITCH + g * FW + w]);
         aq[2 * w] = fmaf(dsq, k.x, aq[2 * w]); aq[2 * w + 1] = fmaf(dsq, k.y, aq[2 * w + 1]);
         ak[2 * w] = fmaf(dsk, q.x, ak[2 * w]); ak[2 * w + 1] = fmaf(dsk, q.y, ak[2 * w + 1]);
         av[2 * w] = fmaf(pk, d.x, av[2 * w]);  av[2 * w + 1] = fmaf(pk, d.y, av[2 * w + 1]);
       }
     }
-    __nv_bfloat16* obase = dqkv + ((long long)bp * SM_N + i) * rs + h * SM_HD + g * 16;
+    __nv_bfloat16* obase = dqkv + ((long long)bp * SM_N + i) * rs + h * HD + g * (HD / 4);
 #pragma unroll
     for (int slot = 0; slot < 3; ++slot) {
       const float* a = slot == 0 ? aq : (slot == 1 ? ak : av);
-      uint4 o0, o1;
-      o0.x = pack_bf16x2(a[0], a[1]);   o0.y = pack_bf16x2(a[2], a[3]);
-      o0.z = pack_bf16x2(a[4], a[5]);   o0.w = pack_bf16x2(a[6], a[7]);
-      o1.x = pack_bf16x2(a[8], a[9]);   o1.y = pack_bf16x2(a[10], a[11]);
-      o1.z = pack_bf16x2(a[12], a[13]); o1.w = pack_bf16x2(a[14], a[15]);
       uint4* dst = reinterpret_cast<uint4*>(obase + slot * cs);
-      dst[0] = o0;
-      dst[1] = o1;
+#pragma unroll
+      for (int u = 0; u < FW / 4; ++u) {
+        const float* b = a + 8 * u;
+        dst[u] = make_uint4(pack_bf16x2(b[0], b[1]), pack_bf16x2(b[2], b[3]), pack_bf16x2(b[4], b[5]), pack_bf16x2(b[6], b[7]));
+      }
     }
     __syncwarp();
   }
 }
 
-// persistent grid = resident CTAs (register-limited: 3/SM forward, 2/SM backward) so that every warp walks several
-// problems and the register prefetch of the next problem overlaps the current one
+// persistent grid = resident CTAs (register-limited; at head dim 64 3/SM forward, 2/SM backward) so that every warp walks
+// several problems and the register prefetch of the next problem overlaps the current one
+template <int HD>
 static int small_grid(int nprob, int ctas_per_sm) {
+  constexpr int SM_WARPS = Attn8<HD>::WARPS;
   int blocks = (nprob + SM_WARPS - 1) / SM_WARPS;
   const int cap = sm_count() * ctas_per_sm;
   return blocks < cap ? blocks : cap;
 }
 
+// resident CTAs per SM of the forward / backward at each head dim, from their ptxas register counts (forward 48, 64, 128,
+// 128 registers; backward 64, 80, 128, 168 at head dim 32, 64, 96, 128; 8 warps per CTA up to 64, 4 above)
+template <int HD> constexpr int attn8_fwd_ctas() { return HD == 32 ? 5 : HD == 64 ? 3 : 4; }
+template <int HD> constexpr int attn8_bwd_ctas() { return HD == 32 ? 4 : HD == 64 ? 2 : HD == 96 ? 4 : 3; }
+
 int attn8_fwd_launch(const vt_attn_fwd_params* p, cudaStream_t st) {
   const int nprob = p->Bp * p->H;
-  attn8_fwd_kernel<<<small_grid(nprob, 3), SM_WARPS * 32, 0, st>>>(static_cast<const __nv_bfloat16*>(p->qkv),
-                                                                static_cast<__nv_bfloat16*>(p->ctx), p->lse, nprob, p->H, p->scale);
-  return check_launch("attn8_fwd_kernel");
+  return with_head_dim(p->hd, [&](auto hd) {
+    constexpr int HD = hd.value;
+    attn8_fwd_kernel<HD><<<small_grid<HD>(nprob, attn8_fwd_ctas<HD>()), Attn8<HD>::WARPS * 32, 0, st>>>(
+        static_cast<const __nv_bfloat16*>(p->qkv), static_cast<__nv_bfloat16*>(p->ctx), p->lse, nprob, p->H, p->scale);
+    return check_launch("attn8_fwd_kernel");
+  });
 }
 
 int attn8_bwd_launch(const vt_attn_bwd_params* p, cudaStream_t st) {
   const int nprob = p->Bp * p->H;
-  attn8_bwd_kernel<<<small_grid(nprob, 2), SM_WARPS * 32, 0, st>>>(
-      static_cast<const __nv_bfloat16*>(p->qkv), static_cast<const __nv_bfloat16*>(p->ctx),
-      static_cast<const __nv_bfloat16*>(p->dctx), p->lse, static_cast<__nv_bfloat16*>(p->dqkv), nprob, p->H, p->scale);
-  return check_launch("attn8_bwd_kernel");
+  return with_head_dim(p->hd, [&](auto hd) {
+    constexpr int HD = hd.value;
+    attn8_bwd_kernel<HD><<<small_grid<HD>(nprob, attn8_bwd_ctas<HD>()), Attn8<HD>::WARPS * 32, 0, st>>>(
+        static_cast<const __nv_bfloat16*>(p->qkv), static_cast<const __nv_bfloat16*>(p->ctx),
+        static_cast<const __nv_bfloat16*>(p->dctx), p->lse, static_cast<__nv_bfloat16*>(p->dqkv), nprob, p->H, p->scale);
+    return check_launch("attn8_bwd_kernel");
+  });
 }
 
 }  // namespace vt

@@ -5,6 +5,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <type_traits>
+
 #include "../../include/vt_b200.h"
 
 namespace vt {
@@ -30,7 +32,31 @@ int layernorm_fwd_small(const vt_ln_fwd_params* p, void* stream);
 int layernorm_bwd_small(const vt_ln_bwd_params* p, void* stream);
 int persistent_sm_count();   // sm_count() minus vt_set_reserved_sms(): the SM count the GEMM tile planning assumes
 
+// Head widths of the packed-qkv attention kernels (vt_attn_*).  with_head_dim(hd, f) returns
+// f(std::integral_constant<int, hd>{}) for a width attn_head_dim_ok accepts, so each kernel is instantiated per width.
+inline bool attn_head_dim_ok(int hd) { return hd == 32 || hd == 64 || hd == 96 || hd == 128; }
+template <class F>
+int with_head_dim(int hd, F&& f) {
+  switch (hd) {
+    case 32: return f(std::integral_constant<int, 32>{});
+    case 64: return f(std::integral_constant<int, 64>{});
+    case 96: return f(std::integral_constant<int, 96>{});
+    default: return f(std::integral_constant<int, 128>{});
+  }
+}
+
 // ---- device helpers ---------------------------------------------------------------------------
+// x / d and x % d for x >= 0: a shift and a mask when d is a power of two
+template <int D>
+__host__ __device__ __forceinline__ int div_pos(int x) {
+  if constexpr ((D & (D - 1)) == 0) { int s = 0; while ((1 << s) < D) ++s; return x >> s; }
+  else return x / D;
+}
+template <int D>
+__host__ __device__ __forceinline__ int mod_pos(int x) {
+  if constexpr ((D & (D - 1)) == 0) return x & (D - 1);
+  else return x % D;
+}
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

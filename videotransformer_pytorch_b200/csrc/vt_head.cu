@@ -172,34 +172,37 @@ __global__ void scale_by_scalar_kernel(const float* __restrict__ in, const float
 }
 
 // ------------------------------------------------------------------------------------------------
-// Attention probabilities for any sequence length (head dim 64): probs[bp, h, i, :] = softmax_j(q_i . k_j * scale)
+// Attention probabilities for any sequence length (head dim 32, 64, 96 or 128): probs[bp, h, i, :] = softmax_j(q_i . k_j * scale)
 // CTA = PR_ROWS query rows of one (batch', head): raw scores of those rows live in shared memory (rows x N fp32),
-// keys stream through in tiles of 64; then a row softmax in place and coalesced fp32 stores.
+// keys stream through in tiles of 64 (pitch HD + 1 floats: lane = key reads are conflict free); then a row softmax in
+// place and coalesced fp32 stores.
 // ------------------------------------------------------------------------------------------------
 constexpr int PR_ROWS = 8;
 constexpr int PR_KT = 64;
 
+template <int HD>
 __global__ void __launch_bounds__(256)
 attn_probs_kernel(const __nv_bfloat16* __restrict__ qkv, float* __restrict__ probs, int N, int H, float scale) {
+  constexpr int KP = HD + 1, CPR = HD / 8;          // key pitch (floats), 16-byte chunks per row
   extern __shared__ float psm[];
   float* S = psm;                                   // [PR_ROWS][N]
-  float* Q = S + (size_t)PR_ROWS * N;               // [PR_ROWS][64]
-  float* Kt = Q + PR_ROWS * 64;                     // [64 keys][65]
+  float* Q = S + (size_t)PR_ROWS * N;               // [PR_ROWS][HD]
+  float* Kt = Q + PR_ROWS * HD;                     // [64 keys][HD + 1]
   const int bh = blockIdx.y, bp = bh / H, h = bh - bp * H;
   const int i0 = blockIdx.x * PR_ROWS;
-  const long long rs = 3LL * H * 64;
-  const __nv_bfloat16* base = qkv + (long long)bp * N * rs + h * 64;
-  for (int idx = threadIdx.x; idx < PR_ROWS * 64; idx += 256) {
-    const int r = idx >> 6, d = idx & 63;
+  const long long rs = 3LL * H * HD;
+  const __nv_bfloat16* base = qkv + (long long)bp * N * rs + h * HD;
+  for (int idx = threadIdx.x; idx < PR_ROWS * HD; idx += 256) {
+    const int r = div_pos<HD>(idx), d = mod_pos<HD>(idx);
     Q[idx] = (i0 + r < N) ? __bfloat162float(base[(long long)(i0 + r) * rs + d]) * scale : 0.f;
   }
   for (int j0 = 0; j0 < N; j0 += PR_KT) {
     __syncthreads();
-    for (int idx = threadIdx.x; idx < PR_KT * 8; idx += 256) {         // 64 keys x 8 vectors of 8 bf16
-      const int j = idx >> 3, c = idx & 7;
+    for (int idx = threadIdx.x; idx < PR_KT * CPR; idx += 256) {       // 64 keys x HD / 8 vectors of 8 bf16
+      const int j = div_pos<CPR>(idx), c = mod_pos<CPR>(idx);
       uint4 v = make_uint4(0u, 0u, 0u, 0u);
-      if (j0 + j < N) v = *reinterpret_cast<const uint4*>(base + (long long)(j0 + j) * rs + (long long)H * 64 + c * 8);
-      float* d = Kt + j * 65 + c * 8;
+      if (j0 + j < N) v = *reinterpret_cast<const uint4*>(base + (long long)(j0 + j) * rs + (long long)H * HD + c * 8);
+      float* d = Kt + j * KP + c * 8;
       const float2 a = unpack_bf16x2(v.x), b2 = unpack_bf16x2(v.y), c2 = unpack_bf16x2(v.z), e2 = unpack_bf16x2(v.w);
       d[0] = a.x; d[1] = a.y; d[2] = b2.x; d[3] = b2.y; d[4] = c2.x; d[5] = c2.y; d[6] = e2.x; d[7] = e2.y;
     }
@@ -208,10 +211,10 @@ attn_probs_kernel(const __nv_bfloat16* __restrict__ qkv, float* __restrict__ pro
     const int r = threadIdx.x >> 5, lane = threadIdx.x & 31;
     float s0 = 0.f, s1 = 0.f;
 #pragma unroll 16
-    for (int d = 0; d < 64; ++d) {
-      const float q = Q[r * 64 + d];
-      s0 = fmaf(q, Kt[lane * 65 + d], s0);
-      s1 = fmaf(q, Kt[(lane + 32) * 65 + d], s1);
+    for (int d = 0; d < HD; ++d) {
+      const float q = Q[r * HD + d];
+      s0 = fmaf(q, Kt[lane * KP + d], s0);
+      s1 = fmaf(q, Kt[(lane + 32) * KP + d], s1);
     }
     if (j0 + lane < N) S[(size_t)r * N + j0 + lane] = s0;
     if (j0 + lane + 32 < N) S[(size_t)r * N + j0 + lane + 32] = s1;
@@ -284,19 +287,25 @@ __global__ void im2col_u8_mix_kernel(const uint8_t* __restrict__ x, const float*
   }
 }
 
-// the probs output of vt_attn_fwd on the tensor-core path (vt_attention.cu); qkv is the packed projection at head dim 64
-int attn_probs_launch(const void* qkv, float* probs, int Bp, int N, int H, float scale, cudaStream_t st) {
-  const size_t smem = ((size_t)PR_ROWS * N + PR_ROWS * 64 + PR_KT * 65) * sizeof(float);
+template <int HD>
+static int attn_probs_launch_hd(const void* qkv, float* probs, int Bp, int N, int H, float scale, cudaStream_t st) {
+  const size_t smem = ((size_t)PR_ROWS * N + PR_ROWS * HD + PR_KT * (HD + 1)) * sizeof(float);
   VT_REQUIRE(smem <= 200 * 1024, "vt_attn_fwd: N=%d too long for the probs output (%zu bytes of shared memory)", N, smem);
   static size_t max_set = 48 * 1024;
   if (smem > max_set) {
-    cudaError_t e = cudaFuncSetAttribute(attn_probs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(attn_probs_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     VT_REQUIRE(e == cudaSuccess, "vt_attn_fwd: probs smem attribute: %s", cudaGetErrorString(e));
     max_set = 200 * 1024;
   }
   dim3 grid((N + PR_ROWS - 1) / PR_ROWS, Bp * H);
-  attn_probs_kernel<<<grid, 256, smem, st>>>(static_cast<const __nv_bfloat16*>(qkv), probs, N, H, scale);
+  attn_probs_kernel<HD><<<grid, 256, smem, st>>>(static_cast<const __nv_bfloat16*>(qkv), probs, N, H, scale);
   return check_launch("attn_probs_kernel");
+}
+
+// the probs output of vt_attn_fwd on the tensor-core path (vt_attention.cu); qkv is the packed projection at head dim hd
+// (checked by vt_attn_fwd)
+int attn_probs_launch(const void* qkv, float* probs, int Bp, int N, int H, int hd, float scale, cudaStream_t st) {
+  return with_head_dim(hd, [&](auto d) { return attn_probs_launch_hd<d.value>(qkv, probs, Bp, N, H, scale, st); });
 }
 
 static int grid_1d(long long n, int threads) {
