@@ -269,7 +269,7 @@ def _captured_body_worker(rank, world, port, q):
         for n, p in net.named_parameters():
             if 'temporal_fc' in n:
                 p.normal_(std=0.05)
-    red = GradientBuckets(net, bucket_bytes=4096, direct_wgrad=True)
+    red = GradientBuckets(net, bucket_bytes=4096)
     params = [p for p in net.parameters() if p.requires_grad]
     g = torch.Generator().manual_seed(70 + rank)
     x = torch.randn(2, 2, 3, 32, 32, generator=g)
@@ -296,7 +296,7 @@ def _captured_body_worker(rank, world, port, q):
     dist.destroy_process_group()
 
 
-def test_captured_step_body_writes_weight_gradients_into_buckets():
+def test_captured_step_body_always_writes_weight_gradients_into_buckets():
     import numpy as np
     ctx = mp.get_context('spawn')
     q = ctx.Queue()

@@ -358,13 +358,12 @@ def test_cls_rows_against_fp64(B, T, D, S):
     print(f'[rowwise-edges] cls_rows B={B} T={T} D={D}: {rep}')
 
 
-# ---- fused and separate column sums in the temporal block -----------------------------------------------------------
-def test_temporal_block_fused_and_separate_column_sums_agree(monkeypatch):
+# ---- the temporal block's fused column sums against the separate kernels --------------------------------------------
+def test_temporal_block_fused_column_sums_agree_with_separate_kernels(monkeypatch):
     """TemporalAttnFn.backward with DropPath on: d_fc_b and v (the column sums of the scaled rows) from the fused producer
-    (FUSED_COLSUM=True) lie within the two kernels' column-sum bounds of those of gather_cast + colsum, over the same bf16
-    rows"""
+    (gather_cast_colsum with unscaled_sums) lie within the two kernels' column-sum bounds of those of gather_cast + colsum
+    run on the same arguments, over the same bf16 rows"""
     from videotransformer_pytorch_b200 import _lib as L
-    from videotransformer_pytorch_b200 import ops
     from videotransformer_pytorch_b200.transformer import DividedTemporalAttentionWithPreNorm, DropPath
     torch.manual_seed(0)
     D, H, T, B, P = 768, 12, 8, 2, 196
@@ -375,31 +374,22 @@ def test_temporal_block_fused_and_separate_column_sums_agree(monkeypatch):
     y = blk(x)
     dy = torch.randn_like(y)
     Kc = type(L.K)
-    seen = {}
+    seen = []
+    orig = Kc.gather_cast_colsum
 
-    def spy(name):
-        orig = getattr(Kc, name)
-
-        def f(self, *a, **kw):
-            out = orig(self, *a, **kw)
-            seen.setdefault(name, []).append((a, kw, out))
-            return out
-        return f
-    for name in ('gather_cast_colsum', 'gather_cast', 'colsum'):
-        monkeypatch.setattr(Kc, name, spy(name))
-    got = {}
-    for fused in (True, False):
-        seen.clear()
-        monkeypatch.setattr(ops, 'FUSED_COLSUM', fused)
-        grads = torch.autograd.grad(y, [blk.temporal_fc.bias], dy, retain_graph=True)
-        if fused:
-            (a, kw, (gs, v, dfb)), = [s for s in seen['gather_cast_colsum'] if s[1].get('unscaled_sums')]
-            got[fused] = dict(gs=gs, v=v, d_fc_b=dfb, unscaled=None)
-        else:
-            gs = seen['gather_cast'][0][2]
-            got[fused] = dict(gs=gs, v=seen['colsum'][0][2], d_fc_b=seen['colsum'][1][2], unscaled=seen['gather_cast'][1][2])
-        assert torch.equal(grads[0], got[fused]['d_fc_b'])
-    f, s = got[True], got[False]
+    def spy(self, *a, **kw):
+        out = orig(self, *a, **kw)
+        seen.append((a, kw, out))
+        return out
+    monkeypatch.setattr(Kc, 'gather_cast_colsum', spy)
+    grads = torch.autograd.grad(y, [blk.temporal_fc.bias], dy)
+    (a, kw, (gs, v, dfb)), = [s for s in seen if s[1].get('unscaled_sums')]
+    f = dict(gs=gs, v=v, d_fc_b=dfb)
+    assert torch.equal(grads[0], f['d_fc_b'])
+    # the separate kernels on the fused call's arguments: the scaled rows and their sums, the unscaled rows and theirs
+    gs_s = L.K.gather_cast(a[0], in_row=kw['in_row'], row_scale=kw['row_scale'], rows=kw['rows'])
+    unscaled = L.K.gather_cast(a[0], in_row=kw['in_row'], rows=kw['rows'])
+    s = dict(gs=gs_s, v=L.K.colsum(gs_s), d_fc_b=L.K.colsum(unscaled), unscaled=unscaled)
     assert torch.equal(_bits(f['gs']), _bits(s['gs'])), 'the fused and separate producers give other bf16 rows'
     Mt = B * P * T
     nf, ns = R.gcc_plan(Mt, _sm())[2], R.colsum_n(Mt)

@@ -49,13 +49,8 @@ def test_timesformer_eval_tokens_attention(golden, emu, name):
     assert rel_err(attn, g.out['last_attn']) < 2e-5
 
 
-@pytest.mark.parametrize('merged_fc', [False, True], ids=['proj-then-fc', 'product-weight'])
-@pytest.mark.parametrize('fused_colsum', [False, True], ids=['colsum-pass', 'colsum-from-producers'])
 @pytest.mark.parametrize('name', ['timesformer_tiny', 'timesformer_hd64'])
-def test_timesformer_train_forward_backward(golden, emu, name, fused_colsum, merged_fc, monkeypatch):
-    from videotransformer_pytorch_b200 import ops
-    monkeypatch.setattr(ops, 'FUSED_COLSUM', fused_colsum)       # bias gradients from the dY producers or a separate pass
-    monkeypatch.setattr(ops, 'MERGE_TEMPORAL_FC', merged_fc)     # temporal_fc(DropPath(proj(.))) as one GEMM with W_fc W_proj
+def test_timesformer_train_forward_backward(golden, emu, name):
     g = golden(name)
     m = build_ts(g).train()
     x = g.x.clone().requires_grad_(True)

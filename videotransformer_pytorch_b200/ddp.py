@@ -28,15 +28,11 @@ import torch.distributed as dist
 
 class GradientBuckets:
     def __init__(self, module: torch.nn.Module, bucket_bytes: int = 32 << 20, process_group=None,
-                 broadcast_parameters: bool = True, direct_wgrad=None):
+                 broadcast_parameters: bool = True):
         if not dist.is_initialized():
             raise RuntimeError('GradientBuckets needs an initialised torch.distributed process group')
         self.group = process_group
         self.world = dist.get_world_size(process_group)
-        # weight-gradient GEMMs of a captured step write straight into the bucket slices (backward_into_buckets): measured
-        # at 2 GPUs 19.70 vs 20.00 ms per step, bucket contents identical to 8e-9 (bench.py ddp_check); VT_DDP_DIRECT=0/1 overrides
-        import os
-        self.direct_wgrad = (os.environ.get('VT_DDP_DIRECT', '1') == '1') if direct_wgrad is None else bool(direct_wgrad)
         params = [p for p in module.parameters() if p.requires_grad]
         if not params:
             raise RuntimeError('module has no trainable parameters')
@@ -146,15 +142,16 @@ class GradientBuckets:
         """Backward of `loss` with the gradients landing in the flat buckets and every bucket's all-reduce issued as soon as
         it is complete (the body of a captured data-parallel step, graph.GraphedTrainStep; also usable eagerly while every
         p.grad is its bucket view, as zero_grad() leaves it).  Uses torch.autograd.grad, so nothing is ACCUMULATED:
-        weight-gradient GEMMs may therefore write directly into their bucket slice (ops.GRAD_DEST), other gradients are
-        copied in by grad_ready().  Every parameter's slice is overwritten in full, so the buckets need no zeroing first."""
+        weight-gradient GEMMs therefore write directly into their bucket slice (ops.GRAD_DEST), other gradients are copied
+        in by grad_ready().  Writing in place instead of copying measured 19.70 vs 20.00 ms per step at 2 GPUs (before the
+        port to H100; not re-measured since), bucket contents equal to 8e-9 (bench.py ddp_check).  Every parameter's slice
+        is overwritten in full, so the buckets need no zeroing first."""
         from . import ops
         params = list(params)
         self._pending = [len(ps) for ps in self._bucket_params]
         self._arrived = [[] for _ in self._bucket_params]
         handles = [p.register_hook(lambda g, p=p: self.grad_ready(p, g)) for p in params]
-        if self.direct_wgrad:
-            ops.set_grad_destinations({p.data_ptr(): v for p, v in self._view.items()})
+        ops.set_grad_destinations({p.data_ptr(): v for p, v in self._view.items()})
         try:
             grads = torch.autograd.grad(loss, params)
         finally:

@@ -19,8 +19,7 @@ from __future__ import annotations
 import torch
 
 from . import _lib
-from . import ops as _ops
-from .ops import _act, _cast_with_colsum, _dgrad, _gemm, _lse, _stats, _wgrad
+from .ops import _act, _dgrad, _fc1_gelu, _gemm, _lse, _stats, _wgrad
 
 
 def K():
@@ -154,7 +153,7 @@ class PoolAttnFn(torch.autograd.Function):
         Nq = dy.shape[1]
         Mq = B * Nq
         dy2 = dy.view(Mq, d)
-        g, d_pb = _cast_with_colsum(k, dy2)
+        g, d_pb = k.gather_cast_colsum(dy2)
         d_pw = _wgrad(g, o.view(Mq, d), d, d, Mq)
         do = _dgrad(g, proj_wh, Mq, d, d, epi='bf16')
         sq, sk, sv = _slots(qkv, B, N1, d)
@@ -201,12 +200,8 @@ class MlpFn(torch.autograd.Function):
         x2 = x.view(M, d)
         save = ctx is not None
         xn, mean, rstd = k.ln_fwd(x2, n2w, n2b, eps, **_stats(save))
-        if save:
-            z = k.gemm(xn, w1h, M, Dh, d, bias=b1, epi='bf16')
-            h = k.gelu(z)
-        else:
-            xn = _act(k, xn, w1h)          # fp8: quantised once for FC1 and the width-changing proj
-            z, h = None, _gemm(k, xn, w1h, M, Dh, d, bias=b1, epi='gelu_h')
+        xn = _act(k, xn, w1h)              # fp8: quantised once for FC1 and the width-changing proj
+        z, h = _fc1_gelu(k, xn, w1h, b1, M, Dh, d, save)
         has_proj = pjh is not None
         r = _gemm(k, xn, pjh, M, do, d, bias=pjb, epi='f32') if has_proj else x2
         y = _gemm(k, h, w2h, M, do, Dh, bias=b2, epi='f32', aux=r)
@@ -225,13 +220,9 @@ class MlpFn(torch.autograd.Function):
         Dh, do = w1h.shape[0], w2h.shape[0]
         dy = dy.contiguous()
         dy2 = dy.view(M, do)
-        g, d_b2 = _cast_with_colsum(k, dy2)
+        g, d_b2 = k.gather_cast_colsum(dy2)
         d_w2 = _wgrad(g, h, do, Dh, M)
-        if _ops.FUSED_COLSUM:
-            dz, d_b1 = k.dgelu_colsum(_dgrad(g, w2h, M, Dh, do, epi='bf16'), z)
-        else:
-            dz = k.dgelu(_dgrad(g, w2h, M, Dh, do, epi='bf16'), z)
-            d_b1 = k.colsum(dz)
+        dz, d_b1 = k.dgelu_colsum(_dgrad(g, w2h, M, Dh, do, epi='bf16'), z)
         d_w1 = _wgrad(dz, xn, Dh, d, M)
         dx = torch.empty_like(x)
         d_pjw = d_pjb = None

@@ -43,21 +43,6 @@ def K():
 
 _MASK_ARENA = None
 
-# FFN activation: fused into the FC1 / FC2-dgrad GEMM epilogues (VT_EPI_GELU / VT_EPI_DGELU) or as stand-alone
-# bandwidth kernels after a plain bf16 epilogue.  Round 1 measured the split form faster (the erf math sat in the slow
-# transposing epilogue); the forward GELU epilogue now stores z and h as two TMA boxes — VT_FUSED_GELU=1 selects it
-# for FC1 (the dGELU epilogue of the FC2 data gradient stays split).
-import os as _os
-FUSED_GELU_FWD = _os.environ.get('VT_FUSED_GELU', '0') == '1'
-FUSED_DGELU_BWD = _os.environ.get('VT_TMA_DGELU', '0') == '1'      # dGELU epilogue of the FC2 data gradient on TMA
-FUSED_GELU_EPILOGUE = False
-# bias gradients from the kernels that produce dY (gather_cast / dgelu with column sums) instead of a separate pass;
-# VT_FUSED_COLSUM=0/1 overrides
-FUSED_COLSUM = _os.environ.get('VT_FUSED_COLSUM', '1') == '1'
-# temporal_fc(DropPath(proj(.))) as ONE token GEMM with the product weight W_fc W_proj (two 768^3 GEMMs per step instead of
-# two 12544 x 768 x 768 ones forward, and the same saving twice in backward); VT_MERGE_TEMPORAL_FC=0/1 overrides
-MERGE_TEMPORAL_FC = _os.environ.get('VT_MERGE_TEMPORAL_FC', '1') == '1'
-
 
 def run(fn, *args):
     """fn.apply(*args) when autograd records the call; otherwise fn.forward(None, *args), the forward-only form of the
@@ -222,14 +207,6 @@ def _dgrad(dout, w, m_tok, k_in, n_out, **kw):
     return K().gemm(dout, w, m_tok, k_in, n_out, b_mn=True, **kw)
 
 
-def _cast_with_colsum(k, src2d, in_row=None, row_scale=None, rows=None):
-    """dY in bf16 (gathered / scaled rows of the fp32 gradient stream) and its column sums = the bias gradient."""
-    if FUSED_COLSUM:
-        return k.gather_cast_colsum(src2d, in_row=in_row, row_scale=row_scale, rows=rows)
-    g = k.gather_cast(src2d, in_row=in_row, row_scale=row_scale, rows=rows)
-    return g, k.colsum(g)
-
-
 def _stats(save):
     """LayerNorm / pooling keyword for a forward that saves (default form) or one that does not (statistics not written)."""
     return {} if save else {'stats': False}
@@ -240,13 +217,11 @@ def _lse(save):
 
 
 def _fc1_gelu(k, xn, w1h, b1, M, Dh, D, save):
-    """(z, h) of h = gelu(z), z = xn W1^T + b1, both bf16.  Saving forward: z is kept for backward — fused 'gelu' epilogue
-    or 'bf16' GEMM + GELU kernel per FUSED_GELU_FWD.  Forward-only: the 'gelu_h' epilogue writes h alone (z is None), bit
-    for bit the split form's h."""
+    """(z, h) of h = gelu(z), z = xn W1^T + b1, both bf16.  Saving forward: a 'bf16' GEMM and the GELU kernel, z kept for
+    the backward (the 'gelu' epilogue measured no faster: its erf arithmetic runs before the tile's stores, DESIGN.md §7).
+    Forward-only: the 'gelu_h' epilogue writes h alone (z is None), bit for bit the saving form's h."""
     if not save:
         return None, _gemm(k, xn, w1h, M, Dh, D, bias=b1, epi='gelu_h')
-    if FUSED_GELU_EPILOGUE or FUSED_GELU_FWD:
-        return k.gemm(xn, w1h, M, Dh, D, bias=b1, epi='gelu')
     z = k.gemm(xn, w1h, M, Dh, D, bias=b1, epi='bf16')
     return z, k.gelu(z)
 
@@ -278,25 +253,16 @@ class TemporalAttnFn(torch.autograd.Function):
         cx, lse, _ = k.attn_fwd(qkv, B * P, T, H, hd, hd ** -0.5, **_lse(save))
         y = torch.empty_like(x)
         y2 = y.view(B * S, D)
-        merged = MERGE_TEMPORAL_FC
-        if merged:
-            # y = s (W_f (W_p c + b_p)) + b_f + x = s (W_c c + b_c) + b_f + x,  W_c = W_f W_p,  b_c = W_f b_p
-            # (transformer.py:261-267: two nn.Linear with only DropPath's per-sample scale between them)
-            # fp8: fc_wh is already the e4m3 product weight (ShadowWeights.get_e4m3 of W_f W_p)
-            wc = fc_wh if isinstance(fc_wh, _lib.E4M3) else k.gemm(fc_wh, proj_wh, D, D, D, b_mn=True, epi='bf16')
-            bc = torch.mv(fc_w.detach().float(), proj_b.detach().float())
-            _gemm(k, cx, wc, Mt, D, D, bias=bc, bias2=fc_b, epi='f32', aux=x2, aux_row=maps['temporal'], out=y2,
-                  out_row=maps['temporal'], row_scale=dp, row_map=affine_row_maps(B, T, P, D)['temporal'], tag='proj')
-            a = wc
-        else:
-            a = _gemm(k, cx, proj_wh, Mt, D, D, bias=proj_b, epi='bf16', row_scale=dp, tag='proj')
-            _gemm(k, a, fc_wh, Mt, D, D, bias=fc_b, epi='f32', aux=x2, aux_row=maps['temporal'], out=y2,
-                  out_row=maps['temporal'], row_map=affine_row_maps(B, T, P, D)['temporal'])
+        # one token GEMM: y = s (W_f (W_p c + b_p)) + b_f + x = s (W_c c + b_c) + b_f + x,  W_c = W_f W_p,  b_c = W_f b_p
+        # (transformer.py:261-267: two nn.Linear with only DropPath's per-sample scale between them; DESIGN.md §4)
+        # fp8: fc_wh is already the e4m3 product weight (ShadowWeights.get_e4m3 of W_f W_p)
+        wc = fc_wh if isinstance(fc_wh, _lib.E4M3) else k.gemm(fc_wh, proj_wh, D, D, D, b_mn=True, epi='bf16')
+        bc = torch.mv(fc_w.detach().float(), proj_b.detach().float())
+        _gemm(k, cx, wc, Mt, D, D, bias=bc, bias2=fc_b, epi='f32', aux=x2, aux_row=maps['temporal'], out=y2,
+              out_row=maps['temporal'], row_scale=dp, row_map=affine_row_maps(B, T, P, D)['temporal'], tag='proj')
         k.cls_rows(y[:, 0], x[:, 0])
         if save:
-            ctx.merged = merged
-            ctx.save_for_backward(x, ln_w, mean, rstd, xn, qkv, cx, lse, a, qkv_wh, proj_wh, fc_wh, dp,
-                                  fc_w if merged else None, proj_b if merged else None)
+            ctx.save_for_backward(x, ln_w, mean, rstd, xn, qkv, cx, lse, wc, qkv_wh, proj_wh, fc_wh, dp, fc_w, proj_b)
             ctx.geom = (B, S, D, T, H, P)
             ctx.wptrs = (qkv_w.data_ptr(), proj_w.data_ptr(), fc_w.data_ptr())
         return y
@@ -304,7 +270,7 @@ class TemporalAttnFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         k = K()
-        x, ln_w, mean, rstd, xn, qkv, cx, lse, a, qkv_wh, proj_wh, fc_wh, dp, fc_w, proj_b = ctx.saved_tensors
+        x, ln_w, mean, rstd, xn, qkv, cx, lse, wc, qkv_wh, proj_wh, fc_wh, dp, fc_w, proj_b = ctx.saved_tensors
         B, S, D, T, H, P = ctx.geom
         maps = token_maps(B, T, P, str(x.device))
         hd = D // H
@@ -312,33 +278,20 @@ class TemporalAttnFn(torch.autograd.Function):
         dy = dy.contiguous()
         dy2 = dy.view(B * S, D)
         x2 = x.reshape(B * S, D)
-        if ctx.merged:
-            # gs = s * dY rows;  v = colsum(gs);  G = gs^T c
-            # dc = gs W_c;  dW_f = G W_p^T + v b_p^T;  db_f = colsum(dY);  dW_p = W_f^T G;  db_p = W_f^T v
-            wc = a
-            if dp is None:
-                gs, v = _cast_with_colsum(k, dy2, in_row=maps['temporal'], rows=Mt)
-                d_fc_b = v
-            elif FUSED_COLSUM:
-                gs, v, d_fc_b = k.gather_cast_colsum(dy2, in_row=maps['temporal'], row_scale=dp, rows=Mt, unscaled_sums=True)
-            else:
-                gs = k.gather_cast(dy2, in_row=maps['temporal'], row_scale=dp, rows=Mt)
-                v = k.colsum(gs)
-                d_fc_b = k.colsum(k.gather_cast(dy2, in_row=maps['temporal'], rows=Mt))
-            dcx = _dgrad(gs, wc, Mt, D, D, epi='bf16', tag='proj')
-            G = k.gemm(gs, cx, D, D, Mt, a_mn=True, b_mn=True, epi='f32', split_ok=True, tag='proj')
-            Gh = k.cast_bf16(G)
-            d_fc_w = k.gemm(Gh, proj_wh, D, D, D, epi='f32', out=_grad_dest(ctx.wptrs[2], D, D))
-            d_fc_w.addr_(v, proj_b.detach().float())
-            d_proj_w = k.gemm(fc_wh, Gh, D, D, D, a_mn=True, b_mn=True, epi='f32', out=_grad_dest(ctx.wptrs[1], D, D))
-            d_proj_b = torch.mv(fc_w.detach().float().t(), v)
+        # gs = s * dY rows;  v = colsum(gs);  G = gs^T c
+        # dc = gs W_c;  dW_f = G W_p^T + v b_p^T;  db_f = colsum(dY);  dW_p = W_f^T G;  db_p = W_f^T v
+        if dp is None:
+            gs, v = k.gather_cast_colsum(dy2, in_row=maps['temporal'], rows=Mt)
+            d_fc_b = v
         else:
-            g, d_fc_b = _cast_with_colsum(k, dy2, in_row=maps['temporal'], rows=Mt)
-            d_fc_w = _wgrad(g, a, D, D, Mt, wptr=ctx.wptrs[2])
-            da = _dgrad(g, fc_wh, Mt, D, D, epi='bf16', row_scale=dp)
-            d_proj_w = _wgrad(da, cx, D, D, Mt, tag='proj', wptr=ctx.wptrs[1])
-            d_proj_b = k.colsum(da)
-            dcx = _dgrad(da, proj_wh, Mt, D, D, epi='bf16', tag='proj')
+            gs, v, d_fc_b = k.gather_cast_colsum(dy2, in_row=maps['temporal'], row_scale=dp, rows=Mt, unscaled_sums=True)
+        dcx = _dgrad(gs, wc, Mt, D, D, epi='bf16', tag='proj')
+        G = k.gemm(gs, cx, D, D, Mt, a_mn=True, b_mn=True, epi='f32', split_ok=True, tag='proj')
+        Gh = k.cast_bf16(G)
+        d_fc_w = k.gemm(Gh, proj_wh, D, D, D, epi='f32', out=_grad_dest(ctx.wptrs[2], D, D))
+        d_fc_w.addr_(v, proj_b.detach().float())
+        d_proj_w = k.gemm(fc_wh, Gh, D, D, D, a_mn=True, b_mn=True, epi='f32', out=_grad_dest(ctx.wptrs[1], D, D))
+        d_proj_b = torch.mv(fc_w.detach().float().t(), v)
         dqkv = k.attn_bwd(qkv, cx, dcx, lse, B * P, T, H, hd, hd ** -0.5)
         d_qkv_w = _wgrad(dqkv, xn, 3 * D, D, Mt, tag='qkv', wptr=ctx.wptrs[0])
         d_qkv_b = k.colsum(dqkv)
@@ -390,7 +343,7 @@ class SpatialAttnFn(torch.autograd.Function):
         dy = dy.contiguous()
         dy2 = dy.view(R, D)
         x2 = x.reshape(R, D)
-        g, d_proj_b = _cast_with_colsum(k, dy2, in_row=maps['sp_in'], row_scale=_mul_opt(dp, maps['sp_cls_scale']), rows=Ms)
+        g, d_proj_b = k.gather_cast_colsum(dy2, in_row=maps['sp_in'], row_scale=_mul_opt(dp, maps['sp_cls_scale']), rows=Ms)
         d_proj_w = _wgrad(g, cx, D, D, Ms, tag='proj', wptr=ctx.wptrs[1])
         dcx = _dgrad(g, proj_wh, Ms, D, D, epi='bf16', tag='proj')
         dqkv = k.attn_bwd(qkv, cx, dcx, lse, B * T, P + 1, H, hd, hd ** -0.5)
@@ -437,7 +390,7 @@ class JointAttnFn(torch.autograd.Function):
         dy = dy.contiguous()
         dy2 = dy.view(M, D)
         x2 = x.reshape(M, D)
-        g, d_proj_b = _cast_with_colsum(k, dy2, row_scale=dp)
+        g, d_proj_b = k.gather_cast_colsum(dy2, row_scale=dp)
         d_proj_w = _wgrad(g, cx, D, D, M, tag='proj', wptr=ctx.wptrs[1])
         dcx = _dgrad(g, proj_wh, M, D, D, epi='bf16', tag='proj')
         dqkv = k.attn_bwd(qkv, cx, dcx, lse, Bp, N, H, hd, hd ** -0.5)
@@ -480,19 +433,10 @@ class FFNFn(torch.autograd.Function):
         dy = dy.contiguous()
         dy2 = dy.view(M, D)
         x2 = x.reshape(M, D)
-        g, d_b2 = _cast_with_colsum(k, dy2, row_scale=dp)
+        g, d_b2 = k.gather_cast_colsum(dy2, row_scale=dp)
         d_w2 = _wgrad(g, h, D, Dh, M, wptr=ctx.wptrs[1])
-        d_b1 = None
-        if FUSED_GELU_EPILOGUE or FUSED_DGELU_BWD:
-            dz = _dgrad(g, w2h, M, Dh, D, epi='dgelu', aux=z)
-        else:
-            if FUSED_COLSUM:
-                dz, d_b1 = k.dgelu_colsum(_dgrad(g, w2h, M, Dh, D, epi='bf16'), z)
-            else:
-                dz = k.dgelu(_dgrad(g, w2h, M, Dh, D, epi='bf16'), z)
+        dz, d_b1 = k.dgelu_colsum(_dgrad(g, w2h, M, Dh, D, epi='bf16'), z)
         d_w1 = _wgrad(dz, xn, Dh, D, M, wptr=ctx.wptrs[0])
-        if d_b1 is None:
-            d_b1 = k.colsum(dz)
         dxn = _dgrad(dz, w1h, M, D, Dh, epi='bf16')
         dx = torch.empty_like(x)
         _, _, d_ln_w, d_ln_b = k.ln_bwd(dxn, x2, mean, rstd, ln_w, dres=dy2, dx=dx.view(M, D))
@@ -574,7 +518,7 @@ class PatchTokensFn(torch.autograd.Function):
             maps = token_maps(B, Tp, P, str(dout.device))
         else:
             maps = frame_maps(B * Tp, P, str(dout.device))
-        g, db = _cast_with_colsum(k, d2, in_row=maps['emb_out'], rows=M)
+        g, db = k.gather_cast_colsum(d2, in_row=maps['emb_out'], rows=M)
         dw = _wgrad(g, cols, D, Kc, M).view(wshape)
         dcls = dout[:, 0].sum(dim=0)
         if mode == 'timesformer':

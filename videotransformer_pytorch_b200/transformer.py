@@ -295,12 +295,10 @@ class DividedTemporalAttentionWithPreNorm(_DividedBase):
     Hot-path configuration: use_cls_token=False (cls bypasses the block, `temporal_fc` after DropPath)."""
 
     def _e4m3_shadows(self, D):
-        """(qkv, proj, temporal_fc) e4m3 shadows; with the merged temporal_fc . proj GEMM (ops.MERGE_TEMPORAL_FC) the third
-        is the product W_f W_p, formed from the bf16 shadows in fp32 and quantised per output channel, and proj is unused."""
+        """(qkv, None, product) e4m3 shadows for ops.TemporalAttnFn, which runs temporal_fc . proj as one GEMM: the product
+        W_f W_p is formed from the bf16 shadows in fp32 and quantised per output channel; proj has no shadow of its own."""
         a, sh = self.attn, self.attn._shadow
         qh = sh.get_e4m3('qkv:e4m3', [a.qkv.weight])
-        if not ops.MERGE_TEMPORAL_FC:
-            return qh, sh.get_e4m3('proj:e4m3', [a.proj.weight]), sh.get_e4m3('temporal_fc:e4m3', [self.temporal_fc.weight])
         product = lambda: _lib.K.gemm(sh.get('temporal_fc', self.temporal_fc.weight), sh.get('proj', a.proj.weight), D, D, D,
                                       b_mn=True, epi='f32')
         return qh, None, sh.get_e4m3('wc:e4m3', [self.temporal_fc.weight, a.proj.weight], derive=product)
