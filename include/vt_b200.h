@@ -414,8 +414,11 @@ int vt_mse_bwd(const vt_mse_bwd_params* p, void* stream);
  * clip_gradients + optimizer.py:33-38 SGD(momentum 0.9, nesterov) / AdamW(0.9, 0.999)).
  * Multi-tensor form: tensor i has parameter pptr[i], gradient gptr[i], state s1ptr[i] (momentum buffer / exp_avg) and
  * s2ptr[i] (exp_avg_sq), all fp32 device addresses stored as int64 in device arrays; `chunks` is a device table of
- * {int32 tensor, int32 len, int64 offset} (16 bytes each) covering every tensor; lr / wd are per-tensor fp32 arrays.
+ * {int32 tensor, int32 len, int64 offset} (16 bytes each) covering every tensor, each tensor's chunks consecutive and in
+ * offset order; lr / wd are per-tensor fp32 arrays.
  *   vt_opt_norm2 : norm2[i] = sum(grad_i^2)                          (the trainer's total norm = sqrt(sum_i norm2[i]))
+ *                  one fp32 partial per chunk into `partials` (n_chunks floats), then each tensor's partials added in
+ *                  chunk order: bitwise reproducible.  The update kernels do not read `partials`.
  *   vt_opt_sgd   : g = grad * min(1, clip / (sqrt(norm2) + 1e-6)) [clip > 0];  d = g + wd*p;  buf = first ? d : mom*buf + d;
  *                  p -= lr * (nesterov ? d + mom*buf : buf)           (torch.optim.SGD, dampening 0)
  *   vt_opt_adamw : p *= 1 - lr*wd;  m = b1 m + (1-b1) g;  v = b2 v + (1-b2) g^2;
@@ -428,6 +431,7 @@ typedef struct {
   float* norm2; const float* lr; const float* wd;
   float clip, momentum, beta1, beta2, eps, bc1, bc2;
   int32_t nesterov, first_step;
+  float* partials;          /* vt_opt_norm2 workspace: n_chunks floats */
 } vt_opt_params;
 int vt_opt_norm2(const vt_opt_params* p, void* stream);
 int vt_opt_sgd(const vt_opt_params* p, void* stream);
@@ -439,7 +443,7 @@ int vt_opt_adamw(const vt_opt_params* p, void* stream);
 
 /* Skinny fp32 linear layer  y[M,N] = x[M,K] W[N,K]^T + b  (ClassificationHead.forward, transformer.py:78-80: 8 x 768 -> 400)
  * and its adjoints  dW = dy^T x, db = colsum(dy), dx = dy W  (dw / dx may be NULL to skip).  Warp-per-output GEMV on
- * the fp32 parameters themselves (no bf16 shadow); M <= 4096, K % 4 == 0. */
+ * the fp32 parameters themselves (no bf16 shadow); M <= 4096, K % 4 == 0, x / w / dw / dx 16-byte aligned (float4 rows). */
 typedef struct { const float* x; const float* w; const float* b; float* y; int32_t M, N, K; } vt_linear_small_params;
 int vt_linear_small_fwd(const vt_linear_small_params* p, void* stream);
 typedef struct { const float* dy; const float* x; const float* w; float* dw; float* db; float* dx; int32_t M, N, K; } vt_linear_small_bwd_params;
@@ -447,7 +451,10 @@ int vt_linear_small_bwd(const vt_linear_small_bwd_params* p, void* stream);
 
 /* Softmax cross-entropy, mean over rows: nn.CrossEntropyLoss (model_trainer.py:91, :208) with int64 `labels`, or timm's
  * SoftTargetCrossEntropy (:89) with fp32 `soft_targets` [M,N] (exactly one of the two).  One launch writes loss[0],
- * optional per-row losses and dlogits = d loss / d logits. */
+ * optional per-row losses and dlogits = d loss / d logits.  Row loss = sum_c t_c * log(sum_c e^(z_c - max z)) -
+ * sum_c t_c (z_c - max z) over the classes with t_c != 0, so a -inf logit off the label gives torch's finite result.
+ * Labels must lie in [0, N): any other label (torch's ignore_index -100 included) acts as a row of zero targets, whose
+ * loss and dlogits are 0, and it still counts in the mean's 1/M. */
 typedef struct {
   const float* logits; const int64_t* labels; const float* soft_targets;
   float* loss; float* row_loss; float* dlogits; int32_t M, N;

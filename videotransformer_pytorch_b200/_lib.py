@@ -225,7 +225,7 @@ class OptParams(C.Structure):
                 ('pptr', c_vp), ('gptr', c_vp), ('s1ptr', c_vp), ('s2ptr', c_vp),
                 ('norm2', c_vp), ('lr', c_vp), ('wd', c_vp),
                 ('clip', c_f32), ('momentum', c_f32), ('beta1', c_f32), ('beta2', c_f32), ('eps', c_f32), ('bc1', c_f32),
-                ('bc2', c_f32), ('nesterov', c_i32), ('first_step', c_i32)]
+                ('bc2', c_f32), ('nesterov', c_i32), ('first_step', c_i32), ('partials', c_vp)]
 
 
 class LinearSmallParams(C.Structure):
@@ -1248,6 +1248,7 @@ class CudaKernels:
         p.pptr, p.gptr = tbl['pptr'].data_ptr(), tbl['gptr'].data_ptr()
         p.s1ptr, p.s2ptr = tbl['s1ptr'].data_ptr(), _ptr(tbl.get('s2ptr'))
         p.norm2, p.lr, p.wd = tbl['norm2'].data_ptr(), tbl['lr'].data_ptr(), tbl['wd'].data_ptr()
+        p.partials = _ptr(tbl.get('partials'))
         p.clip = float(clip or 0.0)
         for k, v in hp.items():
             setattr(p, k, v)

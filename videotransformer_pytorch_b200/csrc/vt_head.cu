@@ -109,7 +109,10 @@ linear_small_dgrad_kernel(const float* __restrict__ dy, const float* __restrict_
 
 // ------------------------------------------------------------------------------------------------
 // Softmax cross-entropy, mean over the M rows (nn.CrossEntropyLoss; timm SoftTargetCrossEntropy with `soft`):
-//   loss = 1/M sum_m ( lse(z_m) * sum_c t_mc - sum_c t_mc z_mc ),   dz_mc = (softmax(z_m)_c * sum_c' t_mc' - t_mc) / M
+//   loss = 1/M sum_m ( log(sum_c e^(z_mc - mx_m)) * sum_c t_mc - sum_c t_mc (z_mc - mx_m) ),   mx_m = max_c z_mc
+//   dz_mc = (softmax(z_m)_c * sum_c' t_mc' - t_mc) / M
+// The row loss is formed from z - mx, so it does not cancel at the magnitude of the logits, and classes with t = 0 are
+// skipped, so a -inf logit that is not the label gives torch's finite loss rather than 0 * -inf = NaN.
 // One CTA, rows in sequence (M is the per-GPU batch); deterministic.
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
@@ -138,23 +141,22 @@ softmax_ce_kernel(const float* __restrict__ z, const int64_t* __restrict__ label
     float se = 0.f, tz = 0.f, ts = 0.f;
     const long long lab = labels ? (long long)labels[m] : -1;
     for (int c = threadIdx.x; c < N; c += 256) {
-      const float v = zr[c];
-      se += expf(v - mx);
+      const float d = zr[c] - mx;
+      se += expf(d);
       const float t = soft ? soft[(long long)m * N + c] : (c == lab ? 1.f : 0.f);
-      tz = fmaf(t, v, tz);
+      if (t != 0.f) tz = fmaf(t, d, tz);
       ts += t;
     }
     se = block_reduce(se, false);
     tz = block_reduce(tz, false);
     ts = block_reduce(ts, false);
-    const float lse = mx + logf(se);
     const float inv_se = 1.0f / se;
     for (int c = threadIdx.x; c < N; c += 256) {
       const float t = soft ? soft[(long long)m * N + c] : (c == lab ? 1.f : 0.f);
       dz[(long long)m * N + c] = (expf(zr[c] - mx) * inv_se * ts - t) * inv_m;
     }
     if (threadIdx.x == 0) {
-      const float l = lse * ts - tz;
+      const float l = logf(se) * ts - tz;
       if (row_loss) row_loss[m] = l;
       total += l;
     }
@@ -324,6 +326,8 @@ extern "C" int vt_linear_small_fwd(const vt_linear_small_params* p, void* stream
   VT_REQUIRE(p && p->x && p->w && p->y, "vt_linear_small_fwd: null pointer");
   VT_REQUIRE(p->M > 0 && p->N > 0 && p->K > 0 && p->K % 4 == 0, "vt_linear_small_fwd: bad shape M=%d N=%d K=%d (K %% 4 == 0)", p->M, p->N, p->K);
   VT_REQUIRE(p->M <= 4096, "vt_linear_small_fwd: M=%d is not skinny (use vt_gemm)", p->M);
+  VT_REQUIRE(((reinterpret_cast<uintptr_t>(p->x) | reinterpret_cast<uintptr_t>(p->w)) & 15) == 0,
+             "vt_linear_small_fwd: x and w must be 16-byte aligned");
   dim3 grid((p->N + 7) / 8, (p->M + LS_ROWS - 1) / LS_ROWS);
   linear_small_fwd_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(p->x, p->w, p->b, p->y, p->M, p->N, p->K);
   return check_launch("linear_small_fwd_kernel");
@@ -333,6 +337,9 @@ extern "C" int vt_linear_small_bwd(const vt_linear_small_bwd_params* p, void* st
   VT_REQUIRE(p && p->dy && p->x && p->w, "vt_linear_small_bwd: null pointer");
   VT_REQUIRE(p->M > 0 && p->N > 0 && p->K > 0 && p->K % 4 == 0, "vt_linear_small_bwd: bad shape");
   VT_REQUIRE(p->M <= 4096, "vt_linear_small_bwd: M=%d is not skinny", p->M);
+  VT_REQUIRE(((reinterpret_cast<uintptr_t>(p->x) | reinterpret_cast<uintptr_t>(p->w) | reinterpret_cast<uintptr_t>(p->dw) |
+               reinterpret_cast<uintptr_t>(p->dx)) & 15) == 0,
+             "vt_linear_small_bwd: x, w, dw and dx must be 16-byte aligned");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (p->dw) {
     linear_small_wgrad_kernel<<<(p->N + 7) / 8, 256, 0, st>>>(p->dy, p->x, p->dw, p->db, p->M, p->N, p->K);

@@ -3,7 +3,8 @@
 // The reference clips every parameter's gradient to `clip_grad` by its own L2 norm (model_trainer.py:155-170: one
 // torch.norm launch + one host comparison per parameter, 247 of them for TimeSformer-B) and then runs torch.optim
 // SGD(momentum 0.9, nesterov) or AdamW (optimizer.py:33-38).  Here that is two launches for the whole model:
-//   1. multi_norm2: squared L2 norm of every gradient tensor (chunked, fp32 atomics per tensor)
+//   1. multi_norm2 + norm2_finish: squared L2 norm of every gradient tensor (one partial per chunk, then each tensor's
+//      partials summed in chunk order: the same inputs give the same bits on every call)
 //   2. fused update: per element g = grad * min(1, clip / (norm + 1e-6)), then the SGD-nesterov or AdamW step.
 // Tensors are addressed through device arrays of pointers (multi-tensor apply), so parameters, gradients (per-tensor
 // .grad or views of the DDP flat buckets) and optimizer state stay wherever PyTorch put them.
@@ -23,7 +24,7 @@ struct OptChunk {
 static_assert(sizeof(OptChunk) == 16, "chunk table layout");
 
 __global__ void __launch_bounds__(OPT_THREADS)
-multi_norm2_kernel(const OptChunk* __restrict__ chunks, const long long* __restrict__ gptr, float* __restrict__ norm2) {
+multi_norm2_kernel(const OptChunk* __restrict__ chunks, const long long* __restrict__ gptr, float* __restrict__ partials) {
   const OptChunk c = chunks[blockIdx.x];
   const float* g = reinterpret_cast<const float*>(gptr[c.tensor]) + c.offset;
   float s = 0.f;
@@ -45,8 +46,21 @@ multi_norm2_kernel(const OptChunk* __restrict__ chunks, const long long* __restr
   if (threadIdx.x == 0) {
     float a = 0.f;
     for (int i = 0; i < OPT_THREADS / 32; ++i) a += sh[i];
-    atomicAdd(norm2 + c.tensor, a);
+    partials[blockIdx.x] = a;
   }
+}
+
+// norm2[t] = the partials of tensor t's chunks added in table order; one thread per chunk, the thread of a tensor's first
+// chunk walks its run (a tensor's chunks are consecutive in the table)
+__global__ void norm2_finish_kernel(const OptChunk* __restrict__ chunks, const float* __restrict__ partials,
+                                    float* __restrict__ norm2, int n_chunks) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= n_chunks) return;
+  const int t = chunks[c].tensor;
+  if (c > 0 && chunks[c - 1].tensor == t) return;
+  float s = partials[c];
+  for (int j = c + 1; j < n_chunks && chunks[j].tensor == t; ++j) s += partials[j];
+  norm2[t] = s;
 }
 
 struct OptArgs {
@@ -110,12 +124,16 @@ using namespace vt;
 
 extern "C" int vt_opt_norm2(const vt_opt_params* p, void* stream) {
   VT_REQUIRE(p && p->chunks && p->gptr && p->norm2 && p->n_chunks > 0 && p->n_tensors > 0, "vt_opt_norm2: bad params");
+  VT_REQUIRE(p->partials, "vt_opt_norm2: partials workspace (n_chunks floats) missing");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  cudaError_t e = cudaMemsetAsync(p->norm2, 0, sizeof(float) * p->n_tensors, st);
+  cudaError_t e = cudaMemsetAsync(p->norm2, 0, sizeof(float) * p->n_tensors, st);   // tensors without chunks
   VT_REQUIRE(e == cudaSuccess, "vt_opt_norm2: memset: %s", cudaGetErrorString(e));
-  multi_norm2_kernel<<<p->n_chunks, OPT_THREADS, 0, st>>>(static_cast<const OptChunk*>(p->chunks), reinterpret_cast<const long long*>(p->gptr),
-                                                        p->norm2);
-  return check_launch("multi_norm2_kernel");
+  const OptChunk* chunks = static_cast<const OptChunk*>(p->chunks);
+  multi_norm2_kernel<<<p->n_chunks, OPT_THREADS, 0, st>>>(chunks, reinterpret_cast<const long long*>(p->gptr), p->partials);
+  int rc = check_launch("multi_norm2_kernel");
+  if (rc) return rc;
+  norm2_finish_kernel<<<(p->n_chunks + 255) / 256, 256, 0, st>>>(chunks, p->partials, p->norm2, p->n_chunks);
+  return check_launch("norm2_finish_kernel");
 }
 
 static int opt_args(const vt_opt_params* p, OptArgs* a, const char* who, bool need_s2) {

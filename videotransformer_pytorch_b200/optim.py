@@ -51,6 +51,7 @@ class TensorTable:
             'gptr': torch.zeros(n, dtype=torch.int64, device=dev),
             's1ptr': torch.tensor([s.data_ptr() for s in self.state[0]], dtype=torch.int64, device=dev),
             'norm2': torch.zeros(n, dtype=torch.float32, device=dev),
+            'partials': torch.zeros(len(rows), dtype=torch.float32, device=dev),    # vt_opt_norm2: one sum per chunk
             'lr': torch.zeros(n, dtype=torch.float32, device=dev),
             'wd': torch.zeros(n, dtype=torch.float32, device=dev),
         }
