@@ -53,8 +53,6 @@ int vt_launch_count(void);
  *   VT_EPI_BF16  : out_bf16[orow(m), n]  = s(m) * (acc + bias[n])
  *   VT_EPI_F32   : out_f32 [orow(m), n]  = s(m) * (acc + bias[n]) + (aux ? aux_f32[arow(m), n] : 0)
  *                  (residual add / pos+time-embed add / fp32 gradients)
- *   VT_EPI_GELU  : out_bf16[m,n] = z = acc + bias[n];  out2_bf16[m,n] = gelu_erf(z)     (transformer.py:501-503)
- *   VT_EPI_DGELU : out_bf16[m,n] = acc * gelu_erf'(aux_bf16[m,n])                        (autograd of nn.GELU)
  *   VT_EPI_GELU_H: out_bf16[orow(m), n] = gelu_erf(bf16(s(m) * (acc + bias[n])))  — forward-only FC1: h alone, z is not
  *                  written.  Bit for bit VT_EPI_BF16 followed by vt_gelu_fwd_bf16 (same per-element code, same tiles).
  * orow(m) = out_row ? out_row[m] : m  (negative => row skipped);  arow likewise (negative => no addend);  s(m) = row_scale ? row_scale[m] : 1
@@ -63,8 +61,10 @@ int vt_launch_count(void);
  * Split-K: when `workspace` is given and the tile count under-fills the GPU (weight gradients:
  * K = tokens), K is split; partial tiles go to the fp32 workspace and are summed by a second kernel.
  * Only with VT_EPI_F32, no row maps.
+ *
+ * Epilogue values 2 and 3 are unassigned and rejected; the others keep their numbers for ABI compatibility.
  * ------------------------------------------------------------------------------------------- */
-enum { VT_EPI_BF16 = 0, VT_EPI_F32 = 1, VT_EPI_GELU = 2, VT_EPI_DGELU = 3, VT_EPI_GELU_H = 4 };
+enum { VT_EPI_BF16 = 0, VT_EPI_F32 = 1, VT_EPI_GELU_H = 4 };
 
 typedef struct {
   const void* a;      /* bf16 */
@@ -75,9 +75,9 @@ typedef struct {
   int32_t epilogue;
   const float* bias;       /* [N] or NULL */
   void* out;               /* bf16 or fp32 per epilogue */
-  void* out2;              /* VT_EPI_GELU only */
-  const void* aux;         /* fp32 (VT_EPI_F32) or bf16 (VT_EPI_DGELU) or NULL */
-  int64_t ldo, ldo2, ldaux;
+  void* out2;              /* unused; kept for ABI compatibility */
+  const void* aux;         /* fp32, VT_EPI_F32 only (rejected with the other epilogues), or NULL */
+  int64_t ldo, ldo2, ldaux;  /* ldo2: unused; kept for ABI compatibility */
   const int32_t* out_row;  /* [M] or NULL */
   const int32_t* aux_row;  /* [M] or NULL */
   const float* row_scale;  /* [M] or NULL */
@@ -114,7 +114,7 @@ int vt_gemm(const vt_gemm_params* p, void* stream);
  * __nv_fp8_e4m3), lda / ldb in elements; both operands K-major (a_mn_major = b_mn_major = 0).  Each 128-wide k-block
  * is accumulated by 4 x wgmma k32 into a fresh fp32 register tile and then added on the CUDA cores to the tile's fp32
  * accumulator.  K % 16 == 0, lda % 16 == 0, ldb % 16 == 0, 16-byte aligned bases.  No split-K: workspace is ignored.
- * VT_EPI_GELU / VT_EPI_DGELU are rejected.  sm_90 only.
+ * sm_90 only.
  * ------------------------------------------------------------------------------------------- */
 typedef struct { vt_gemm_params g; const float* a_scale; const float* b_scale; } vt_gemm_e4m3_params;
 int vt_gemm_e4m3(const vt_gemm_e4m3_params* p, void* stream);
@@ -189,8 +189,9 @@ int vt_gather_cast_bf16(const vt_gather_cast_params* p, void* stream);
 
 /* Exact-erf GELU on bf16 (nn.GELU default, transformer.py:483 / :502) as stand-alone bandwidth kernels:
  *   vt_gelu_fwd_bf16: out = gelu(z)            vt_gelu_bwd_bf16: out = dh * gelu'(z)
- * The FFN uses them instead of the fused GEMM epilogues when the epilogue's erf math would out-cost the tile's
- * MMAs (4 erf per 4 columns in 8 epilogue warps); both forms are kept and tested. n = element count (n % 8 == 0). */
+ * These are the FFN's activation in training: FC1 writes z with VT_EPI_BF16 and vt_gelu_fwd_bf16 computes h from it;
+ * the backward takes dz from vt_gelu_bwd_bf16, or from vt_gelu_bwd_colsum_bf16 together with FC1's bias gradient.  Only
+ * the forward-only FC1 computes h in the GEMM (VT_EPI_GELU_H).  n = element count (n % 8 == 0). */
 typedef struct { const void* z; const void* dh; void* out; int64_t n; } vt_gelu_params;
 int vt_gelu_fwd_bf16(const vt_gelu_params* p, void* stream);
 int vt_gelu_bwd_bf16(const vt_gelu_params* p, void* stream);

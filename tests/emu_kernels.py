@@ -60,8 +60,8 @@ class EmuKernels:
     def _idx(self, t):
         return t.to(torch.int64)
 
-    def gemm(self, a, b, M, N, Kdim, *, a_mn=False, b_mn=False, epi='bf16', bias=None, bias2=None, out=None, out2=None,
-             aux=None, out_row=None, aux_row=None, row_scale=None, out_rows=None, split_ok=False,
+    def gemm(self, a, b, M, N, Kdim, *, a_mn=False, b_mn=False, epi='bf16', bias=None, bias2=None, out=None, aux=None,
+             out_row=None, aux_row=None, row_scale=None, out_rows=None, split_ok=False,
              force_splits=0, force_bn=0, row_map=None, tag=None):
         self.calls.append(('gemm', M, N, Kdim, a_mn, b_mn, epi))
         if row_map is not None:
@@ -86,15 +86,7 @@ class EmuKernels:
         acc = A @ Bm
         if bias is not None:
             acc = acc + self._up(bias)
-        if epi == 'gelu':
-            z = acc
-            h = 0.5 * z * (1 + torch.erf(z / math.sqrt(2.0)))
-            return self._h(z), self._h(h)
-        if epi == 'dgelu':
-            z = self._up(aux)
-            cdf = 0.5 * (1 + torch.erf(z / math.sqrt(2.0)))
-            pdf = torch.exp(-0.5 * z * z) / math.sqrt(2 * math.pi)
-            return self._h(acc * (cdf + z * pdf))
+        assert epi in ('bf16', 'f32', 'gelu_h') and (aux is None or epi == 'f32'), epi
         if row_scale is not None:
             acc = acc * self._up(row_scale)[:, None]
         if bias2 is not None:

@@ -76,22 +76,6 @@ def test_gemm_f32_residual_rowmaps():
     assert rel(out, exp) < 1e-5
 
 
-def test_gemm_gelu_and_dgelu():
-    M, N, Kd = 256, 512, 128
-    a, b = mk((M, Kd), 12, 0.3).bfloat16(), mk((N, Kd), 13, 0.3).bfloat16()
-    bias = mk((N,), 14)
-    z, h = K().gemm(a, b, M, N, Kd, epi='gelu', bias=bias)
-    zr = ref_mm(a, b, False, False) + bias
-    assert rel(z, zr) < 4e-3
-    assert rel(h, torch.nn.functional.gelu(zr)) < 4e-3
-    # dgelu: out = acc * gelu'(z)
-    g = mk((M, Kd), 15, 0.3).bfloat16()
-    out = K().gemm(g, b, M, N, Kd, epi='dgelu', aux=z)
-    zz = z.float().requires_grad_(True)
-    torch.nn.functional.gelu(zz).sum().backward()
-    assert rel(out, ref_mm(g, b, False, False) * zz.grad) < 4e-3
-
-
 @pytest.mark.parametrize('bn,staged', [(0, '1'), (128, '0'), (192, '1'), (256, '1')],
                          ids=['auto', 'bn128-register', 'bn192', 'bn256'])
 @pytest.mark.parametrize('splits', [2, 5, 16])
@@ -130,6 +114,55 @@ def test_gemm_rejects_bad_args():
         K().gemm(a.float(), b, 64, 64, 64)
     with pytest.raises(RuntimeError):
         K().gemm(a, b, 64, 60, 64)        # N not a multiple of 8 / shape mismatch
+    with pytest.raises(RuntimeError, match="'bf16', 'f32', 'gelu_h'"):
+        K().gemm(a, b, 64, 64, 64, epi='gelu')
+    with pytest.raises(RuntimeError, match='fp32 epilogue only'):
+        K().gemm(a, b, 64, 64, 64, epi='bf16', aux=a)
+
+
+def test_vt_gemm_refuses_retired_epilogues_and_bf16_addend():
+    """The C entry point refuses epilogue values 2 and 3 (the retired GELU / dGELU forms) and an addend with an epilogue
+    other than fp32, which no bf16 form reads: each call returns an error, launches nothing and leaves the output as it
+    was.  The same parameters with the plain bf16 epilogue and no addend run."""
+    import ctypes as C
+    from videotransformer_pytorch_b200 import _lib
+    lib = _lib.load_library()
+    M, N, Kd = 256, 256, 128
+    a, b = mk((M, Kd), 12, 0.3).bfloat16(), mk((N, Kd), 13, 0.3).bfloat16()
+    out = torch.full((M, N), 3.0, device='cuda', dtype=torch.bfloat16)
+    other = mk((M, N), 14).bfloat16()
+
+    def params(epilogue, out2=None, aux=None):
+        p = _lib.GemmParams()
+        p.a, p.b, p.lda, p.ldb = a.data_ptr(), b.data_ptr(), a.stride(0), b.stride(0)
+        p.M, p.N, p.K, p.epilogue = M, N, Kd, epilogue
+        p.out, p.ldo = out.data_ptr(), out.stride(0)
+        if out2 is not None:
+            p.out2, p.ldo2 = out2.data_ptr(), out2.stride(0)
+        if aux is not None:
+            p.aux, p.ldaux = aux.data_ptr(), aux.stride(0)
+        p.map_special_base = -1
+        return p
+
+    for what, p, msg in (('epilogue 2', params(2, out2=other.clone()), 'bad epilogue 2'),
+                         ('epilogue 3', params(3, aux=other), 'bad epilogue 3'),
+                         ('bf16 with aux', params(_lib.EPI['bf16'], aux=other), 'aux'),
+                         ('gelu_h with aux', params(_lib.EPI['gelu_h'], aux=other), 'aux')):
+        torch.cuda.synchronize()
+        n0 = _lib.launch_count()
+        rc = lib.vt_gemm(C.byref(p), _lib._stream())
+        torch.cuda.synchronize()
+        err = C.create_string_buffer(512)
+        lib.vt_last_error(err, 512)
+        assert rc != 0, what
+        assert msg in err.value.decode(), (what, err.value)
+        assert _lib.launch_count() == n0, what
+        assert bool((out == 3.0).all()), what
+    n0 = _lib.launch_count()
+    assert lib.vt_gemm(C.byref(params(_lib.EPI['bf16'])), _lib._stream()) == 0
+    torch.cuda.synchronize()
+    assert _lib.launch_count() == n0 + 1
+    assert rel(out, ref_mm(a, b, False, False)) < 4e-3
 
 
 @pytest.mark.parametrize('M,N,Kd', [(12552, 768, 3072), (12608, 2304, 768), (1000, 576, 192)])
@@ -170,7 +203,7 @@ def test_gemm_forced_tile_widths(M, N, Kd, a_mn, b_mn, bn):
     assert rel(out, ref_mm(a, b, a_mn, b_mn)) < 1e-5
 
 
-@pytest.mark.parametrize('epi', ['bf16', 'f32res', 'gelu', 'dgelu'])
+@pytest.mark.parametrize('epi', ['bf16', 'f32res'])
 def test_gemm_epilogues_partial_last_tile(epi):
     """every epilogue with M = 1000: the last row of tiles holds 104 valid rows"""
     M, N, Kd = 1000, 512, 256
@@ -188,18 +221,9 @@ def test_gemm_epilogues_partial_last_tile(epi):
         exp = torch.zeros(M, N, device='cuda')
         exp[perm.long()] = r + bias + aux[perm.long()]
         assert rel(out, exp) < 1e-5
-    elif epi == 'gelu':
-        z, h = K().gemm(a, b, M, N, Kd, epi='gelu', bias=bias)
-        assert rel(z, r + bias) < 4e-3 and rel(h, torch.nn.functional.gelu(r + bias)) < 4e-3
-    else:
-        z = mk((M, N), 45).bfloat16()
-        out = K().gemm(a, b, M, N, Kd, epi='dgelu', aux=z)
-        zz = z.float().requires_grad_(True)
-        torch.nn.functional.gelu(zz).sum().backward()
-        assert rel(out, r * zz.grad) < 4e-3
 
 
-# ---- fp32 residual epilogue with plain rows and affine row maps, short last row tiles, GELU / dGELU epilogues ----------
+# ---- fp32 residual epilogue with plain rows and affine row maps, short last row tiles ---------------------------------
 def _ops():
     from videotransformer_pytorch_b200 import ops
     return ops
@@ -282,30 +306,6 @@ def test_short_last_row_tile_deterministic(bn, M, N, Kd, form):
     tol = 1e-5 if form == 'fwd_f32_residual' else 4e-3
     assert rel(got, r) < tol
     assert torch.equal(got, again)
-
-
-@pytest.mark.parametrize('staged', ['0', '1'], ids=['register', 'staged'])
-@pytest.mark.parametrize('M,N,Kd', [(12552, 3072, 768), (1000, 512, 128), (130, 96, 64)])
-def test_gelu_and_dgelu_epilogues_deterministic(M, N, Kd, staged, monkeypatch):
-    """FC1 with z and h = gelu(z) from one epilogue, and the FC2 data gradient with gelu'(z) multiplied in, on the register
-    and on the staged epilogue: both match torch, and a second call gives the same bits."""
-    monkeypatch.setenv('VT_GEMM_STAGED_EPI', staged)
-    a, b = mk((M, Kd), 60, 0.3).bfloat16(), mk((N, Kd), 61, 0.3).bfloat16()
-    bias = mk((N,), 62)
-    z, h = K().gemm(a, b, M, N, Kd, epi='gelu', bias=bias)
-    zr = ref_mm(a, b, False, False) + bias
-    assert rel(z, zr) < 4e-3 and rel(h, torch.nn.functional.gelu(zr)) < 4e-3
-    z_again, _ = K().gemm(a, b, M, N, Kd, epi='gelu', bias=bias)
-    # h is taken from the bf16-rounded z: identical to the stand-alone GELU kernel on z
-    assert torch.equal(z, z_again) and torch.equal(h, K().gelu(z))
-    g = mk((M, Kd), 63, 0.3).bfloat16()
-    w = mk((Kd, N), 64, 0.3).bfloat16()                       # [n_out = Kd, k_in = N], read MN-major
-    d = K().gemm(g, w, M, N, Kd, b_mn=True, epi='dgelu', aux=z)
-    d_again = K().gemm(g, w, M, N, Kd, b_mn=True, epi='dgelu', aux=z)
-    zz = z.float().requires_grad_(True)
-    torch.nn.functional.gelu(zz).sum().backward()
-    assert rel(d_again, (g.float() @ w.float()) * zz.grad) < 4e-3
-    assert torch.equal(d, d_again)
 
 
 @pytest.mark.parametrize('staged', ['0', '1'], ids=['register', 'staged'])

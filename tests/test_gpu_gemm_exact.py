@@ -4,14 +4,14 @@ A. Exact regime (tests/gemm_exact.py): integer operands and dyadic epilogue oper
    output must equal the float64 result rounded once, bit for bit: every form, both epilogue paths, every tile width and
    operand layout, tile / k-block edges, split-K, the persistent walk on reduced grids and M a few rows past a tile.
    Which kernel each configuration reaches is read from torch.profiler, in one session in a child process
-   (test_dispatch_reaches_every_tensor_core_cell): a profiler session per case, in the process that runs the suite, left
-   the later sessions of that process without records of kernels that had already run, and so blinded the profiler
-   checks of other modules.
+   (test_dispatch_reaches_every_register_and_staged_cell): a profiler session per case, in the process that runs the
+   suite, left the later sessions of that process without records of kernels that had already run, and so blinded the
+   profiler checks of other modules.
 B. Every operand is a view into a NaN-filled allocation (padded pitch, rows past K / M / N), and every output lives in a
    sentinel-filled buffer with a padded pitch, so a read the tensor maps should have clipped turns
    outputs into NaN, and a stray write changes a sentinel.
-C. GELU over all 65 536 bf16 inputs, stand-alone and through the GEMM epilogues, against the float64 GELU within the
-   derived per-element bound of tests/gemm_exact.py.
+C. GELU over all 65 536 bf16 inputs: the stand-alone kernels against the float64 GELU within the derived per-element
+   bound of tests/gemm_exact.py, and the forward-only gelu_h epilogue bit for bit against the stand-alone kernel.
 D. Gaussian operands at the model's shapes against float64 within K 2^-23 (|A||B|)_mn plus the epilogue's roundings.
 E. Host checks of the reference arithmetic (no GPU).
 """
@@ -25,14 +25,9 @@ import torch
 
 from tests import gemm_exact as X
 
-FORMS = ('bf16', 'f32', 'gelu', 'dgelu', 'gelu_h')
+FORMS = ('bf16', 'f32', 'gelu_h')
 SENT16 = 0x7FAB                          # bf16 NaN payload no kernel writes
 SENT32 = 0x7FC0DEAD                      # fp32 NaN payload no kernel writes
-# dgelu's z: gelu'(z) is exactly 1 in fp32 for z >= 8 (exp(-z^2 / 2) < 2^-46 leaves 1 - P t e and 1 + z c e at 1), and
-# exactly +0 for z <= -16 (exp(-128) is below the smallest fp32 subnormal, so 0.5 (1 - 1) + z c 0 = +0).  Between -16
-# and about -13 __expf returns a subnormal and gelu'(z) is a tiny negative number, not zero.
-DGELU_ONE = (8.0, 12.0, 16.0, 96.0, 1024.0, 30720.0)
-DGELU_ZERO = (-16.0, -20.0, -24.0, -100.0, -1024.0, -30720.0)
 
 
 def K():
@@ -104,8 +99,6 @@ def expected_cell(form, staged, bn, ta, tb):
         return ('wgmma', 0, bn, ta, tb)
     if form in ('bf16', 'gelu_h'):
         return ('wgmma', 1, bn, ta, tb)
-    if form in ('gelu', 'dgelu'):
-        return ('wgmma', 2, bn, ta, tb)
     return ('wgmma', 0, bn, ta, tb) if bn == 256 else ('f32', 3, bn, ta, tb)
 
 
@@ -118,22 +111,13 @@ def int_operands(M, N, Kd, ta, tb, seed, pad):
     return A, B, a, b
 
 
-def dgelu_z(M, N, seed):
-    """z of the exact dgelu checks: each element from DGELU_ONE or DGELU_ZERO; -> (z [M, N] fp32, mask of gelu' = 1)"""
-    g = torch.Generator(device='cpu').manual_seed(seed)
-    one = torch.rand((M, N), generator=g) < 0.5
-    pick = torch.randint(0, len(DGELU_ONE), (M, N), generator=g)
-    z = torch.where(one, torch.tensor(DGELU_ONE)[pick], torch.tensor(DGELU_ZERO)[pick])
-    return z, one
-
-
 def run_exact(form, M, N, Kd, *, ta=0, tb=0, bn=0, seed=0, pad=8, bias=False, rs=False, aux=False, bias2=False,
               rowmap=False, tag=''):
     """one vt_gemm call in the exact regime, checked bit for bit over its whole output buffers"""
     A, B, a, b = int_operands(M, N, Kd, ta, tb, seed, pad)
     g = seed * 7 + 3
     bias_t = X.quarter_values((N,), g) if bias else None
-    rs_t = X.pow2_scale(M, g + 1) if rs and form in ('bf16', 'gelu_h', 'f32') else None
+    rs_t = X.pow2_scale(M, g + 1) if rs else None
     Raux = M + 5
     aux_t = X.quarter_values((Raux, N), g + 2) if aux and form == 'f32' else None
     bias2_t = X.quarter_values((N,), g + 3) if bias2 and aux_t is not None else None
@@ -148,7 +132,7 @@ def run_exact(form, M, N, Kd, *, ta=0, tb=0, bn=0, seed=0, pad=8, bias=False, rs
     gen = torch.Generator(device='cpu').manual_seed(g + 4)
     R = M
     rows = torch.arange(M)
-    if rowmap and form in ('bf16', 'gelu_h', 'f32'):
+    if rowmap:
         R = M + 3
         rows = torch.randperm(R, generator=gen)[:M]
         rows[torch.rand(M, generator=gen) < 0.15] = -1
@@ -164,13 +148,6 @@ def run_exact(form, M, N, Kd, *, ta=0, tb=0, bn=0, seed=0, pad=8, bias=False, rs
     odt = torch.float32 if form == 'f32' else torch.bfloat16
     out = Out(R, N, odt, 3)
     kw['out'] = out.view
-    out2 = None
-    if form == 'gelu':
-        out2 = Out(M, N, torch.bfloat16, 5)
-        kw['out2'] = out2.view
-    if form == 'dgelu':
-        z, one = dgelu_z(M, N, g + 5)
-        kw['aux'] = nan_view(z, 3)
     K().gemm(a, b, M, N, Kd, **kw)
 
     v = A.double().cuda() @ B.double().cuda().t()
@@ -190,33 +167,19 @@ def run_exact(form, M, N, Kd, *, ta=0, tb=0, bn=0, seed=0, pad=8, bias=False, rs
     tag = f'{tag} {form} M={M} N={N} K={Kd} ta={ta} tb={tb} bn={bn} bias={bias} rs={rs} aux={aux} bias2={bias2} map={rowmap}'
     if form == 'f32':
         out.check(out.expected(dst, X.round_once(v, torch.float32)[keep.cuda()]), tag)
-    elif form in ('bf16', 'gelu'):
-        zb = X.round_once(v, torch.bfloat16)
-        out.check(out.expected(dst, zb[keep.cuda()]), tag)
-        if form == 'gelu':
-            out2.check(out2.expected(torch.arange(M, device='cuda'), K().gelu(zb.contiguous())), tag + ' (h)')
-    elif form == 'gelu_h':
+    elif form == 'bf16':
+        out.check(out.expected(dst, X.round_once(v, torch.bfloat16)[keep.cuda()]), tag)
+    else:  # gelu_h
         h = K().gelu(X.round_once(v, torch.bfloat16).contiguous())
         out.check(out.expected(dst, h[keep.cuda()]), tag)
-    else:  # dgelu: gelu'(z) = 1 -> bf16(v); gelu'(z) = +0 -> +0 / -0 by the sign of v (either sign where v = 0)
-        vb = X.round_once(v, torch.bfloat16).view(torch.int16)
-        one = one.cuda()
-        zero_bits = torch.where(v < 0, torch.full_like(vb, -0x8000), torch.zeros_like(vb))
-        exp_bits = torch.where(one, vb, zero_bits)
-        got_bits = out.view.view(torch.int16)
-        either = (~one) & (v == 0) & ((got_bits == 0) | (got_bits == -0x8000))
-        exp_bits = torch.where(either, got_bits, exp_bits)
-        out.check(out.expected(dst, exp_bits.view(torch.bfloat16)), tag)
 
 
 def variants(form):
     if form in ('bf16', 'gelu_h'):
         return [{}, dict(bias=True), dict(rs=True), dict(bias=True, rs=True), dict(bias=True, rs=True, rowmap=True)]
-    if form == 'f32':
-        return [{}, dict(bias=True), dict(rs=True), dict(aux=True), dict(aux=True, bias2=True),
-                dict(bias=True, rs=True, aux=True, bias2=True), dict(bias=True, rs=True, aux=True, bias2=True, rowmap=True),
-                dict(bias=True, rowmap=True)]
-    return [{}, dict(bias=True)]
+    return [{}, dict(bias=True), dict(rs=True), dict(aux=True), dict(aux=True, bias2=True),
+            dict(bias=True, rs=True, aux=True, bias2=True), dict(bias=True, rs=True, aux=True, bias2=True, rowmap=True),
+            dict(bias=True, rowmap=True)]
 
 
 # M, N, K: partial row and column tiles, one row, below one k-block, partial last k-blocks, several n-tiles
@@ -232,7 +195,7 @@ CELL_SHAPES = ((129, 200, 136), (1, 8, 8), (8, 72, 40), (127, 776, 72))
 @pytest.mark.parametrize('form', FORMS)
 def test_exact_cell(form, staged, bn, ta, tb, monkeypatch):
     """every form x epilogue path x tile width x operand layout on small edge shapes, bit for bit (the kernel each of
-    these configurations reaches: test_dispatch_reaches_every_tensor_core_cell)"""
+    these configurations reaches: test_dispatch_reaches_every_register_and_staged_cell)"""
     monkeypatch.setenv('VT_GEMM_STAGED_EPI', str(staged))
     for i, (M, N, Kd) in enumerate(CELL_SHAPES):
         for j, var in enumerate(variants(form)):
@@ -240,10 +203,10 @@ def test_exact_cell(form, staged, bn, ta, tb, monkeypatch):
 
 
 def dispatch_probe():
-    """Body of the child process of test_dispatch_reaches_every_tensor_core_cell: one vt_gemm call per configuration
-    of test_exact_cell (shape 129 x 200 x 136), all inside one torch.profiler session, with every operand allocated
-    before it.  Prints one JSON line: the configurations in call order and the cells of the GEMM kernels in launch
-    order."""
+    """Body of the child process of test_dispatch_reaches_every_register_and_staged_cell: one vt_gemm call per
+    configuration of test_exact_cell (shape 129 x 200 x 136), all inside one torch.profiler session, with every operand
+    allocated before it.  Prints one JSON line: the configurations in call order and the cells of the GEMM kernels in
+    launch order."""
     import itertools
     import json
     import os
@@ -254,10 +217,6 @@ def dispatch_probe():
         _, _, a, b = int_operands(M, N, Kd, ta, tb, seed=1, pad=8)
         kw = dict(a_mn=bool(ta), b_mn=bool(tb), epi=form, force_bn=bn,
                   out=torch.empty((M, N), dtype=torch.float32 if form == 'f32' else torch.bfloat16, device='cuda'))
-        if form == 'gelu':
-            kw['out2'] = torch.empty((M, N), dtype=torch.bfloat16, device='cuda')
-        if form == 'dgelu':
-            kw['aux'] = dgelu_z(M, N, 2)[0].bfloat16().cuda()
         calls.append(([form, staged, bn, ta, tb], {'VT_GEMM_STAGED_EPI': str(staged)}, (a, b, M, N, Kd), kw))
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
@@ -271,7 +230,7 @@ def dispatch_probe():
 
 
 @pytest.mark.gpu
-def test_dispatch_reaches_every_tensor_core_cell():
+def test_dispatch_reaches_every_register_and_staged_cell():
     """The kernel cell each configuration of test_exact_cell reaches: every (kernel, SE, BN, TA, TB) cell of the bf16
     wgmma GEMM that the dispatch can reach.  Calls run in order on one stream, so the i-th GEMM kernel launched belongs
     to the i-th call."""
@@ -293,7 +252,7 @@ def test_dispatch_reaches_every_tensor_core_cell():
         want = expected_cell(form, staged, bn, ta, tb) if bn else (cell[0], cell[1], cell[2], ta, tb)
         assert cell == want, (cfg, cell, want)
         reached.setdefault(cell, []).append(cfg)
-    want_cells = {('wgmma', se, bn, ta, tb) for se in (0, 1, 2) for bn in (128, 192, 256) for ta in (0, 1) for tb in (0, 1)}
+    want_cells = {('wgmma', se, bn, ta, tb) for se in (0, 1) for bn in (128, 192, 256) for ta in (0, 1) for tb in (0, 1)}
     want_cells |= {('f32', 3, bn, ta, tb) for bn in (128, 192) for ta in (0, 1) for tb in (0, 1)}
     assert want_cells <= set(reached), sorted(want_cells - set(reached))
     for cell in sorted(reached):
@@ -302,8 +261,7 @@ def test_dispatch_reaches_every_tensor_core_cell():
 
 @pytest.mark.gpu
 @pytest.mark.parametrize('form,M,N,Kd,tb', [('bf16', 12552, 2304, 768, 0), ('bf16', 12552, 768, 2304, 1),
-                                            ('f32', 12552, 768, 3072, 0), ('gelu', 12552, 3072, 768, 0),
-                                            ('gelu_h', 12552, 3072, 768, 0), ('dgelu', 12552, 3072, 768, 1)])
+                                            ('f32', 12552, 768, 3072, 0), ('gelu_h', 12552, 3072, 768, 0)])
 def test_exact_persistent_walk(form, M, N, Kd, tb, monkeypatch):
     """the model's shapes with every SM, one fewer and 64 fewer: many tiles per CTA, each CTA's ring and staging buffers
     reused across tiles of different row and column blocks"""
@@ -438,12 +396,11 @@ def test_gelu_every_bf16_input():
 @pytest.mark.gpu
 @pytest.mark.parametrize('staged', [0, 1])
 @pytest.mark.parametrize('bn', [0, 128, 256])
-def test_gelu_epilogues_every_bf16_input(bn, staged, monkeypatch):
-    """the same patterns as GEMM outputs (a = the pattern matrix, b = identity): gelu's z must come out unchanged and its
-    h, like gelu_h's output, equal the stand-alone kernel's result bit for bit; dgelu with z = every pattern (aux) and
-    acc = +-2^j must give +-2^j times the stand-alone gelu' table except where a value is subnormal.  Non-finite patterns
-    cannot pass through the MMA (NaN / inf times the identity's zeros spoils the row) and neither can -0 (the zeros of
-    the other products make it +0): those enter a as 0 and are checked by the stand-alone test."""
+def test_gelu_h_epilogue_every_bf16_input(bn, staged, monkeypatch):
+    """the same patterns as GEMM outputs (a = the pattern matrix, b = identity): gelu_h's output must equal the
+    stand-alone kernel's result bit for bit.  Non-finite patterns cannot pass through the MMA (NaN / inf times the
+    identity's zeros spoils the row) and neither can -0 (the zeros of the other products make it +0): those enter a as 0
+    and are checked by the stand-alone test."""
     monkeypatch.setenv('VT_GEMM_STAGED_EPI', str(staged))
     bits = all_bf16().cuda()
     pat = bits.view(torch.bfloat16)
@@ -451,27 +408,8 @@ def test_gelu_epilogues_every_bf16_input(bn, staged, monkeypatch):
     a = torch.where(ok, pat, torch.zeros_like(pat))
     eye = torch.eye(256, device='cuda').bfloat16()
     table_h = K().gelu(a)
-    z, h = K().gemm(nan_view(a, 8), nan_view(eye, 8), 256, 256, 256, epi='gelu', force_bn=bn)
-    assert torch.equal(z.contiguous().view(torch.int16), a.view(torch.int16))
+    h = K().gemm(nan_view(a, 8), nan_view(eye, 8), 256, 256, 256, epi='gelu_h', force_bn=bn)
     assert torch.equal(h.contiguous().view(torch.int16), table_h.view(torch.int16))
-    hh = K().gemm(nan_view(a, 8), nan_view(eye, 8), 256, 256, 256, epi='gelu_h', force_bn=bn)
-    assert torch.equal(hh.contiguous().view(torch.int16), table_h.view(torch.int16))
-    # dgelu: a[m, 0] = s_m = +-2^j and b[n, 0] = 1, every other element 0, so acc[m, n] = s_m exactly
-    j = torch.arange(256, device='cuda') % 7 - 3
-    s = torch.where(torch.arange(256, device='cuda') % 2 == 0, 1.0, -1.0) * torch.exp2(j.float())
-    ga = torch.zeros((256, 256), device='cuda')
-    ga[:, 0] = s
-    gb = torch.zeros((256, 256), device='cuda')
-    gb[:, 0] = 1.0
-    table_d = K().dgelu(torch.ones_like(pat), pat).float()
-    out = K().gemm(nan_view(ga, 8), nan_view(gb, 8), 256, 256, 256, epi='dgelu', aux=nan_view(pat, 8),
-                   force_bn=bn).float()
-    exp = s[:, None] * table_d
-    nan = torch.isnan(exp)
-    sub = (exp.abs() < X.TINY) | (table_d.abs() < X.TINY)
-    assert torch.equal(torch.isnan(out), nan)
-    same = (out == exp) | nan | (sub & ((out - exp).abs() <= X.TINY))
-    assert bool(same.all()), int((~same).sum())
 
 
 # ---- D: random operands against the fp64 bound --------------------------------------------------------------------

@@ -41,7 +41,7 @@ def rows_for(n_tiles_per_cta):
 
 @pytest.mark.parametrize('bn', [128, 192, 256])
 @pytest.mark.parametrize('N', [136, 200])
-@pytest.mark.parametrize('form', ['bf16', 'f32res', 'gelu', 'dgelu'])
+@pytest.mark.parametrize('form', ['bf16', 'f32res'])
 def test_epilogues_across_tiles(form, N, bn, reserved):
     K = reserved
     M, Kd = rows_for(2.5), 72
@@ -51,7 +51,7 @@ def test_epilogues_across_tiles(form, N, bn, reserved):
     if form == 'bf16':
         out = K.gemm(a, b, M, N, Kd, epi='bf16', bias=bias, row_scale=rs, force_bn=bn)
         assert rel(out, (r + bias) * rs[:, None]) < 4e-3
-    elif form == 'f32res':
+    else:
         R = M + 50
         aux = mk((R, N), 5)
         out_row = torch.randperm(R, generator=torch.Generator().manual_seed(0))[:M].to(torch.int32).cuda()
@@ -66,16 +66,6 @@ def test_epilogues_across_tiles(form, N, bn, reserved):
         ok = out_row >= 0
         exp[out_row[ok].long()] = y[ok]
         assert rel(out, exp) < 1e-5
-    elif form == 'gelu':
-        z, h = K.gemm(a, b, M, N, Kd, epi='gelu', bias=bias, force_bn=bn)
-        assert rel(z, r + bias) < 4e-3 and rel(h, torch.nn.functional.gelu(r + bias)) < 4e-3
-        assert torch.equal(h, K.gelu(z))
-    else:
-        z = mk((M, N), 6).bfloat16()
-        out = K.gemm(a, b, M, N, Kd, epi='dgelu', aux=z, force_bn=bn)
-        zz = z.float().requires_grad_(True)
-        torch.nn.functional.gelu(zz).sum().backward()
-        assert rel(out, r * zz.grad) < 4e-3
 
 
 @pytest.mark.parametrize('bn', [128, 192, 256])
@@ -123,7 +113,7 @@ def _bitwise_case(seed):
 
 
 @pytest.mark.parametrize('bn', [128, 192, 256])
-def test_bitwise_independent_of_grid_and_run(bn):
+def test_f32_gelu_h_split_k_bitwise_independent_of_grid_and_run(bn):
     """fixed tile width and split count: identical bits for the full grid, a 64-SM-smaller grid, and a second run"""
     K = lib().K
     M, N, Kd, a, b, bias, aux = _bitwise_case(20)
@@ -131,9 +121,9 @@ def test_bitwise_independent_of_grid_and_run(bn):
 
     def run():
         y = K.gemm(a, b, M, N, Kd, epi='f32', bias=bias, aux=aux, force_bn=bn)
-        z, h = K.gemm(a, b, M, N, Kd, epi='gelu', bias=bias, force_bn=bn)
+        h = K.gemm(a, b, M, N, Kd, epi='gelu_h', bias=bias, force_bn=bn)
         g = K.gemm(dy, x, 384, 200, 2000, a_mn=True, b_mn=True, epi='f32', split_ok=True, force_splits=3, force_bn=bn)
-        return [y, z, h, g]
+        return [y, h, g]
 
     try:
         full = run()

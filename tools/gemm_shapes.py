@@ -13,7 +13,7 @@ rate this card reaches at its power limit.
 The evaluation forward's FC1 is timed both ways: 'gelu_h' (h alone from the epilogue) against the split form it replaces,
 the 'bf16' GEMM that writes z plus the stand-alone GELU kernel (its own row, "gelu kernel").
 
---k-sweep times the wide-output GEMMs (qkv forward, FC1 forward with GELU, FC2 data gradient with dGELU) at their M x N
+--k-sweep times the wide-output GEMMs (qkv forward, the forward-only FC1 with gelu_h, FC2 data gradient) at their M x N
 with K = 768, 1536, 3072 and 6144 and BN = 128, and fits the time per wave of tiles, t_tile = a * k-blocks + e: e is the
 per-tile cost that does not scale with K (epilogue, pipeline fill), printed for both epilogues.
 
@@ -37,7 +37,7 @@ B, T, P, D, HID = 8, 8, 196, 768, 3072
 S = 1 + P * T
 M_TOK, M_TEMP, M_SPAT = B * S, B * P * T, B * T * (P + 1)     # 12552, 12544, 12608
 SWITCH = 'VT_GEMM_STAGED_EPI'
-SWEEP = ('qkv fwd temporal', 'fc1 fwd (gelu)', 'fc2 dgrad (dgelu)')
+SWEEP = ('qkv fwd temporal', 'fc1 fwd eval (gelu_h)', 'fc2 dgrad')
 SWEEP_K = (768, 1536, 3072, 6144)
 
 
@@ -89,7 +89,6 @@ def cases(dev):
     aff = ops.affine_row_maps(B, T, P, D)
     bias_d, bias_3d, bias_h = (torch.randn(n, device=dev) for n in (D, 3 * D, HID))
     stream = torch.randn(B * S + B * T, D, device=dev)
-    z = torch.randn(M_TOK, HID, device=dev).bfloat16()
     out = [
         ('qkv fwd temporal', M_TEMP, 3 * D, D, (0, 0), dict(epi='bf16', bias=bias_3d), 2, True),
         ('qkv fwd spatial', M_SPAT, 3 * D, D, (0, 0), dict(epi='bf16', bias=bias_3d), 2, True),
@@ -99,11 +98,10 @@ def cases(dev):
         ('proj fwd spatial (affine, cls rows)', M_SPAT, D, D, (0, 0),
          dict(epi='f32', bias=bias_d, aux=stream, out=stream, aux_row=maps['sp_aux'], out_row=maps['sp_out'],
               row_map=aff['spatial']), 8, False),
-        ('fc1 fwd (gelu)', M_TOK, HID, D, (0, 0), dict(epi='gelu', bias=bias_h), 4, False),
         ('fc1 fwd eval (gelu_h)', M_TOK, HID, D, (0, 0), dict(epi='gelu_h', bias=bias_h), 2, False),
         ('fc1 fwd split (bf16; + gelu kernel)', M_TOK, HID, D, (0, 0), dict(epi='bf16', bias=bias_h), 2, False),
         ('fc2 fwd (f32 residual)', M_TOK, D, HID, (0, 0), dict(epi='f32', bias=bias_d, aux=stream[:M_TOK]), 8, False),
-        ('fc2 dgrad (dgelu)', M_TOK, HID, D, (0, 1), dict(epi='dgelu', aux=z), 4, False),
+        ('fc2 dgrad', M_TOK, HID, D, (0, 1), dict(epi='bf16'), 2, False),
         ('fc1 dgrad', M_TOK, D, HID, (0, 1), dict(epi='bf16'), 2, True),
         ('proj dgrad', M_TEMP, D, D, (0, 1), dict(epi='bf16'), 2, True),
         ('qkv dgrad', M_TEMP, D, 3 * D, (0, 1), dict(epi='bf16'), 2, True),

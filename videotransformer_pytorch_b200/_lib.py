@@ -15,7 +15,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libvt_b200.so')
 
-EPI = {'bf16': 0, 'f32': 1, 'gelu': 2, 'dgelu': 3, 'gelu_h': 4}
+EPI = {'bf16': 0, 'f32': 1, 'gelu_h': 4}
 
 c_i32, c_i64, c_f32, c_vp = C.c_int32, C.c_int64, C.c_float, C.c_void_p
 
@@ -376,36 +376,33 @@ class CudaKernels:
         return ws
 
     # -- GEMM ---------------------------------------------------------------------------------
-    def gemm(self, a, b, M, N, Kdim, *, a_mn=False, b_mn=False, epi='bf16', bias=None, bias2=None, out=None, out2=None,
-             aux=None, out_row=None, aux_row=None, row_scale=None, out_rows=None, split_ok=False,
+    def gemm(self, a, b, M, N, Kdim, *, a_mn=False, b_mn=False, epi='bf16', bias=None, bias2=None, out=None, aux=None,
+             out_row=None, aux_row=None, row_scale=None, out_rows=None, split_ok=False,
              force_splits=0, force_bn=0, row_map=None, tag=None):
         """row_map: affine description of out_row / aux_row (ops.affine_row_maps) for the fp32 residual epilogue — the kernel
         computes each row's output and residual addresses from it instead of reading the index arrays.  tag: role label of the launch
         ('qkv', 'proj', ...) for profilers that wrap this method (bench.py); ignored here."""
-        p, out, out2 = self._gemm_params(a, b, M, N, Kdim, torch.bfloat16, a_mn=a_mn, b_mn=b_mn, epi=epi, bias=bias, bias2=bias2,
-                                         out=out, out2=out2, aux=aux, out_row=out_row, aux_row=aux_row, row_scale=row_scale,
-                                         out_rows=out_rows, split_ok=split_ok, force_splits=force_splits, force_bn=force_bn,
-                                         row_map=row_map)
+        p, out = self._gemm_params(a, b, M, N, Kdim, torch.bfloat16, a_mn=a_mn, b_mn=b_mn, epi=epi, bias=bias, bias2=bias2,
+                                   out=out, aux=aux, out_row=out_row, aux_row=aux_row, row_scale=row_scale,
+                                   out_rows=out_rows, split_ok=split_ok, force_splits=force_splits, force_bn=force_bn,
+                                   row_map=row_map)
         _check(load_library().vt_gemm(C.byref(p), _stream()), 'vt_gemm')
-        return (out, out2) if epi == 'gelu' else out
+        return out
 
     def gemm_e4m3(self, a, b, M, N, Kdim, *, epi='bf16', bias=None, bias2=None, out=None, aux=None, out_row=None,
                   aux_row=None, row_scale=None, out_rows=None, force_bn=0, row_map=None, tag=None):
         """The fp8 forward form of gemm(): a, b are E4M3 operands ([M, K] and [N, K], K-major) and the product is
-        dequantised by a.scale[m] * b.scale[n] before the epilogue.  Epilogues 'bf16', 'f32' and 'gelu_h' only; the rest of
-        the arguments are gemm()'s."""
+        dequantised by a.scale[m] * b.scale[n] before the epilogue; the rest of the arguments are gemm()'s."""
         if not isinstance(a, E4M3) or not isinstance(b, E4M3):
             raise RuntimeError('gemm_e4m3: both operands must be E4M3 (quantised rows + scales)')
-        if epi not in ('bf16', 'f32', 'gelu_h'):
-            raise RuntimeError(f'gemm_e4m3: epilogue {epi!r} has no fp8 form')
         check_fp8_device(a.q.device)
         for nm, op, rows in (('a', a, M), ('b', b, N)):
             _req(op.scale, torch.float32, f'gemm_e4m3.{nm}.scale')
             if op.scale.numel() != rows or not op.scale.is_contiguous():
                 raise RuntimeError(f'gemm_e4m3.{nm}.scale: expected {rows} contiguous entries, got {op.scale.numel()}')
-        p, out, _ = self._gemm_params(a.q, b.q, M, N, Kdim, torch.float8_e4m3fn, epi=epi, bias=bias, bias2=bias2, out=out,
-                                      aux=aux, out_row=out_row, aux_row=aux_row, row_scale=row_scale, out_rows=out_rows,
-                                      force_bn=force_bn, row_map=row_map)
+        p, out = self._gemm_params(a.q, b.q, M, N, Kdim, torch.float8_e4m3fn, epi=epi, bias=bias, bias2=bias2, out=out,
+                                   aux=aux, out_row=out_row, aux_row=aux_row, row_scale=row_scale, out_rows=out_rows,
+                                   force_bn=force_bn, row_map=row_map)
         q = GemmE4m3Params()
         q.g, q.a_scale, q.b_scale = p, a.scale.data_ptr(), b.scale.data_ptr()
         _check(load_library().vt_gemm_e4m3(C.byref(q), _stream()), 'vt_gemm_e4m3')
@@ -428,9 +425,13 @@ class CudaKernels:
         return E4M3(q, scale)
 
     def _gemm_params(self, a, b, M, N, Kdim, op_dtype, *, a_mn=False, b_mn=False, epi='bf16', bias=None, bias2=None, out=None,
-                     out2=None, aux=None, out_row=None, aux_row=None, row_scale=None, out_rows=None, split_ok=False,
+                     aux=None, out_row=None, aux_row=None, row_scale=None, out_rows=None, split_ok=False,
                      force_splits=0, force_bn=0, row_map=None):
         """vt_gemm_params of one call (operands of dtype op_dtype), with the output allocated when not given."""
+        if epi not in EPI:
+            raise RuntimeError(f'gemm: unknown epilogue {epi!r} (expected one of {", ".join(map(repr, EPI))})')
+        if aux is not None and epi != 'f32':
+            raise RuntimeError(f'gemm.aux: the addend is for the fp32 epilogue only (epi="f32"), not {epi!r}')
         _rows2d(_req(a, op_dtype, 'gemm.a'), 'gemm.a')
         _rows2d(_req(b, op_dtype, 'gemm.b'), 'gemm.b')
         exp_a = (Kdim, M) if a_mn else (M, Kdim)
@@ -441,8 +442,6 @@ class CudaKernels:
         if out is None:
             out = torch.empty((out_rows if out_rows is not None else M, N), dtype=odt, device=a.device)
         _rows2d(_req(out, odt, 'gemm.out'), 'gemm.out')
-        if epi == 'gelu' and out2 is None:
-            out2 = torch.empty_like(out)
         p = GemmParams()
         p.a, p.b = a.data_ptr(), b.data_ptr()
         p.lda, p.ldb = a.stride(0), b.stride(0)
@@ -453,10 +452,8 @@ class CudaKernels:
         if bias2 is not None:                  # fp32 epilogue with aux only: added after the row scale
             p.bias2 = _req(bias2, torch.float32, 'gemm.bias2').data_ptr()
         p.out, p.ldo = out.data_ptr(), out.stride(0)
-        if out2 is not None:
-            p.out2, p.ldo2 = out2.data_ptr(), out2.stride(0)
         if aux is not None:
-            _rows2d(_req(aux, torch.float32 if epi == 'f32' else torch.bfloat16, 'gemm.aux'), 'gemm.aux')
+            _rows2d(_req(aux, torch.float32, 'gemm.aux'), 'gemm.aux')
             p.aux, p.ldaux = aux.data_ptr(), aux.stride(0)
         for nm, t in (('out_row', out_row), ('aux_row', aux_row)):
             if t is not None:
@@ -482,7 +479,7 @@ class CudaKernels:
             p.map_stride_t, p.map_stride_p, p.map_stride_b = row_map['stride_t'], row_map['stride_p'], row_map['stride_b']
             p.map_base = row_map['base']
             p.map_special_base, p.map_special_stride = row_map.get('special_base', -1), row_map.get('special_stride', 0)
-        return p, out, out2
+        return p, out
 
     # -- LayerNorm ----------------------------------------------------------------------------
     def ln_fwd(self, x2d, gamma, beta, eps, in_row=None, rows=None, out_fp32=False, stats=True):

@@ -218,7 +218,8 @@ def _lse(save):
 
 def _fc1_gelu(k, xn, w1h, b1, M, Dh, D, save):
     """(z, h) of h = gelu(z), z = xn W1^T + b1, both bf16.  Saving forward: a 'bf16' GEMM and the GELU kernel, z kept for
-    the backward (the 'gelu' epilogue measured no faster: its erf arithmetic runs before the tile's stores, DESIGN.md §7).
+    the backward (a GEMM epilogue writing both z and h measured no faster: its erf arithmetic ran before the tile's
+    stores, DESIGN.md §7).
     Forward-only: the 'gelu_h' epilogue writes h alone (z is None), bit for bit the saving form's h."""
     if not save:
         return None, _gemm(k, xn, w1h, M, Dh, D, bias=b1, epi='gelu_h')
