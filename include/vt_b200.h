@@ -248,6 +248,7 @@ typedef struct {
   int32_t impl;
 } vt_attn_bwd_params;
 int vt_attn_bwd(const vt_attn_bwd_params* p, void* stream);
+/* The cls row of the probs output alone and show_attn's threshold masks: vt_attn_maps.h. */
 
 /* ---------------------------------------------------------------------------------------------
  * Patch / tubelet embedding operand: non-overlapping Conv2d k16 s16 (transformer.py:116-120,:145-147)

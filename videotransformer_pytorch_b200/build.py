@@ -27,7 +27,7 @@ def sources():
 def _digest():
     h = hashlib.sha256(ARCH.encode())
     files = sources() + sorted(os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith('.cuh'))
-    files.append(os.path.join(INCLUDE, 'vt_b200.h'))
+    files += sorted(os.path.join(INCLUDE, f) for f in os.listdir(INCLUDE) if f.endswith('.h'))
     for f in files:
         h.update(f.encode())
         with open(f, 'rb') as fh:

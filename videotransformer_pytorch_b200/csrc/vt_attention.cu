@@ -5,6 +5,7 @@
 // Used for the temporal pass of ViViT (N = 9), the probability output at N <= 256 and the other N <= 32; N > 32 runs on
 // the tensor-core kernels (vt_attention_mma.cu), N = 8 on the warp-per-problem kernel (vt_attention_small.cu).
 #include "vt_attention_mma.cuh"
+#include "../../include/vt_attn_maps.h"
 
 namespace vt {
 
@@ -22,6 +23,53 @@ __device__ __forceinline__ void load_rows_to_smem(uint32_t* dst, const __nv_bflo
     const uint4 v = *reinterpret_cast<const uint4*>(base + (long long)row * row_stride + c * 8);
     uint32_t* d = dst + row * PITCH + c * 4;
     d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
+  }
+}
+
+// Softmax probabilities of one query row (qrow: its hd / 2 words of q in global memory) against the N keys staged in
+// Ks, written by one warp to P[0, N) (shared or global memory); the row max and the sum of exponentials come back in
+// mx / l (lse = mx + log l).  The probabilities of the generic kernel are defined here once: attn_fwd_kernel's rows and
+// the cls-row kernel both call it.
+template <int HD>
+__device__ __forceinline__ void generic_probs_row(const uint32_t* qrow, const uint32_t* Ks, int N, float scale, int lane,
+                                                  float* P, float& mx, float& l) {
+  constexpr int NW = HD / 2, PITCH = NW + 1;
+  float s[MAX_N / 32];
+#pragma unroll
+  for (int jj = 0; jj < MAX_N / 32; ++jj) s[jj] = 0.f;
+#pragma unroll 4
+  for (int w = 0; w < NW; ++w) {
+    const float2 q = unpack_bf16x2(__ldg(qrow + w));
+#pragma unroll
+    for (int jj = 0; jj < MAX_N / 32; ++jj) {
+      const int j = lane + 32 * jj;
+      if (j < N) {
+        const float2 k = unpack_bf16x2(Ks[j * PITCH + w]);
+        s[jj] = fmaf(q.x, k.x, fmaf(q.y, k.y, s[jj]));
+      }
+    }
+  }
+  mx = -INFINITY;
+#pragma unroll
+  for (int jj = 0; jj < MAX_N / 32; ++jj) {
+    const int j = lane + 32 * jj;
+    s[jj] = (j < N) ? s[jj] * scale : -INFINITY;
+    mx = fmaxf(mx, s[jj]);
+  }
+  mx = warp_max(mx);
+  l = 0.f;
+#pragma unroll
+  for (int jj = 0; jj < MAX_N / 32; ++jj) {
+    const int j = lane + 32 * jj;
+    s[jj] = (j < N) ? __expf(s[jj] - mx) : 0.f;
+    l += s[jj];
+  }
+  l = warp_sum(l);
+  const float inv = 1.0f / l;
+#pragma unroll
+  for (int jj = 0; jj < MAX_N / 32; ++jj) {
+    const int j = lane + 32 * jj;
+    if (j < N) P[j] = s[jj] * inv;
   }
 }
 
@@ -45,43 +93,8 @@ attn_fwd_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict
   float* P = Ps + warp * npad;
   for (int i = warp; i < N; i += AT_WARPS) {
     const uint32_t* qrow = reinterpret_cast<const uint32_t*>(qbase + (long long)i * rs);
-    float s[MAX_N / 32];
-#pragma unroll
-    for (int jj = 0; jj < MAX_N / 32; ++jj) s[jj] = 0.f;
-#pragma unroll 4
-    for (int w = 0; w < NW; ++w) {
-      const float2 q = unpack_bf16x2(__ldg(qrow + w));
-#pragma unroll
-      for (int jj = 0; jj < MAX_N / 32; ++jj) {
-        const int j = lane + 32 * jj;
-        if (j < N) {
-          const float2 k = unpack_bf16x2(Ks[j * PITCH + w]);
-          s[jj] = fmaf(q.x, k.x, fmaf(q.y, k.y, s[jj]));
-        }
-      }
-    }
-    float mx = -INFINITY;
-#pragma unroll
-    for (int jj = 0; jj < MAX_N / 32; ++jj) {
-      const int j = lane + 32 * jj;
-      s[jj] = (j < N) ? s[jj] * scale : -INFINITY;
-      mx = fmaxf(mx, s[jj]);
-    }
-    mx = warp_max(mx);
-    float l = 0.f;
-#pragma unroll
-    for (int jj = 0; jj < MAX_N / 32; ++jj) {
-      const int j = lane + 32 * jj;
-      s[jj] = (j < N) ? __expf(s[jj] - mx) : 0.f;
-      l += s[jj];
-    }
-    l = warp_sum(l);
-    const float inv = 1.0f / l;
-#pragma unroll
-    for (int jj = 0; jj < MAX_N / 32; ++jj) {
-      const int j = lane + 32 * jj;
-      if (j < N) P[j] = s[jj] * inv;
-    }
+    float mx, l;
+    generic_probs_row<HD>(qrow, Ks, N, scale, lane, P, mx, l);
     if (lane == 0 && lse) lse[(long long)bh * N + i] = mx + __logf(l);
     __syncwarp();
     float o[WPL][2];
@@ -107,6 +120,23 @@ attn_fwd_kernel(const __nv_bfloat16* __restrict__ qkv, __nv_bfloat16* __restrict
       for (int j = lane; j < N; j += 32) pr[j] = P[j];
     }
     __syncwarp();
+  }
+}
+
+// Query row 0 (the cls token) of the generic kernel's probabilities: one CTA per (batch', head) stages K and one warp
+// writes the row straight to out[bh, 0, N).
+template <int HD>
+__global__ void __launch_bounds__(AT_THREADS)
+attn_cls_probs_kernel(const __nv_bfloat16* __restrict__ qkv, float* __restrict__ out, int N, int H, float scale) {
+  extern __shared__ uint32_t sm[];
+  const int bh = blockIdx.x, bp = bh / H, h = bh - bp * H;
+  const long long rs = 3LL * H * HD;
+  const __nv_bfloat16* qbase = qkv + (long long)bp * N * rs + h * HD;
+  load_rows_to_smem<HD>(sm, qbase + (long long)H * HD, rs, N);
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    float mx, l;
+    generic_probs_row<HD>(reinterpret_cast<const uint32_t*>(qbase), sm, N, scale, threadIdx.x, out + (long long)bh * N, mx, l);
   }
 }
 
@@ -267,6 +297,7 @@ attn_bwd_kernel(const __nv_bfloat16* __restrict__ qkv, const __nv_bfloat16* __re
 int attn8_fwd_launch(const vt_attn_fwd_params* p, cudaStream_t st);
 int attn8_bwd_launch(const vt_attn_bwd_params* p, cudaStream_t st);
 int attn_probs_launch(const void* qkv, float* probs, int Bp, int N, int H, int hd, float scale, cudaStream_t st);
+int attn_cls_probs_tiled_launch(const vt_attn_cls_probs_params* p, cudaStream_t st);
 
 // past the generic kernel's N the tensor-core kernels take every call, probabilities included (the 64-row tiles: the
 // whole-problem kernels stop at N = 256)
@@ -336,6 +367,16 @@ static int generic_bwd(const vt_attn_bwd_params* p, cudaStream_t st) {
   return check_launch("attn_bwd_kernel");
 }
 
+template <int HD>
+static int generic_cls_probs(const vt_attn_cls_probs_params* p, cudaStream_t st) {
+  const int smem = p->N * (HD / 2 + 1) * 4;
+  static int max_set = 0;
+  if (raise_smem(attn_cls_probs_kernel<HD>, smem, 100 * 1024, max_set, "vt_attn_cls_probs")) return 1;
+  attn_cls_probs_kernel<HD><<<p->Bp * p->H, AT_THREADS, smem, st>>>(static_cast<const __nv_bfloat16*>(p->qkv), p->probs,
+                                                                   p->N, p->H, p->scale);
+  return check_launch("attn_cls_probs_kernel");
+}
+
 }  // namespace vt
 
 using namespace vt;
@@ -392,4 +433,18 @@ extern "C" int vt_attn_bwd(const vt_attn_bwd_params* p, void* stream) {
   }
   VT_REQUIRE(p->N <= MAX_N, "vt_attn_bwd: N=%d unsupported by the generic kernel (1..%d)", p->N, MAX_N);
   return with_head_dim(p->hd, [&](auto hd) { return generic_bwd<hd.value>(p, st); });
+}
+
+// Row 0 of vt_attn_fwd's probs output from the same device code as the route vt_attn_fwd takes at this N: the generic
+// kernel's row function up to MAX_N, the row-tile softmax kernel's score and softmax functions (vt_head.cu) past it.
+extern "C" int vt_attn_cls_probs(const vt_attn_cls_probs_params* p, void* stream) {
+  VT_REQUIRE(p && p->qkv && p->probs, "vt_attn_cls_probs: null pointer");
+  VT_REQUIRE(attn_head_dim_ok(p->hd), "vt_attn_cls_probs: head dim %d unsupported (32, 64, 96 or 128)", p->hd);
+  VT_REQUIRE(p->N >= 1, "vt_attn_cls_probs: N=%d unsupported", p->N);
+  VT_REQUIRE(p->Bp > 0 && p->H > 0 && (long long)p->Bp * p->H <= 0x7fffffffLL, "vt_attn_cls_probs: bad Bp=%d / H=%d",
+             p->Bp, p->H);
+  VT_REQUIRE(((uintptr_t)p->qkv & 15) == 0, "vt_attn_cls_probs: qkv must be 16-byte aligned");
+  const cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (p->N > MAX_N) return attn_cls_probs_tiled_launch(p, st);
+  return with_head_dim(p->hd, [&](auto hd) { return generic_cls_probs<hd.value>(p, st); });
 }

@@ -2,11 +2,12 @@
 //   * skinny linear layer (classification head: 8 x 768 -> 400) forward / backward — warp-per-output GEMV, fp32 throughout
 //   * softmax cross-entropy (hard labels or soft targets) forward + gradient in one launch
 //   * attention probabilities softmax(q k^T * scale) for long sequences (vt_attn_fwd's probs output past 256 tokens:
-//     get_last_selfattention of the joint variants)
+//     get_last_selfattention of the joint variants), and their cls row alone (vt_attn_cls_probs past 256 tokens)
 //   * uint8 clip -> normalised bf16 patch operand with Mixup / CutMix of the flipped batch folded in
 //   * top-k hit counters of an evaluation step (view mean, optional softmax, rank of the label)
 // All are latency / bandwidth bound warp-primitive kernels (no tensor cores: M <= 64 rows or one-off visualisation work).
 #include "vt_common.cuh"
+#include "../../include/vt_attn_maps.h"
 
 namespace vt {
 
@@ -178,14 +179,55 @@ __global__ void scale_by_scalar_kernel(const float* __restrict__ in, const float
 // CTA = PR_ROWS query rows of one (batch', head): raw scores of those rows live in shared memory (rows x N fp32),
 // keys stream through in tiles of 64 (pitch HD + 1 floats: lane = key reads are conflict free); then a row softmax in
 // place and coalesced fp32 stores.
+// The arithmetic of these probabilities lives in the four functions below, shared with the cls-row kernel: q scaled on
+// load, one fmaf per feature in feature order, and a one-warp softmax (max, then exp and sum in lane-strided order,
+// then one reciprocal).
 // ------------------------------------------------------------------------------------------------
 constexpr int PR_ROWS = 8;
 constexpr int PR_KT = 64;
+constexpr int CLS_KT = 256;    // keys per tile of the cls-row kernel: one per thread
+
+__device__ __forceinline__ float probs_q(__nv_bfloat16 q, float scale) { return __bfloat162float(q) * scale; }
+
+// keys j0 .. j0 + KT - 1 of one head (kbase: key 0's k slice, rows rs elements apart) -> Kt[KT][HD + 1] fp32, zeros past N
+template <int HD, int KT>
+__device__ __forceinline__ void probs_load_keys(float* Kt, const __nv_bfloat16* kbase, long long rs, int N, int j0) {
+  constexpr int KP = HD + 1, CPR = HD / 8;          // key pitch (floats), 16-byte chunks per row
+  for (int idx = threadIdx.x; idx < KT * CPR; idx += 256) {       // KT keys x HD / 8 vectors of 8 bf16
+    const int j = div_pos<CPR>(idx), c = mod_pos<CPR>(idx);
+    uint4 v = make_uint4(0u, 0u, 0u, 0u);
+    if (j0 + j < N) v = *reinterpret_cast<const uint4*>(kbase + (long long)(j0 + j) * rs + c * 8);
+    float* d = Kt + j * KP + c * 8;
+    const float2 a = unpack_bf16x2(v.x), b2 = unpack_bf16x2(v.y), c2 = unpack_bf16x2(v.z), e2 = unpack_bf16x2(v.w);
+    d[0] = a.x; d[1] = a.y; d[2] = b2.x; d[3] = b2.y; d[4] = c2.x; d[5] = c2.y; d[6] = e2.x; d[7] = e2.y;
+  }
+}
+
+// raw score of scaled query q[HD] and key k[HD]
+template <int HD>
+__device__ __forceinline__ float probs_dot(const float* q, const float* k) {
+  float s = 0.f;
+#pragma unroll 16
+  for (int d = 0; d < HD; ++d) s = fmaf(q[d], k[d], s);
+  return s;
+}
+
+// one warp: out[0, N) = softmax of the raw scores row[0, N) (row is overwritten with the exponentials)
+__device__ __forceinline__ void probs_softmax_row(float* row, int N, int lane, float* out) {
+  float mx = -INFINITY;
+  for (int j = lane; j < N; j += 32) mx = fmaxf(mx, row[j]);
+  mx = warp_max(mx);
+  float se = 0.f;
+  for (int j = lane; j < N; j += 32) { const float e = expf(row[j] - mx); row[j] = e; se += e; }
+  se = warp_sum(se);
+  const float inv = 1.0f / se;
+  for (int j = lane; j < N; j += 32) out[j] = row[j] * inv;
+}
 
 template <int HD>
 __global__ void __launch_bounds__(256)
 attn_probs_kernel(const __nv_bfloat16* __restrict__ qkv, float* __restrict__ probs, int N, int H, float scale) {
-  constexpr int KP = HD + 1, CPR = HD / 8;          // key pitch (floats), 16-byte chunks per row
+  constexpr int KP = HD + 1;
   extern __shared__ float psm[];
   float* S = psm;                                   // [PR_ROWS][N]
   float* Q = S + (size_t)PR_ROWS * N;               // [PR_ROWS][HD]
@@ -196,45 +238,48 @@ attn_probs_kernel(const __nv_bfloat16* __restrict__ qkv, float* __restrict__ pro
   const __nv_bfloat16* base = qkv + (long long)bp * N * rs + h * HD;
   for (int idx = threadIdx.x; idx < PR_ROWS * HD; idx += 256) {
     const int r = div_pos<HD>(idx), d = mod_pos<HD>(idx);
-    Q[idx] = (i0 + r < N) ? __bfloat162float(base[(long long)(i0 + r) * rs + d]) * scale : 0.f;
+    Q[idx] = (i0 + r < N) ? probs_q(base[(long long)(i0 + r) * rs + d], scale) : 0.f;
   }
   for (int j0 = 0; j0 < N; j0 += PR_KT) {
     __syncthreads();
-    for (int idx = threadIdx.x; idx < PR_KT * CPR; idx += 256) {       // 64 keys x HD / 8 vectors of 8 bf16
-      const int j = div_pos<CPR>(idx), c = mod_pos<CPR>(idx);
-      uint4 v = make_uint4(0u, 0u, 0u, 0u);
-      if (j0 + j < N) v = *reinterpret_cast<const uint4*>(base + (long long)(j0 + j) * rs + (long long)H * HD + c * 8);
-      float* d = Kt + j * KP + c * 8;
-      const float2 a = unpack_bf16x2(v.x), b2 = unpack_bf16x2(v.y), c2 = unpack_bf16x2(v.z), e2 = unpack_bf16x2(v.w);
-      d[0] = a.x; d[1] = a.y; d[2] = b2.x; d[3] = b2.y; d[4] = c2.x; d[5] = c2.y; d[6] = e2.x; d[7] = e2.y;
-    }
+    probs_load_keys<HD, PR_KT>(Kt, base + (long long)H * HD, rs, N, j0);
     __syncthreads();
     // 256 threads = 8 rows x 32 lanes; lane handles keys lane and lane + 32 of the tile
     const int r = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    float s0 = 0.f, s1 = 0.f;
-#pragma unroll 16
-    for (int d = 0; d < HD; ++d) {
-      const float q = Q[r * HD + d];
-      s0 = fmaf(q, Kt[lane * KP + d], s0);
-      s1 = fmaf(q, Kt[(lane + 32) * KP + d], s1);
-    }
+    const float s0 = probs_dot<HD>(Q + r * HD, Kt + lane * KP);
+    const float s1 = probs_dot<HD>(Q + r * HD, Kt + (lane + 32) * KP);
     if (j0 + lane < N) S[(size_t)r * N + j0 + lane] = s0;
     if (j0 + lane + 32 < N) S[(size_t)r * N + j0 + lane + 32] = s1;
   }
   __syncthreads();
   const int r = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (i0 + r < N) {
-    float* row = S + (size_t)r * N;
-    float mx = -INFINITY;
-    for (int j = lane; j < N; j += 32) mx = fmaxf(mx, row[j]);
-    mx = warp_max(mx);
-    float se = 0.f;
-    for (int j = lane; j < N; j += 32) { const float e = expf(row[j] - mx); row[j] = e; se += e; }
-    se = warp_sum(se);
-    const float inv = 1.0f / se;
-    float* out = probs + ((long long)bh * N + (i0 + r)) * N;
-    for (int j = lane; j < N; j += 32) out[j] = row[j] * inv;
+  if (i0 + r < N) probs_softmax_row(S + (size_t)r * N, N, lane, probs + ((long long)bh * N + (i0 + r)) * N);
+}
+
+// Query row 0 (the cls token) of attn_probs_kernel's probabilities, at any N whose score row fits in shared memory: one
+// CTA per (batch', head), keys in tiles of CLS_KT (thread t scores key j0 + t), then warp 0 runs the row softmax into
+// out[bh, 0, N).
+template <int HD>
+__global__ void __launch_bounds__(256)
+attn_cls_probs_tiled_kernel(const __nv_bfloat16* __restrict__ qkv, float* __restrict__ out, int N, int H, float scale) {
+  constexpr int KP = HD + 1;
+  extern __shared__ float psm[];
+  float* S = psm;                                   // [N]
+  float* Q = S + N;                                 // [HD]
+  float* Kt = Q + HD;                               // [CLS_KT keys][HD + 1]
+  const int bh = blockIdx.x, bp = bh / H, h = bh - bp * H;
+  const long long rs = 3LL * H * HD;
+  const __nv_bfloat16* base = qkv + (long long)bp * N * rs + h * HD;
+  for (int d = threadIdx.x; d < HD; d += 256) Q[d] = probs_q(base[d], scale);
+  for (int j0 = 0; j0 < N; j0 += CLS_KT) {
+    __syncthreads();
+    probs_load_keys<HD, CLS_KT>(Kt, base + (long long)H * HD, rs, N, j0);
+    __syncthreads();
+    const float s = probs_dot<HD>(Q, Kt + threadIdx.x * KP);
+    if (j0 + (int)threadIdx.x < N) S[j0 + threadIdx.x] = s;
   }
+  __syncthreads();
+  if (threadIdx.x < 32) probs_softmax_row(S, N, threadIdx.x, out + (long long)bh * N);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -308,6 +353,28 @@ static int attn_probs_launch_hd(const void* qkv, float* probs, int Bp, int N, in
 // (checked by vt_attn_fwd)
 int attn_probs_launch(const void* qkv, float* probs, int Bp, int N, int H, int hd, float scale, cudaStream_t st) {
   return with_head_dim(hd, [&](auto d) { return attn_probs_launch_hd<d.value>(qkv, probs, Bp, N, H, scale, st); });
+}
+
+template <int HD>
+static int attn_cls_probs_tiled_hd(const vt_attn_cls_probs_params* p, cudaStream_t st) {
+  constexpr size_t limit = 227 * 1024;   // the largest dynamic shared memory a CTA may opt into on sm_90
+  const size_t smem = ((size_t)p->N + HD + CLS_KT * (HD + 1)) * sizeof(float);
+  VT_REQUIRE(smem <= limit, "vt_attn_cls_probs: N=%d at head dim %d needs %zu bytes of shared memory (%zu at most)", p->N,
+             HD, smem, limit);
+  static size_t max_set = 48 * 1024;
+  if (smem > max_set) {
+    cudaError_t e = cudaFuncSetAttribute(attn_cls_probs_tiled_kernel<HD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)limit);
+    VT_REQUIRE(e == cudaSuccess, "vt_attn_cls_probs: smem attribute: %s", cudaGetErrorString(e));
+    max_set = limit;
+  }
+  attn_cls_probs_tiled_kernel<HD><<<p->Bp * p->H, 256, smem, st>>>(static_cast<const __nv_bfloat16*>(p->qkv), p->probs, p->N,
+                                                                    p->H, p->scale);
+  return check_launch("attn_cls_probs_tiled_kernel");
+}
+
+// vt_attn_cls_probs past the generic kernel's N (vt_attention.cu checks the parameters)
+int attn_cls_probs_tiled_launch(const vt_attn_cls_probs_params* p, cudaStream_t st) {
+  return with_head_dim(p->hd, [&](auto d) { return attn_cls_probs_tiled_hd<d.value>(p, st); });
 }
 
 static int grid_1d(long long n, int threads) {

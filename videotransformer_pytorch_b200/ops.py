@@ -12,6 +12,7 @@ C-ABI kernel launches (see _lib.K):
   PosResizeFn     <- the bicubic resize of TimeSformer.interpolate_pos_encoding (video_transformer.py:171-191)
   ClsNormFn       <- final nn.LayerNorm(eps=1e-6) + cls select     (video_transformer.py:251-254)
   AttentionCoreFn <- Attention.forward (stand-alone use)            (transformer.py:165-177)
+  attention_probs <- its probabilities alone, forward-only (get_last_selfattention, visualize_attention.py:71)
 
 Forward-only calls: when autograd will not record a call (grad mode off, or no input or parameter requires grad), `run`
 executes the same forward body with ctx=None instead of Function.apply.  The launch sequence is the same, in the forms
@@ -34,11 +35,16 @@ import functools
 
 import torch
 
-from . import _lib
+from . import _lib, attn_maps_lib
 
 
 def K():
     return _lib.K
+
+
+def maps_K():
+    """the attention-map kernel table (attn_maps_lib.K: vt_attn_cls_probs, vt_attn_mass_mask)"""
+    return attn_maps_lib.K
 
 
 _MASK_ARENA = None
@@ -638,6 +644,21 @@ class AttentionCoreFn(torch.autograd.Function):
         d_qkv_b = k.colsum(dqkv)
         dx = _dgrad(dqkv, qkv_wh, M, C, 3 * C, epi='f32').view(Bp, N, C)
         return dx, d_qkv_w, d_qkv_b, d_proj_w, d_proj_b, None, None, None, None
+
+
+def attention_probs(x, qkv_b, qkv_wh, H, cls_only=False):
+    """Forward-only probabilities of Attention.forward on x [Bp, N, C]: softmax(q k^T * scale) fp32 [Bp, H, N, N], or with
+    cls_only its query row 0, [Bp, H, N], without the full map.  The cast and the qkv GEMM are AttentionCoreFn's, so the
+    result is bit for bit its probs output (row 0 of it); no context, projection or saved tensors."""
+    k = K()
+    Bp, N, C = x.shape
+    M = Bp * N
+    hd = C // H
+    xh = k.gather_cast(x.reshape(M, C).float().contiguous())
+    qkv = k.gemm(xh, qkv_wh, M, 3 * C, C, bias=qkv_b, epi='bf16')
+    if cls_only:
+        return maps_K().attn_cls_probs(qkv, Bp, N, H, hd, hd ** -0.5)
+    return k.attn_fwd(qkv, Bp, N, H, hd, hd ** -0.5, want_probs=True, want_lse=False)[2]
 
 
 # --------------------------------------------------------------------------------------------------

@@ -263,6 +263,14 @@ class Attention(nn.Module):
             return _f32(self.qkv.bias)
         return torch.zeros(self.qkv.weight.shape[0], device=self.qkv.weight.device)
 
+    def attention_probs(self, x, cls_only=False):
+        """forward(x)[1], the fp32 [Bp, H, N, N] probabilities, or with cls_only its query row 0 [Bp, H, N].  When autograd
+        would record the call the full map comes from forward() itself; otherwise, and always for cls_only, from the
+        forward-only ops.attention_probs (same cast, qkv GEMM and probability code: the same bits)."""
+        if not cls_only and not ops._forward_only([x, *self.parameters()]):
+            return self(x)[1]
+        return ops.attention_probs(x, self.qkv_bias_or_zeros(), self.shadows()[0], self.num_heads, cls_only)
+
     def forward(self, x, need_weights=True):
         qh, ph = self.shadows()
         out, attn = ops.AttentionCoreFn.apply(x, _f32(self.qkv.weight), self.qkv_bias_or_zeros(), _f32(self.proj.weight),
@@ -329,7 +337,7 @@ class DividedTemporalAttentionWithPreNorm(_DividedBase):
         if return_attention:
             maps = ops.token_maps(B, T, P, str(x.device))
             xn = ops.run(ops.RowsNormFn, x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, maps['temporal'])
-            return self.attn(xn.view(B * P, T, D))[1]
+            return self.attn.attention_probs(xn.view(B * P, T, D), return_attention == 'cls')
         dp = _dp_scale(self.layer_drop, B * P, T, x.device)
         if ops.fp8_form(self, x):
             qh, ph, fh = self._e4m3_shadows(D)
@@ -366,7 +374,7 @@ class DividedSpatialAttentionWithPreNorm(_DividedBase):
         if return_attention:
             maps = ops.token_maps(B, T, P, str(x.device))
             xn = ops.run(ops.RowsNormFn, x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, maps['sp_in'])
-            return self.attn(xn.view(B * T, P + 1, D))[1]
+            return self.attn.attention_probs(xn.view(B * T, P + 1, D), return_attention == 'cls')
         dp = _dp_scale(self.layer_drop, B * T, P + 1, x.device)
         qh, ph = self.attn.e4m3_shadows() if ops.fp8_form(self, x) else self.attn.shadows()
         return ops.run(
@@ -398,7 +406,7 @@ class MultiheadAttentionWithPreNorm(nn.Module):
         Bp, N, D = x.shape
         if return_attention:
             xn = ops.run(ops.RowsNormFn, x, _f32(self.norm.weight), _f32(self.norm.bias), self.norm.eps, None)
-            return self.attn(xn.view(Bp, N, D))[1]
+            return self.attn.attention_probs(xn.view(Bp, N, D), return_attention == 'cls')
         dp = _dp_scale(self.layer_drop, Bp, N, x.device)
         qh, ph = self.attn.e4m3_shadows() if ops.fp8_form(self, x) else self.attn.shadows()
         return ops.run(
@@ -456,7 +464,7 @@ class TransformerContainer(nn.Module):
     def forward(self, x, return_attention=False):
         last = self.num_transformer_layers - 1
         for idx, layer in enumerate(self.layers):
-            x = layer(x, return_attention=True) if (idx >= last and return_attention) else layer(x)
+            x = layer(x, return_attention=return_attention) if (idx >= last and return_attention) else layer(x)
         return x
 
 
@@ -493,7 +501,7 @@ class BasicTransformerBlock(nn.Module):
         n_attn = len(self.attentions)
         for idx, layer in enumerate(self.attentions):
             if idx >= n_attn - 1 and return_attention:
-                return layer(x, return_attention=True)
+                return layer(x, return_attention=return_attention)
             x = layer(x)
         for layer in self.ffns:
             x = layer(x)

@@ -81,7 +81,60 @@ class _ByteClipInput:
         return x, norm, plan
 
 
-class TimeSformer(_ByteClipInput, InferencePrecision, nn.Module):
+class _AttentionMaps:
+    """The cls query's attention in the last attention layer, the product visualize_attention.py consumes
+    (attentions[:, 0, 1:], :71, turned into heatmaps and threshold masks by show_attn, :66-102).  The model supplies
+    _last_attention(x, return_attention) and _map_layout()."""
+
+    def cls_attention(self, x):
+        """get_last_selfattention(x)[:, :, 0, :], bit for bit: fp32 [B', H, N], without the [B', H, N, N] map.  Always the
+        forward-only form: every block before the last runs as under no_grad (nothing saved), and the last runs only its
+        LayerNorm, the qkv GEMM and vt_attn_cls_probs, where the reference's return_attention stops as well."""
+        with torch.no_grad():
+            return self._last_attention(x, 'cls')
+
+    def attention_maps(self, x, threshold=0.6):
+        """(heatmaps, masks) of the cls query over the patch tokens, per head, from cls_attention(x).
+
+        Spatial maps use show_attn's own axis order: reshape(nh, w_featmap, h_featmap) with w_featmap = H // p and
+        h_featmap = W // p for a clip of H x W pixels, kept as is.  Per-frame attention (divided_space_time, space_only)
+        gives one map per frame, [B * T, nh, w_featmap, h_featmap] (frames in get_last_selfattention's order); joint
+        attention (joint_space_time, token 1 + p * T + t) gives [B, nh, T, w_featmap, h_featmap] per clip.  ViViT's
+        fact_encoder ends in the temporal encoder, whose 1 + T tokens are the cls and one token per frame: its result is
+        the per-frame weight row [B, nh, T], not a spatial map.
+
+        masks (None when threshold is None) has the heatmaps' shape: show_attn's float 0 / 1 mask keeping the largest
+        probabilities of each (frame or clip, head) row until their mass exceeds threshold (vt_attn_mass_mask; a joint
+        clip's row covers all its T * P patches).  Upsampling by the patch size is left to the caller
+        (repeat_interleave on the last two axes is show_attn's nearest interpolation)."""
+        cls = self.cls_attention(x)
+        pat = cls[:, :, 1:]
+        nh = pat.shape[1]
+        kind, grid = self._map_layout(x)
+        with torch.no_grad():
+            masks = None if threshold is None else ops.maps_K().attn_mass_mask(pat, threshold)
+            out = []
+            for t in (pat, masks):
+                if t is None:
+                    out.append(None)
+                elif kind == 'frame':
+                    out.append(t.reshape(t.shape[0], nh, *grid))
+                elif kind == 'clip':
+                    T = t.shape[-1] // (grid[0] * grid[1])
+                    out.append(t.reshape(t.shape[0], nh, grid[0] * grid[1], T).transpose(2, 3).reshape(t.shape[0], nh, T, *grid))
+                else:
+                    out.append(t.contiguous())
+        return out[0], out[1]
+
+    def _featmap(self, x):
+        """(w_featmap, h_featmap) of show_attn: (H // p, W // p) of the clip"""
+        clip = x.clip if isinstance(x, MixedClip) else x
+        h, w = (clip.shape[2], clip.shape[3]) if clip.dtype == torch.uint8 else (clip.shape[3], clip.shape[4])
+        p = self.patch_embed.patch_size
+        return h // p[0], w // p[1]
+
+
+class TimeSformer(_AttentionMaps, _ByteClipInput, InferencePrecision, nn.Module):
     """TimeSformer (divided space-time attention).  forward(x[B,T,3,H,W]) -> [B, embed_dims]."""
 
     supported_attention_types = ['divided_space_time', 'space_only', 'joint_space_time']
@@ -210,8 +263,17 @@ class TimeSformer(_ByteClipInput, InferencePrecision, nn.Module):
         return y.view(b, S, -1)[:, 1:].mean(1)
 
     def get_last_selfattention(self, x):
+        """fp32 [B', H, N, N] probabilities of the last attention layer.  Without autograd recording (no_grad /
+        inference_mode, or nothing requiring grad) the blocks take their forward-only form and the last layer stops
+        after its probabilities; the result is the same either way."""
+        return self._last_attention(x, True)
+
+    def _last_attention(self, x, return_attention):
         x, b = self.prepare_tokens(x)
-        return self.transformer_layers(x, return_attention=True)
+        return self.transformer_layers(x, return_attention=return_attention)
+
+    def _map_layout(self, x):
+        return ('clip' if self.attention_type == 'joint_space_time' else 'frame'), self._featmap(x)
 
 
 def get_vit_base_patch16_224(**kwargs):
@@ -223,7 +285,7 @@ def get_vit_base_patch16_224(**kwargs):
                        return_cls_token=True)
 
 
-class ViViT(_ByteClipInput, InferencePrecision, nn.Module):
+class ViViT(_AttentionMaps, _ByteClipInput, InferencePrecision, nn.Module):
     """ViViT factorised encoder (model 2): tubelet embed -> 12 spatial layers per frame ->
     frame tokens (+ the reference's `x[:b,0,:]` cls gather) -> 4 temporal layers."""
 
@@ -341,10 +403,19 @@ class ViViT(_ByteClipInput, InferencePrecision, nn.Module):
         return y.view(x.shape)[:, 1:].mean(1)
 
     def get_last_selfattention(self, x):
+        """fp32 [B', H, N, N] probabilities of the last attention layer (fact_encoder: the temporal encoder's); forward-only
+        without autograd recording, as TimeSformer.get_last_selfattention."""
+        return self._last_attention(x, True)
+
+    def _last_attention(self, x, return_attention):
         x, cls_tokens, b = self.prepare_tokens(x)
         if self.attention_type != 'fact_encoder':
-            return self.transformer_layers(x, return_attention=True)
+            return self.transformer_layers(x, return_attention=return_attention)
         spatial, temporal = self.transformer_layers
         x = spatial(x)
         x = self._temporal_tokens(x, b)
-        return temporal(x, return_attention=True)
+        return temporal(x, return_attention=return_attention)
+
+    def _map_layout(self, x):
+        kind = {'fact_encoder': 'row', 'joint_space_time': 'clip'}.get(self.attention_type, 'frame')
+        return kind, self._featmap(x)
