@@ -426,7 +426,16 @@ int vt_mse_bwd(const vt_mse_bwd_params* p, void* stream);
  *   vt_opt_adamw : p *= 1 - lr*wd;  m = b1 m + (1-b1) g;  v = b2 v + (1-b2) g^2;
  *                  p -= lr/bc1 * m / (sqrt(v)/sqrt(bc2) + eps)         (torch.optim.AdamW; bc_k = 1 - beta_k^step)
  * Gradients are read, never written back (the reference scales p.grad in place; nothing reads it afterwards).
+ * hyper (optional): a device block of VT_OPT_HYPER_SIZE floats {clip, bc1, bc2, first_step (0 / 1), spare}.  When it is
+ * given, vt_opt_sgd / vt_opt_adamw read those per-step scalars from it at run time and ignore the fields of the same
+ * names (norm2 must then be given, and is read only where the block's clip is > 0), so a CUDA graph that recorded the
+ * launch follows the values the host writes into the block between replays.  NULL: the fields are used, as always.
  * ============================================================================================= */
+#define VT_OPT_HYPER_CLIP 0
+#define VT_OPT_HYPER_BC1 1
+#define VT_OPT_HYPER_BC2 2
+#define VT_OPT_HYPER_FIRST_STEP 3
+#define VT_OPT_HYPER_SIZE 5
 typedef struct {
   const void* chunks; int32_t n_chunks; int32_t n_tensors;
   const int64_t* pptr; const int64_t* gptr; const int64_t* s1ptr; const int64_t* s2ptr;
@@ -434,6 +443,7 @@ typedef struct {
   float clip, momentum, beta1, beta2, eps, bc1, bc2;
   int32_t nesterov, first_step;
   float* partials;          /* vt_opt_norm2 workspace: n_chunks floats */
+  const float* hyper;       /* optional per-step scalars on the device, see above */
 } vt_opt_params;
 int vt_opt_norm2(const vt_opt_params* p, void* stream);
 int vt_opt_sgd(const vt_opt_params* p, void* stream);

@@ -225,7 +225,12 @@ class OptParams(C.Structure):
                 ('pptr', c_vp), ('gptr', c_vp), ('s1ptr', c_vp), ('s2ptr', c_vp),
                 ('norm2', c_vp), ('lr', c_vp), ('wd', c_vp),
                 ('clip', c_f32), ('momentum', c_f32), ('beta1', c_f32), ('beta2', c_f32), ('eps', c_f32), ('bc1', c_f32),
-                ('bc2', c_f32), ('nesterov', c_i32), ('first_step', c_i32), ('partials', c_vp)]
+                ('bc2', c_f32), ('nesterov', c_i32), ('first_step', c_i32), ('partials', c_vp), ('hyper', c_vp)]
+
+
+# vt_opt_params.hyper: slots of the per-step scalar block (VT_OPT_HYPER_* in the header)
+OPT_HYPER = {'clip': 0, 'bc1': 1, 'bc2': 2, 'first_step': 3}
+OPT_HYPER_SIZE = 5
 
 
 class LinearSmallParams(C.Structure):
@@ -1241,6 +1246,9 @@ class CudaKernels:
     # -- fused clip + optimizer (multi-tensor) ---------------------------------------------------
     def _opt_params(self, tbl, clip=0.0, **hp):
         p = OptParams()
+        # optional tbl['hyper']: fp32 device block of OPT_HYPER_SIZE per-step scalars that the update kernels read in
+        # place of clip / first_step / bc1 / bc2 (the table of a captured step: optim's prepare_capture)
+        p.hyper = _ptr(tbl.get('hyper'))
         p.chunks, p.n_chunks, p.n_tensors = tbl['chunks'].data_ptr(), tbl['n_chunks'], tbl['n_tensors']
         p.pptr, p.gptr = tbl['pptr'].data_ptr(), tbl['gptr'].data_ptr()
         p.s1ptr, p.s2ptr = tbl['s1ptr'].data_ptr(), _ptr(tbl.get('s2ptr'))

@@ -8,6 +8,9 @@
 //   2. fused update: per element g = grad * min(1, clip / (norm + 1e-6)), then the SGD-nesterov or AdamW step.
 // Tensors are addressed through device arrays of pointers (multi-tensor apply), so parameters, gradients (per-tensor
 // .grad or views of the DDP flat buckets) and optimizer state stay wherever PyTorch put them.
+// The per-step scalars (clip, bias corrections, first-step flag) are kernel arguments, or, when `hyper` is given, read
+// from that device block: a CUDA graph that recorded the update then takes each step's values from the block, which the
+// host rewrites between replays.  The host computes the values in both forms, so both give the same bits.
 #include <math.h>
 
 #include "vt_common.cuh"
@@ -72,14 +75,15 @@ struct OptArgs {
   const float* norm2;       // NULL => no clipping
   const float* lr;          // per tensor
   const float* wd;          // per tensor
+  const float* hyper;       // NULL, or the device block {clip, bc1, bc2, first_step, spare} replacing the scalars below
   float clip;
   float momentum, beta1, beta2, eps, bc1, bc2;
   int nesterov, first_step;
 };
 
-__device__ __forceinline__ float clip_coef(const OptArgs& a, int t) {
-  if (a.norm2 == nullptr || a.clip <= 0.f) return 1.0f;
-  const float c = a.clip / (sqrtf(a.norm2[t]) + 1e-6f);
+__device__ __forceinline__ float clip_coef(const OptArgs& a, float clip, int t) {
+  if (a.norm2 == nullptr || clip <= 0.f) return 1.0f;
+  const float c = clip / (sqrtf(a.norm2[t]) + 1e-6f);
   return c < 1.0f ? c : 1.0f;
 }
 
@@ -88,11 +92,13 @@ __global__ void __launch_bounds__(OPT_THREADS) fused_sgd_kernel(const OptArgs a)
   float* p = reinterpret_cast<float*>(a.pptr[c.tensor]) + c.offset;
   const float* g = reinterpret_cast<const float*>(a.gptr[c.tensor]) + c.offset;
   float* buf = reinterpret_cast<float*>(a.s1ptr[c.tensor]) + c.offset;
-  const float coef = clip_coef(a, c.tensor), lr = a.lr[c.tensor], wd = a.wd[c.tensor];
+  const float clip = a.hyper ? a.hyper[VT_OPT_HYPER_CLIP] : a.clip;
+  const bool first_step = a.hyper ? a.hyper[VT_OPT_HYPER_FIRST_STEP] != 0.f : a.first_step != 0;
+  const float coef = clip_coef(a, clip, c.tensor), lr = a.lr[c.tensor], wd = a.wd[c.tensor];
   for (int i = threadIdx.x; i < c.len; i += OPT_THREADS) {
     const float w = p[i];
     float d = fmaf(wd, w, g[i] * coef);
-    const float b = a.first_step ? d : fmaf(a.momentum, buf[i], d);
+    const float b = first_step ? d : fmaf(a.momentum, buf[i], d);
     buf[i] = b;
     d = a.nesterov ? fmaf(a.momentum, b, d) : b;
     p[i] = fmaf(-lr, d, w);
@@ -105,8 +111,10 @@ __global__ void __launch_bounds__(OPT_THREADS) fused_adamw_kernel(const OptArgs 
   const float* g = reinterpret_cast<const float*>(a.gptr[c.tensor]) + c.offset;
   float* m = reinterpret_cast<float*>(a.s1ptr[c.tensor]) + c.offset;
   float* v = reinterpret_cast<float*>(a.s2ptr[c.tensor]) + c.offset;
-  const float coef = clip_coef(a, c.tensor), lr = a.lr[c.tensor], wd = a.wd[c.tensor];
-  const float step_size = lr / a.bc1, inv_sqrt_bc2 = rsqrtf(a.bc2);
+  const float clip = a.hyper ? a.hyper[VT_OPT_HYPER_CLIP] : a.clip;
+  const float bc1 = a.hyper ? a.hyper[VT_OPT_HYPER_BC1] : a.bc1, bc2 = a.hyper ? a.hyper[VT_OPT_HYPER_BC2] : a.bc2;
+  const float coef = clip_coef(a, clip, c.tensor), lr = a.lr[c.tensor], wd = a.wd[c.tensor];
+  const float step_size = lr / bc1, inv_sqrt_bc2 = rsqrtf(bc2);
   for (int i = threadIdx.x; i < c.len; i += OPT_THREADS) {
     const float gi = g[i] * coef;
     const float w = p[i] * (1.0f - lr * wd);
@@ -144,9 +152,12 @@ static int opt_args(const vt_opt_params* p, OptArgs* a, const char* who, bool ne
   a->gptr = reinterpret_cast<const long long*>(p->gptr);
   a->s1ptr = reinterpret_cast<const long long*>(p->s1ptr);
   a->s2ptr = reinterpret_cast<const long long*>(p->s2ptr);
-  a->norm2 = p->clip > 0.f ? p->norm2 : nullptr;
+  // with `hyper` the clip value is only known on the device: the kernels test it there
+  VT_REQUIRE(!p->hyper || p->norm2, "%s: the hyper block needs the norm2 array", who);
+  a->norm2 = (p->hyper || p->clip > 0.f) ? p->norm2 : nullptr;
   a->lr = p->lr;
   a->wd = p->wd;
+  a->hyper = p->hyper;
   a->clip = p->clip;
   a->momentum = p->momentum; a->beta1 = p->beta1; a->beta2 = p->beta2; a->eps = p->eps; a->bc1 = p->bc1; a->bc2 = p->bc2;
   a->nesterov = p->nesterov;
@@ -166,7 +177,7 @@ extern "C" int vt_opt_adamw(const vt_opt_params* p, void* stream) {
   OptArgs a;
   int rc = opt_args(p, &a, "vt_opt_adamw", true);
   if (rc) return rc;
-  VT_REQUIRE(p->bc1 > 0.f && p->bc2 > 0.f, "vt_opt_adamw: bias corrections must be positive");
+  VT_REQUIRE(p->hyper || (p->bc1 > 0.f && p->bc2 > 0.f), "vt_opt_adamw: bias corrections must be positive");
   fused_adamw_kernel<<<p->n_chunks, OPT_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(a);
   return check_launch("fused_adamw_kernel");
 }

@@ -11,6 +11,9 @@ it with a single launch; per replay the host only
 bf16 weight shadows are re-cast from the fp32 parameters *inside* the graph, so optimizer updates between
 replays are picked up.  Gradients land in static `.grad` tensors (or in the `GradientBuckets` flat buffers,
 whose NCCL all-reduces are captured on their side stream and overlap the backward).
+With `optimizer=` (optim.FusedSGD / FusedAdamW) the graph also records the per-parameter clip norms and the update after
+the backward, so one replay is the whole training iteration; the optimizer's per-step values (lr, weight decay, bias
+corrections) are refilled from its param_groups with one more copy before each replay.
 """
 from __future__ import annotations
 
@@ -66,23 +69,42 @@ class MaskArena:
 class GraphedTrainStep:
     """loss = step(*inputs): replays  `loss = loss_fn(*static_inputs); loss.backward()`  as one CUDA graph.
 
-    loss_fn : callable taking the input tensors and returning a scalar loss (typically an nn.Module whose
-              forward computes the loss); its parameters' .grad are (re)written by every call.
-    reducer : optional ddp.GradientBuckets — the bucket all-reduces become part of the graph.
+    loss_fn   : callable taking the input tensors and returning a scalar loss (typically an nn.Module whose
+                forward computes the loss); its parameters' .grad are (re)written by every call.
+    reducer   : optional ddp.GradientBuckets — the bucket all-reduces become part of the graph.
+    optimizer : optional optim.FusedSGD / FusedAdamW — the graph also records `optimizer.step(clip_grad=clip_grad)` after
+                the backward (and after the bucket all-reduces), and a call returns `(loss, total_norm)`; total_norm is
+                None when clip_grad is None, as from step().  Its param_groups' lr / weight_decay may change between
+                calls.  Every parameter of its table must get a gradient from this step; frozen parameters
+                (requires_grad False) are never in the table.
     """
 
     def __init__(self, loss_fn: Callable, example_inputs: Sequence[torch.Tensor], reducer=None,
-                 params: Optional[Sequence[torch.nn.Parameter]] = None, warmup: int = 3):
+                 params: Optional[Sequence[torch.nn.Parameter]] = None, warmup: int = 3, optimizer=None,
+                 clip_grad: Optional[float] = None):
         self.loss_fn = loss_fn
         self.reducer = reducer
+        self.optimizer = optimizer
         dev = example_inputs[0].device
         if dev.type != 'cuda':
             raise RuntimeError('GraphedTrainStep needs CUDA tensors')
+        if optimizer is not None:
+            bad = [p for g in optimizer.param_groups for p in g['params'] if p.requires_grad and p.device != dev]
+            if bad:
+                raise RuntimeError(f'GraphedTrainStep: the optimizer has parameters on {bad[0].device}; a captured '
+                                   f'optimizer step needs them on {dev}')
         self.static_inputs = [t.clone() for t in example_inputs]
         if params is None:
             params = list(loss_fn.parameters()) if isinstance(loss_fn, torch.nn.Module) else []
         self.params = [p for p in params if p.requires_grad]
         self.arena = MaskArena(dev)
+        opt_params = None
+        if optimizer is not None:
+            opt_params = optimizer.prepare_capture(clip_grad)
+            known = {id(p) for p in self.params}
+            if any(id(p) not in known for p in opt_params):
+                raise RuntimeError('GraphedTrainStep: an optimizer parameter gets no gradient from this step (pass it in '
+                                   '`params`, or freeze it)')
 
         # warm-up and capture share one side stream: autograd's AccumulateGrad nodes are bound to the stream
         # they were created on, and a node bound to a non-capturing stream would run outside the graph
@@ -118,6 +140,10 @@ class GraphedTrainStep:
                     # their GEMM straight into the flat buckets, the rest is copied there, and completed buckets are
                     # all-reduced on the side stream while backward continues
                     grads = reducer.backward_into_buckets(self.static_loss, self.params)
+                if optimizer is not None:
+                    # after the backward; with a reducer, backward_into_buckets has already made this stream wait for
+                    # every bucket's all-reduce (GradientBuckets.finish)
+                    self.static_total_norm = optimizer.launch_captured()
         finally:
             self.arena.recording = False
             ops.set_mask_arena(None)
@@ -130,6 +156,12 @@ class GraphedTrainStep:
             self.static_grads = [g.detach() for g in grads]
             for p_, g_ in zip(self.params, self.static_grads):
                 p_.grad = g_                                             # rewritten in place by every replay
+        if optimizer is not None:
+            # the update reads the graph's own gradients: the static tensors, or the bucket views
+            by_id = {id(p): g for p, g in zip(self.params, self.static_grads)} if reducer is None else \
+                {id(p): reducer._view[p] for p in self.params}
+            optimizer.capture_ready([by_id[id(p)] for p in opt_params])
+            torch.cuda.synchronize(dev)
 
     def _zero(self, set_to_none=True):
         if self.reducer is not None:
@@ -139,6 +171,8 @@ class GraphedTrainStep:
                 p.grad = None
 
     def __call__(self, *inputs):
+        if self.optimizer is not None:
+            self.optimizer.refill()       # first: it refuses a changed parameter list before anything is issued
         for dst, src in zip(self.static_inputs, inputs):
             if dst.data_ptr() != src.data_ptr():
                 dst.copy_(src, non_blocking=True)
@@ -150,6 +184,9 @@ class GraphedTrainStep:
             for p_, g_ in zip(self.params, self.static_grads):
                 if p_.grad is not g_:
                     p_.grad = g_
+        if self.optimizer is not None:
+            self.optimizer.advance()
+            return self.static_loss, self.static_total_norm
         return self.static_loss
 
 
